@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — decode tokens/s of the quantized-decode hot path (BASELINE.json metric) on N B200s of one node.
+"""bench.py — decode tokens/s of the quantized-decode hot path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--model llama3-70b] [--impl b200|reference]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
@@ -41,7 +41,7 @@ MODELS = {
                                 n_ctx_orig=32768, rope_freq_base=1000000.0, rope_freq_scale=1.0, rms_eps=1e-6), ftype=1, name="Qwen2.5-72B Q5_K_M"),
 }
 PROMPT = 128
-METRIC = "decode tokens/sec Llama-3-70B Q4_K_M b=1 @1/2/4/8 B200; % HBM roofline"
+METRIC = "decode tokens/sec Llama-3-70B Q4_K_M b=1 @1/2/4/8 H100; % HBM roofline"
 
 
 def peaks():
@@ -49,16 +49,7 @@ def peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, STREAM-style copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
-
-
-def ncu_traffic(model_key):
-    """DRAM bytes (read + write) the GEMV launches of one token move, from the committed `ncu --set full` capture of the shipped kernel
-    (profiles/r2_gemv_traffic.json: per-launch dram__bytes_read.sum + dram__bytes_write.sum at every launch shape of the model)."""
-    p = ROOT / "profiles" / "r2_gemv_traffic.json"
-    if model_key != "llama3-70b" or not p.exists():
-        return None
-    return float(json.loads(p.read_text())["llama3-70b_q4_K_M_per_token_MB"]) * 1e6
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 def tensor_peak():
@@ -67,7 +58,7 @@ def tensor_peak():
         d = json.loads(p.read_text())
         if "bf16_tflops" in d:
             return float(d["bf16_tflops"]), "measured (MEASURED_PEAKS.json bf16_tflops: cuBLAS bf16 8192^3 burst; the prefill batch is timed alone)"
-    return 2250.0, "fallback (B200_PROFILING.md 2.25 PFLOP/s dense bf16/fp16)"
+    return 989.0, "H100 SXM data sheet (989 TFLOP/s dense fp16 at 700 W)"
 
 
 def prefill_flops(hp, T):
@@ -224,8 +215,9 @@ def cpu_reference_subprocess(model_key, steps, warmup):
 
 
 def boundary_leg(eng, cfg, hp, args, lib):
-    """e2e through the ggml-backend boundary (N=1): the model lives a second time in the plugin's backend buffers (weights copied
-    device to device from the engine's synthetic ones), the host's ggml builds the decode graph and the plugin computes it."""
+    """e2e through the ggml-backend boundary (N=1): the model moves into the plugin's backend buffers (the engine's synthetic weights,
+    staged in host memory because two resident copies of a 70B model do not fit one 80-GB GPU; the engine is released), the host's ggml
+    builds the decode graph and the plugin computes it."""
     import numpy as np
     import torch
     sys.path.insert(0, str(ROOT / "host"))
@@ -238,18 +230,29 @@ def boundary_leg(eng, cfg, hp, args, lib):
             names += [f"blk.{il}.attn_{x}.bias" for x in "qkv"]
     info = {n: eng.tensor_device(n) for n in names}
     types = {n: t for n, (p, b, t) in info.items() if n.endswith(".weight") and t not in (0,)}
-    hm = HG.HostModel(hp, types, "B200_0", has_bias=(hp["rope_mode"] == 2), has_freq_factors=False)
     class U8:   # __cuda_array_interface__ view of raw device memory: torch only moves bytes here
         def __init__(self, ptr, n):
             self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 2}
 
     dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
-    for n, (ptr, nbytes, t) in info.items():
-        dst, dbytes = hm.tensor_ptr(n)
-        assert dbytes == nbytes, (n, dbytes, nbytes)
-        torch.as_tensor(U8(dst, nbytes), device=dev).copy_(torch.as_tensor(U8(ptr, nbytes), device=dev))
-    torch.cuda.synchronize()
     nv = hp["n_vocab"]
+    # the engine's logits for a token at position 0 of an empty cache, compared below with the plugin's on the same weights
+    eng_logits = np.zeros(nv, dtype=np.float32)
+    eng.kv_clear()
+    eng.decode(token_at(1, nv), 0, eng_logits)
+    need = sum(nbytes for (_, nbytes, _) in info.values())
+    free = os.sysconf("SC_AVPHYS_PAGES") * os.sysconf("SC_PAGE_SIZE")
+    if need * 1.1 > free:
+        raise RuntimeError(f"boundary leg: {need / 1e9:.1f} GB of weights to stage in host memory, {free / 1e9:.1f} GB free")
+    staged = {n: torch.as_tensor(U8(ptr, nbytes), device=dev).cpu() for n, (ptr, nbytes, t) in info.items()}
+    eng.close()
+    hm = HG.HostModel(hp, types, "B200_0", has_bias=(hp["rope_mode"] == 2), has_freq_factors=False)
+    for n, h in staged.items():
+        dst, dbytes = hm.tensor_ptr(n)
+        assert dbytes == h.numel(), (n, dbytes, h.numel())
+        torch.as_tensor(U8(dst, dbytes), device=dev).copy_(h)
+    del staged
+    torch.cuda.synchronize()
     logits = np.zeros(nv, dtype=np.float32)
     first = PROMPT + args.warmup
     # same protocol as the engine arm: prompt tokens fill the cache (untimed), warm-up, then K timed steps; host wall clock, since
@@ -270,9 +273,7 @@ def boundary_leg(eng, cfg, hp, args, lib):
     launches = lib.c.pb200_kernel_launches() - n0
     # the two paths on the same weights: a token at position 0 of an empty cache through each (later steps sit on different histories
     # of a random-init, unit-gain 80-layer net and are not comparable; the whole-graph parity test lives in tests/test_gpu_ggml_graph.py)
-    eng_logits = np.zeros(nv, dtype=np.float32)
-    eng.kv_clear(); hm.kv_clear()
-    eng.decode(token_at(1, nv), 0, eng_logits)
+    hm.kv_clear()
     hm.decode([token_at(1, nv)], 0, logits)
     n_kv_pad = (first + args.steps + 32) // 32 * 32
     res = {"value": args.steps / dt, "unit": "tokens/s", "ms_per_step": dt / args.steps * 1e3,
@@ -289,7 +290,7 @@ def boundary_leg(eng, cfg, hp, args, lib):
 
 # ------------------------------------------------------------------------------------------------ same-box GPU comparator
 def ggml_cuda_arm(args, cfg, hp, config):
-    """--impl ggml-cuda: the reference's OWN ggml-cuda backend (unmodified, built for sm_100 by oracle/Makefile.cudaref — BASELINE.md §3
+    """--impl ggml-cuda: the reference's OWN ggml-cuda backend (unmodified, built for sm_90a by oracle/Makefile.cudaref — BASELINE.md §3
     "the existing kernel to beat") on the same box, same synthetic weights, same host graph (host/llama_graph_host.cpp), same protocol
     as the B200 arm's e2e leg: host token / position / mask in, logits out, every step.  Measurement infrastructure: none of the
     product's kernels run inside the timed region (the engine is used before it, to synthesise the weights, and is then freed)."""
@@ -317,34 +318,48 @@ def ggml_cuda_arm(args, cfg, hp, config):
     # over dequantized to f32 — same values, and the gather is not part of what is compared
     emb_ptr, emb_bytes, emb_type = info["token_embd.weight"]
     types["token_embd.weight"] = 0
-    hm = HG.HostModel(hp, types, "CUDA0", has_bias=(hp["rope_mode"] == 2), has_freq_factors=False)
 
     class U8:
         def __init__(self, ptr, n):
             self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 2}
 
-    for n, (ptr, nbytes, t) in info.items():
-        dst, dbytes = hm.tensor_ptr(n)
-        if n == "token_embd.weight":
-            assert dbytes == nv * E * 4
-            ids = torch.arange(nv, dtype=torch.int32, device=dev)
-            step_rows = 8192
-            for r0 in range(0, nv, step_rows):
-                nr = min(step_rows, nv - r0)
-                lib.check(lib.c.pb200_get_rows(emb_type, C.c_void_p(emb_ptr), C.c_int64(E), C.c_void_p(ids.data_ptr() + 4 * r0), C.c_int64(nr),
-                                               C.c_void_p(dst + r0 * E * 4), None), "get_rows")
-            torch.cuda.synchronize()
-            continue
-        assert dbytes == nbytes, (n, dbytes, nbytes)
-        torch.as_tensor(U8(dst, nbytes), device=dev).copy_(torch.as_tensor(U8(ptr, nbytes), device=dev))
-    torch.cuda.synchronize()
     eng_logits = np.zeros(nv, dtype=np.float32)
     eng.kv_clear()
     eng.decode(token_at(1, nv), 0, eng_logits)
     wbytes = eng.weight_bytes
+    # two resident copies of a 70B model do not fit one 80-GB GPU: the weights are staged in host memory and the engine is freed
+    # before the ggml-cuda buffers are allocated
+    need = sum(nbytes for (_, nbytes, _) in info.values()) + nv * E * 4
+    free = os.sysconf("SC_AVPHYS_PAGES") * os.sysconf("SC_PAGE_SIZE")
+    if need * 1.1 > free:
+        raise RuntimeError(f"ggml-cuda arm: {need / 1e9:.1f} GB of weights to stage in host memory, {free / 1e9:.1f} GB free")
+    staged = {}
+    for n, (ptr, nbytes, t) in info.items():
+        if n == "token_embd.weight":
+            emb = torch.empty(nv * E, dtype=torch.float32)
+            ids = torch.arange(nv, dtype=torch.int32, device=dev)
+            step_rows = 8192
+            rows = torch.empty(step_rows * E, dtype=torch.float32, device=dev)
+            for r0 in range(0, nv, step_rows):
+                nr = min(step_rows, nv - r0)
+                lib.check(lib.c.pb200_get_rows(emb_type, C.c_void_p(emb_ptr), C.c_int64(E), C.c_void_p(ids.data_ptr() + 4 * r0), C.c_int64(nr),
+                                               C.c_void_p(rows.data_ptr()), None), "get_rows")
+                torch.cuda.synchronize()
+                emb[r0 * E:(r0 + nr) * E].copy_(rows[:nr * E])
+            staged[n] = emb.view(torch.uint8)
+            del rows
+            continue
+        staged[n] = torch.as_tensor(U8(ptr, nbytes), device=dev).cpu()
     eng.close()
     del eng
     torch.cuda.empty_cache()
+    hm = HG.HostModel(hp, types, "CUDA0", has_bias=(hp["rope_mode"] == 2), has_freq_factors=False)
+    for n, h in staged.items():
+        dst, dbytes = hm.tensor_ptr(n)
+        assert dbytes == h.numel(), (n, dbytes, h.numel())
+        torch.as_tensor(U8(dst, dbytes), device=dev).copy_(h)
+    del staged
+    torch.cuda.synchronize()
     logits = np.zeros(nv, dtype=np.float32)
     hm.decode([token_at(1, nv)], 0, logits)
     nmse = float(np.sum((logits - eng_logits) ** 2) / max(np.sum(eng_logits ** 2), 1e-30))
@@ -366,7 +381,7 @@ def ggml_cuda_arm(args, cfg, hp, config):
     line = {"impl": "ggml-cuda", "metric": METRIC, "value": v, "unit": "tokens/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": dt / args.steps * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
             "dtype": "q8_1 activations x k-quant weights (mul_mat_vec_q), f32 accumulate", "data": "synthetic", "config": config,
-            "what": "the reference's unmodified ggml-cuda backend compiled -arch=sm_100 (oracle/Makefile.cudaref), CUDA graphs on, same box, same weights, "
+            "what": "the reference's unmodified ggml-cuda backend compiled for sm_90a (oracle/Makefile.cudaref), CUDA graphs on, same box, same weights, "
                     "same host graph and host I/O as the B200 arm's e2e leg",
             "e2e": {"value": v, "unit": "tokens/s", "h2d_bytes_per_step": 8 + n_kv_pad * 32 * 4, "d2h_bytes_per_step": nv * 4},
             "roofline": {"bound": "hbm", "achieved": wbytes * v / 1e9, "peak": hbm, "unit": "GB/s", "frac": wbytes * v / 1e9 / hbm, "peak_source": src,
@@ -405,6 +420,9 @@ def main():
                     "pipeline in 512-token micro-batches (pb200_prefill_stage, NCCL hand-off of the hidden states), e.g. config C5: "
                     "--model qwen2.5-72b --gpus 8 --pp 2048 --n-ctx 4096")
     ap.add_argument("--ncu", action="store_true", help="bracket the timed region with cudaProfilerStart/Stop (ncu --profile-from-start off)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed decode path returned in its last step (logits; at N > 1 also the greedy token) as "
+                         "DIR/<name>.npy, so that two builds can be compared output for output (the inputs are seeded)")
     args = ap.parse_args()
     PROMPT = args.prompt
     rank = int(os.environ.get("RANK", "0"))
@@ -416,7 +434,7 @@ def main():
     hp = dict(cfg["hp"], n_ctx=args.n_ctx)
     config = {"workload": f"{cfg['name']} decode b=1, synthetic random-init weights, {args.prompt}-token prompt then tg steps, n_ctx {args.n_ctx}, KV f16, FA off",
               "parallelism": "single GPU" if world == 1 else f"layer pipeline pp{world} (NCCL send/recv hand-off)",
-              "l2": "no explicit flush: every step streams the shard's weights (>> 126 MB L2) once"}
+              "l2": "no explicit flush: every step streams the shard's weights (>> 50 MB L2) once"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -450,7 +468,7 @@ def main():
     assert args.steps + args.warmup + PROMPT <= args.n_ctx, "n_ctx too small for prompt + warmup + steps"
 
     L = hp["n_layer"]
-    # uniform contiguous layer windows (prima: n_layer_window; 8 identical B200s need no ILP scheduler)
+    # uniform contiguous layer windows (prima: n_layer_window; 8 identical GPUs need no ILP scheduler)
     bounds = [round(r * L / world) for r in range(world + 1)]
     l0, l1 = bounds[rank], bounds[rank + 1]
     H = pkg.HParams(**hp)
@@ -554,6 +572,18 @@ def main():
     ms_dev, launches, clocks = timed(False, first)
     if args.ncu:
         torch.cuda.profiler.stop()
+
+    def dump_output(name, arr):
+        d = Path(args.dump_outputs)
+        d.mkdir(parents=True, exist_ok=True)
+        np.save(d / f"{name}.npy", arr)
+
+    if args.dump_outputs and rank == world - 1:
+        # the last timed step's results as a caller of the decode path receives them: n_vocab logits, and at N > 1 the device argmax
+        # that travels back to rank 0 (at N = 1 the timed path does not sample)
+        dump_output("decode_logits", logits_t.cpu().numpy().astype(np.float32))
+        if world > 1:
+            dump_output("decode_token", tok_t.cpu().numpy().astype(np.float64))
     eng.kv_clear() if False else None
     ms_e2e, _, clocks_e2e = timed(True, first)     # same positions again: the KV rows are simply rewritten
     # pipeline only: every rank times the same number of steps of its OWN stage with no communication; the difference between
@@ -714,14 +744,12 @@ def main():
         "e2e": e2e_engine,
         "gpu_launches": launches,
         "clocks": clocks, "clocks_e2e": clocks_e2e,
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": ncu_traffic(args.model),
-                     "traffic_note": "ncu dram__bytes_read.sum + dram__bytes_write.sum summed over the same launches (profiles/r2_gemv_traffic.json); algorithmic bytes are `how`",
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "kernel": "k_gemv_kquant (TMA-staged k-quant GEMV)", "peak_source": peak_src,
                      "how": f"algorithmic bytes of the {gemv_launches} GEMV launches of one token ({gemv_bytes} B = sum of ggml_nbytes of the weight "
                             f"matrices read) / their summed CUDA-event durations ({gemv_ms:.3f} ms, events on the launching stream, mean of 4 profiled steps)",
                      "whole_step": {"algorithmic_bytes_per_token": wb + kv_bytes, "achieved": (wb + kv_bytes) / (ms_step * 1e-3) / 1e9,
-                                    "frac": (wb + kv_bytes) / (ms_step * 1e-3) / 1e9 / peak,
-                                    "frac_of_8TBs_north_star": (wb + kv_bytes) / (ms_step * 1e-3) / 8e12}},
+                                    "frac": (wb + kv_bytes) / (ms_step * 1e-3) / 1e9 / peak}},
         "model_load_s": t_load,
     }
     if pp_result is not None:
@@ -767,7 +795,7 @@ def main():
                               "roofline": {"bound": "tensor", "achieved": (mm + att + head) / best / 1e12, "peak": tpeak, "unit": "TFLOP/s",
                                            "frac": (mm + att + head) / best / 1e12 / tpeak, "peak_source": tsrc,
                                            "algorithmic_flops": {"matmul": mm, "attention_causal": att, "lm_head_last_token": head},
-                                           "kernel": "k_mmq_tc (tcgen05 k-quant mat-mul); attention on CUDA cores (k_attn_prefill_tiled: K/V tiles shared by the GQA group x 4 tokens)"}}
+                                           "kernel": "k_mmq_tc (wgmma k-quant mat-mul); attention on CUDA cores (k_attn_prefill_tiled: K/V tiles shared by the GQA group x 4 tokens)"}}
         except Exception as ex:   # the extra measurement must never take the headline line down
             out["prefill"] = {"value": None, "unit": "tokens/s", "error": repr(ex)}
 
@@ -778,7 +806,7 @@ def main():
         except Exception as ex:   # the boundary leg needs host/_ggml (built where the reference tree exists); keep the engine number otherwise
             out["e2e_boundary_error"] = repr(ex)
     if world == 1 and not args.no_gpu_comparator:
-        # same-box GPU comparator: the reference's own ggml-cuda (sm_100 build) in a process of its own, after this one released the GPU memory
+        # same-box GPU comparator: the reference's own ggml-cuda (sm_90a build) in a process of its own, after this one released the GPU memory
         try:
             eng.close()
             torch.cuda.empty_cache()

@@ -12,7 +12,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 HOST = ROOT / "host"
 PLUGIN = ROOT / "prima.cpp_b200" / "libggml-b200.so"
-# same-box GPU comparator (measurement infrastructure, oracle/Makefile.cudaref): the reference's own ggml-cuda backend built for sm_100
+# same-box GPU comparator (measurement infrastructure, oracle/Makefile.cudaref): the reference's own ggml-cuda backend built for sm_90a
 CUDAREF = ROOT / "oracle" / "_ref" / "cuda" / "libggml-cuda-ref.so"
 
 
@@ -23,7 +23,8 @@ class HParams(C.Structure):
 
 
 def build() -> None:
-    if Path("/root/reference/ggml/src/ggml.c").exists():
+    # the reference tree oracle/Makefile points at (REF) must be readable by this user
+    if subprocess.call(["make", "-s", "-C", str(ROOT / "oracle"), "have-ref"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL) == 0:
         subprocess.check_call(["make", "-C", str(HOST), "-j8"], stdout=subprocess.DEVNULL)
 
 
@@ -36,13 +37,13 @@ def load(with_plugin: bool = True, with_cudaref: bool = False):
     if _libs is not None:
         return _libs
     if with_cudaref and not CUDAREF.exists():
-        raise RuntimeError(f"{CUDAREF} is missing: make -C oracle -f Makefile.cudaref (needs /root/reference)")
+        raise RuntimeError(f"{CUDAREF} is missing: make -C oracle -f Makefile.cudaref (needs the reference source tree)")
     core = HOST / "_ggml" / "libggml_host.so"
     drv = HOST / "_ggml" / "libllama_graph_host.so"
     if not core.exists() or not drv.exists():
         build()
     if not core.exists() or not drv.exists():
-        raise RuntimeError("host/_ggml is not built (needs the reference tree: run __graft_entry__.build() where /root/reference exists)")
+        raise RuntimeError("host/_ggml is not built (needs the reference tree: run __graft_entry__.build() where it is readable)")
     C.CDLL(str(core), mode=C.RTLD_GLOBAL)
     plug = None
     if with_plugin:

@@ -1,11 +1,11 @@
 /*
- * include/ggml_b200.h — the drop-in boundary: a ggml backend ("B200") that exposes the sm_100a kernels of
+ * include/ggml_b200.h — the drop-in boundary: a ggml backend ("B200") that exposes the sm_90a kernels of
  * libprima_b200.so through the reference's own plugin interface, the C structs of function pointers in
  * ggml/src/ggml-backend-impl.h:15-220 (ggml_backend_reg_i / _device_i / _i / _buffer_type_i / _buffer_i).
  *
  * It replaces ggml_backend_cuda_reg() (ggml/src/ggml-cuda.cu:3302) for the decode hot path.  src/llama.cpp discovers GPUs
  * purely through the registry (src/llama.cpp:20443-20456, 21118-21127), so registering this reg before
- * llama_load_model_from_file makes the ggml scheduler place the ops listed under supports_op on the B200 and everything else
+ * llama_load_model_from_file makes the ggml scheduler place the ops listed under supports_op on the GPU and everything else
  * on the CPU backend — no change to llama.cpp, ggml-backend.cpp or the tests (tests/test-backend-ops.cpp enumerates the
  * registry, :3765-3861).
  *

@@ -1,11 +1,11 @@
 /*
- * include/prima_b200.h — C ABI of libprima_b200.so, the B200-native (sm_100a) quantized-decode hot path of prima.cpp.
+ * include/prima_b200.h — C ABI of libprima_b200.so, the H100-native (sm_90a) quantized-decode hot path of prima.cpp.
  *
  * Plain pointers and sizes only; no torch / ggml types.  All functions return 0 on success, a cudaError_t (>0) for
  * CUDA failures or a negative PB200_E* code for argument errors; nothing throws or aborts across the ABI.
  * Device pointers are raw CUDA device addresses, `stream` is a cudaStream_t passed as void* (NULL = default stream).
  *
- * What each entry point replaces in the reference (paths under /root/reference):
+ * What each entry point replaces in the reference (paths relative to the reference source tree):
  *   pb200_mul_mat_vec*      ggml_cuda_mul_mat -> ggml_cuda_op_mul_mat_vec_q -> mul_mat_vec_q<type,1>
  *                           ggml/src/ggml-cuda.cu:1883-1948, ggml-cuda/mmvq.cu:55-202, vecdotq.cuh:357-787
  *                           (+ the per-call quantize_row_q8_1_cuda, quantize.cu:129-141); CPU semantics:
@@ -17,7 +17,7 @@
  *   pb200_attn_decode       FA-off attention chain: ggml_cuda_mul_mat_batched_cublas x2 + soft_max + cont,
  *                           ggml-cuda.cu:1737-1881; graph src/llama.cpp:10032-10165
  *   pb200_mul_mat_q         ggml_cuda_op_mul_mat_q mmq.cu:3-98 -> mul_mat_q<type,...> mmq.cuh:2583-2650 (+ quantize_mmq_q8_1_cuda
- *                           quantize.cu:143-169): the batched / prefill product, here on tcgen05 + TMEM
+ *                           quantize.cu:143-169): the batched / prefill product, here on wgmma tensor cores
  *   pb200_get_rows          ggml_cuda_op_get_rows getrows.cu (k-quant rows are unsupported there, ggml-cuda.cu:3033-3047)
  *   pb200_model_* / pb200_decode*   the per-token loop ggml_backend_cuda_graph_compute ggml-cuda.cu:2508-2778 over the
  *                           graph of build_llama / build_qwen2 (src/llama.cpp:11000-11216, 12736-12916) — one fused,

@@ -7,11 +7,11 @@
  * prima.cpp_b200/ may link, import or call it.
  *
  * Parity pin: every function here is checked (tests/test_oracle_port.py) against
- *   (1) the real reference compiled from /root/reference into oracle/_ref/ (when present), and
+ *   (1) the real reference compiled into oracle/_ref/, through its outputs recorded in tests/golden/reference_golden.npz, and
  *   (2) committed golden vectors in tests/golden/*.npz generated from that same compiled
  *       reference by tests/golden/make_golden.py.
  *
- * Each function cites the reference file:line it follows (paths relative to /root/reference).
+ * Each function cites the reference file:line it follows (paths relative to the reference source tree).
  * Written from the algorithm description; scalar form only (SIMD paths of the reference are
  * integer-identical and differ only in fp32 summation order).
  */

@@ -4,7 +4,7 @@
 // (src/llama.cpp:11000-11216, 12736-12916; helpers llm_build_norm :9772, llm_build_ffn :9804,
 // llm_build_kv_store :9673, llm_build_kqv :10032, KQ mask :10838 + llama_set_inputs :17276, KV padding
 // :4485) that is EXECUTED BY THE UNMODIFIED REFERENCE CPU ggml BACKEND (oracle/_ref/*/libggml_ref.so,
-// compiled from /root/reference/ggml/src).  libllama itself cannot be built here (needs <zmq.h>,
+// compiled from the reference's ggml/src).  libllama itself cannot be built here (needs <zmq.h>,
 // src/llama.cpp:1), so only the op sequence is restated; every kernel that runs is the reference's.
 // FA off, KV cache f16, V cache transposed — the reference defaults (common/common.h:275).
 //

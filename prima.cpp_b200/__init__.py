@@ -1,4 +1,4 @@
-"""prima.cpp_b200 — B200-native (sm_100a) quantized-decode hot path of prima.cpp behind a C ABI.
+"""prima.cpp_b200 — H100-native (sm_90a) quantized-decode hot path of prima.cpp behind a C ABI.
 
 The product is ``libprima_b200.so`` (CUDA kernels + C++ decode engine, ``include/prima_b200.h``) and
 ``libggml-b200.so`` (the same kernels behind the reference's ggml-backend vtables, ``include/ggml_b200.h``).

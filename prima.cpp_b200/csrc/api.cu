@@ -30,7 +30,7 @@ bool type_ok(int t) { return t == T_Q4_K || t == T_Q5_K || t == T_Q6_K || t == T
 
 extern "C" {
 
-const char * pb200_version(void) { return "prima.cpp_b200 0.1 (sm_100a)"; }
+const char * pb200_version(void) { return "prima.cpp_b200 0.1 (sm_90a)"; }
 
 const char * pb200_error_string(int code) {
     switch (code) {

@@ -1,4 +1,4 @@
-// prima.cpp_b200/csrc/common.cuh — shared device helpers for the sm_100a quantized-decode kernels.
+// prima.cpp_b200/csrc/common.cuh — shared device helpers for the sm_90a quantized-decode kernels.
 //
 // Wire formats are the reference's GGUF block layouts, read byte-for-byte from HBM
 // (ggml/src/ggml-common.h:173-204, 286-335).  Nothing here is copied from ggml-cuda: the kernels use a
@@ -46,7 +46,7 @@ struct ActQ {
     float * s;        // [K/32]        (Q8_1 only)
     // per-super-block strides (Q8_K mode): 0 = dense (256 B of qs, 16 bsums).  The shared-memory copy inside the GEMV uses
     // 272 B / 24 int16 so that 32 lanes reading 32 different super-blocks with 128-bit loads hit 32 different bank groups
-    // (dense 256-B strides are a 32-way bank conflict: measured 4 us per prologue, profiles/r1_persistent_timeline.txt).
+    // (dense 256-B strides are a 32-way bank conflict).
     int qs_stride;    // bytes
     int bs_stride;    // int16 elements
 };

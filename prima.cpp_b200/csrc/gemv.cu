@@ -92,7 +92,7 @@ __device__ __forceinline__ void fill_rest(const GemvParams & P, GemvSmemCtl * ct
 }
 
 // TYPE = weight type of every matrix of the launch (one dot routine in the hot loop: the three unrolled routines together are
-// ~126 KB of SASS and the instruction cache became the top stall, profiles/r2_gemv_ncu_v1.md), or 0 = mixed (q|k|v with a Q5_K / Q6_K v)
+// ~126 KB of SASS, more than the instruction cache holds), or 0 = mixed (q|k|v with a Q5_K / Q6_K v)
 template <int TYPE>
 __device__ __forceinline__ float dot_block(int type, const uint8_t * bp, const ActRegs & r) {
     if (TYPE == T_Q4_K) return dot_q4K(bp, r);

@@ -5,13 +5,13 @@
 // Numerics follow the CPU oracle instead (ggml_vec_dot_q{4,5,6}_K_q8_K, ggml-quants.c:7713-9566): the activation
 // is q8_K, every integer sub-result is exact, only the order of the final fp32 adds differs.
 //
-// B200 design (memory-bound, no tensor cores):
+// Design (memory-bound, no tensor cores):
 //   * persistent grid of TWO 256-thread CTAs per SM (<= 113 KB of shared memory and 128 registers each).  Two CTAs per SM is
 //     what lets consecutive kernels of the token overlap under programmatic dependent launch: when a CTA of launch A exits,
 //     a CTA of launch B becomes resident on that SM and streams its first weight tiles (they never depend on A) while the
 //     rest of A drains; a small kernel between two GEMVs (attention, silu-quant) runs while the next GEMV's rings fill.
-//     Round 1's single 512-thread / 227-KB CTA per SM serialised every launch boundary: 9.25 us fixed cost per launch
-//     (profiles/r1_gemv_microbench.txt) x 321 launches = 3 ms of a 10-ms token;
+//     a single 512-thread CTA per SM owning all of shared memory serialises every launch boundary instead (the next launch
+//     cannot become resident before the previous one has left);
 //   * row tiles of raw blocks stream HBM -> shared memory with cp.async.bulk (1-D TMA, SASS UBLKCP) into an nstage-deep ring
 //     (4-8 stages of ~16-24 KB chosen per launch; ~185 KB in flight per SM).  There is no producer warp: the consumer warp
 //     that finishes a stage last re-arms its mbarrier and issues the refill itself;
@@ -58,20 +58,8 @@ struct GemvMat {
 //   PRO_RMSNORM_DIST  act = q8_K( rms_norm(in0) * in1 )     llm_build_norm + quantize_row_q8_K   (in1 = norm weight)
 //   PRO_SILU_DIST     act = q8_K( silu(in0) * in1 )         llm_build_ffn LLM_FFN_SILU / LLM_FFN_PAR -> ffn_down
 //   Distributed: CTA c quantizes super-block c into `act` (HBM/L2), ONE grid barrier (all CTAs of the persistent grid are
-//   co-resident), then every CTA stages the finished vector like PRO_NONE.  No tiny kernel + launch boundary in front of the GEMV
-//   (measured chain ~9.5 us from "previous GEMV done" to "first tile consumed", profiles/r2_token_trace_v2.txt), and 1/296 of the
-//   work per CTA instead of every CTA recomputing the whole vector from L2 (round 1: ~7 us and 19 MB of L2 reads per launch).
-//   Built, measured on the B200 and REMOVED in round 2 (profiles/r2_ab_sweeps.txt, ab14-ab16):
-//   * L2 look-ahead — prefetching a launch's tiles beyond its ring, and the next launch's first weights from ring slots that have no tile
-//     left, to keep HBM busy during the dependency chain at a launch boundary: DRAM bytes unchanged (ncu), the launch that is fed from L2
-//     gains (ffn_down -4.6 us) but the prefetching launch loses more (gate|up +7 us), and the small latency-critical loads of the prologue
-//     queue behind the prefetches: 107 -> 98-105 tok/s in every setting tried (cp.async.bulk.prefetch.L2 and per-line prefetch.global.L2);
-//   * a cluster variant of the distributed prologue (4 CTAs exchange their quarter of the activation through distributed shared memory
-//     instead of the grid barrier + L2 round trip): same tokens/s, and its code cost the hot loop 4 % (109.9 -> 105.4).
-//   * a "tail task": the last CTA of wo / ffn_down to finish (atomic arrival counter) produces q8_K(rms_norm(y) * w) of the vector the
-//     launch has just written, so that the next GEMV starts with PRO_NONE instead of the distributed prologue.  Bit-identical, but the
-//     single CTA needs ~9 us for it (its loads of y and of the norm weights queue behind the next launch's ring fill, which has the HBM
-//     queues full at that moment): 110.1 -> 101.8-103.3 tok/s (profiles/r2_ab_sweeps.txt ab24 / ab25, r2_token_trace_v7).
+//   co-resident), then every CTA stages the finished vector like PRO_NONE.  No tiny kernel + launch boundary in front of the GEMV,
+//   and each CTA quantizes one super-block instead of every CTA recomputing the whole vector from L2.
 enum : int { PRO_NONE = 0, PRO_RMSNORM_DIST = 4, PRO_SILU_DIST = 5 };
 
 struct GemvParams {

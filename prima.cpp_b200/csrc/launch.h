@@ -1,4 +1,4 @@
-// prima.cpp_b200/csrc/launch.h — host-side launchers of the sm_100a kernels (internal C++ API; the public C ABI is
+// prima.cpp_b200/csrc/launch.h — host-side launchers of the sm_90a kernels (internal C++ API; the public C ABI is
 // include/prima_b200.h).  Every launcher enqueues on `stream` and returns a cudaError_t as int (0 = success).
 #pragma once
 #include <cuda_runtime.h>
@@ -112,7 +112,7 @@ int launch_soft_max(const float * x, const float * mask, float * y, int ncols, i
                     cudaStream_t stream);
 
 // get_rows on a quantized / f16 / f32 table: y[i][:] = dequant(table[ids[i]])   (getrows.cu; ggml.c get_rows_q)
-// batched k-quant mat-mul on tcgen05 (mmq.cu): dst[T][N] = X[T][K] . W[N][K]^T (+ bias[N]); ws from mmq_workspace_bytes
+// batched k-quant mat-mul on the wgmma tensor cores (mmq.cu): dst[T][N] = X[T][K] . W[N][K]^T (+ bias[N]); ws from mmq_workspace_bytes
 size_t mmq_workspace_bytes(int64_t K, int64_t T);
 bool mmq_supported(int type, int64_t K);
 struct MmqPre {            // producer fused into the activation pass: 1: x <- silu(x) * aux[t][k] (ld_aux floats per row), 2: x <- rms_norm(x, eps) * aux[k]

@@ -1,4 +1,4 @@
-// prima.cpp_b200/csrc/mmq.cu — batched (prefill) k-quant mat-mul on the 5th-generation tensor cores (tcgen05 + TMEM).
+// prima.cpp_b200/csrc/mmq.cu — batched (prefill) k-quant mat-mul on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces: ggml_cuda_op_mul_mat_q -> mul_mat_q<type,mmq_x,8,chk> (ggml-cuda/mmq.cu:3-98, mmq.cuh:2583-2650: int8 mma.sync
 // tiles with __syncthreads ping-pong) and quantize_mmq_q8_1_cuda (quantize.cu:143-169), SURVEY §8 row a-4.
@@ -12,22 +12,23 @@
 // Also the 32-element block types Q8_0 / Q5_1 (K % 64 == 0; activations quantized per 32 values like their CPU dot): Qwen2.5-72B's
 // ffn_down, whose K = 29 568 rules the k-quants out (src/llama.cpp:19516-19551).
 //
-// Work decomposition (round 2: stream-K, persistent).  A work UNIT = one 256-element K group of one output tile (128 weight rows x 1 or 2
-// token tiles of BN <= 256 columns: two accumulators = all 512 TMEM columns share every expanded weight stage when T is large enough).
-// The units of a launch, ordered tile by tile, are cut into one contiguous range per CTA (at most one CTA per SM), so every SM gets the same
-// number of 64-element MMA steps whatever N, K and T are: round 1's one-tile-per-CTA grid left 84 of 148 SMs idle on an 8192-row matrix
-// at 512 tokens and 2/3 of the last wave idle on ffn_gate/up.  A CTA walks its range segment by segment (segment = its part of one
-// tile); a segment that covers the tile's whole K stores its result, a partial one adds it into the pre-zeroed dst with fp32 atomics
-// (two or three addends per element: the order of fp32 adds is the only non-determinism, below the kernel's own fp16 rounding).
-// Inside a CTA the pipeline never drains between segments (raw-block ring, A and B stages and their barriers run on CTA-wide counters):
-//   warp 0      owns TMEM; one lane issues 4 x tcgen05.mma (M=128, N=BN, K=16, kind::f16) per step and accumulator, one commit per step
-//   warp 1      activation producer: one cp.async.bulk per step and accumulator of the pre-tiled fp16 chunk (BN x 128 B, already in the
-//               UMMA swizzle-128B image), 2-4 stages deep
-//   warps 2..17 (16 expansion warps, 4 threads per weight row) fetch their rows' raw quantized blocks (16-byte cp.async pieces, 3 K groups
+// Work decomposition (stream-K, persistent).  A work UNIT = one 256-element K group of one output tile (128 weight rows x one token
+// tile of BN <= 128 columns).  The units of a launch, ordered tile by tile, are cut into one contiguous range per CTA (at most one CTA
+// per SM), so every SM gets the same number of 64-element MMA steps whatever N, K and T are.  A CTA walks its range segment by segment
+// (segment = its part of one tile); a segment that covers the tile's whole K stores its result, a partial one adds it into the
+// pre-zeroed dst with fp32 atomics (two or three addends per element: the order of fp32 adds is the only non-determinism, below the
+// kernel's own fp16 rounding).  Inside a CTA the pipeline never drains between segments (raw-block ring, A and B stages and their
+// barriers run on CTA-wide counters):
+//   warps 0..7  two consumer warpgroups: warpgroup w issues 4 x wgmma.mma_async (M=64, N=BN, K=16, f16 in, f32 accumulators in
+//               registers) per step for weight rows [64w, 64w + 64) of the tile, keeps one step in flight, and at the end of a segment
+//               stores / adds its accumulators into dst
+//   warp 8      activation producer: one cp.async.bulk per step of the pre-tiled fp16 chunk (BN x 128 B, already in the 128-byte
+//               swizzle image wgmma reads), 2-4 stages deep
+//   warps 9..16 (8 expansion warps, 2 threads per weight row) fetch their rows' raw quantized blocks (16-byte cp.async pieces, 3 K groups
 //               deep, completion through cp.async.mbarrier.arrive) and expand 128 x 64 weights per step to fp16 straight into the swizzled A
-//               stage (generic-proxy stores + fence.proxy.async), 2 stages (4 with CTA pairs); at the end of a segment warps 2..9 read the
-//               accumulators out of TMEM (tcgen05.ld 32x32b: quadrant = warp % 4, accumulator = (warp - 2) / 4) and store / add into dst
-// CG = 2 (opt-in): the CTA pair of a cluster shares one M = 256 MMA (cta_group::2), see launch_mmq.
+//               stage (generic-proxy stores + fence.proxy.async), 2 stages
+// Registers bound the tile: 17 warps leave 96 registers per thread (five warps share one SM sub-partition's register file), and a
+// consumer thread holds BN / 2 fp32 accumulators; the epilogue therefore streams its residuals 16 columns at a time.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -41,13 +42,15 @@ namespace pb {
 
 constexpr int MMQ_BM = 128;
 constexpr int MMQ_BK = 64;
+constexpr int MMQ_BN_MAX = 128;   // token columns of a tile: 64 accumulator registers per consumer thread
 constexpr int MMQ_A_MAX = 4;      // expanded-weight stages: P.a_nst = 2 or 4 (a power of two) of 16 KB, chosen at launch from the shared-memory budget
 constexpr int MMQ_B_NST = 4;      // activation stages (L2 loads: the deep ring)
-constexpr int MMQ_DQ_WARPS = 16;  // expansion warps: 4 threads per weight row, 16 weights per thread and step (8 warps were the latency-bound bottleneck: 45 % tensor pipe)
-constexpr int MMQ_DQ_WARP0 = 2;   // warps 0,1 = MMA issuer (owns TMEM), activation producer
+constexpr int MMQ_MMA_WARPS = 8;  // two consumer warpgroups, 64 weight rows each
+constexpr int MMQ_DQ_WARPS = 8;   // expansion warps: 2 threads per weight row, 32 weights per thread and step
+constexpr int MMQ_DQ_WARP0 = MMQ_MMA_WARPS + 1;   // warp MMQ_MMA_WARPS = activation producer
 constexpr int MMQ_THREADS = (MMQ_DQ_WARP0 + MMQ_DQ_WARPS) * 32;
 constexpr int MMQ_A_BYTES = MMQ_BM * 128;   // one A stage: 128 rows x 64 fp16
-constexpr int MMQ_CTL_BYTES = 320;
+constexpr int MMQ_CTL_BYTES = 256;
 
 struct MmqParams {
     int * abort_flag;      // host-mapped, raised by the wait watchdog
@@ -58,20 +61,15 @@ struct MmqParams {
     const float * resid;   // [T][N] or null: residual added in the epilogue
     int64_t row_bytes, total_bytes;
     int nraw, b_nst, a_nst;   // ring depths chosen at launch from the shared-memory budget (a_nst: 2 or 4)
-    int nacc, ttiles;      // accumulators (token tiles) per output tile, number of token tiles
     int ngrp, rtiles;      // 256-K groups per row (the last one may be short: 32-element block types), row tiles
     int upc, total_units;  // work units per CTA (CTA c owns units [c * upc, min((c + 1) * upc, total_units)) ), units of the launch
-    int N, K, T, BN, bpb, slot;   // slot: bytes reserved per row in a raw stage (16-B aligned window around one block)
-    uint32_t tmem_cols, idesc;
+    int N, K, T, bpb, slot;   // slot: bytes reserved per row in a raw stage (16-B aligned window around one block)
 };
 
 struct MmqCtl {
     uint64_t raw_full[3], raw_empty[3];
     uint64_t a_ready[MMQ_A_MAX], b_full[MMQ_B_NST];
-    uint64_t step_done[MMQ_B_NST];   // one tcgen05.commit per step: step u arrives on step_done[u % 4]; frees A stage u % 2 and B stage u % b_nst
-    uint64_t acc_ready, acc_free;    // per segment: accumulators complete (tcgen05.commit) / read out by the 4 epilogue warps (of both CTAs of a pair)
-    uint64_t peer_ready[MMQ_B_NST];  // CTA pairs: step g's A and B stages of the peer CTA are filled (forwarded by the peer's otherwise idle warp 0)
-    uint32_t tmem_base;
+    uint64_t step_done[MMQ_B_NST];   // both consumer warpgroups arrive once step u's wgmma completed: step_done[u % 4] frees A stage u % a_nst and B stage u % b_nst
     volatile int abort;
 };
 static_assert(sizeof(MmqCtl) <= MMQ_CTL_BYTES, "ctl");
@@ -99,7 +97,7 @@ __device__ __forceinline__ bool mmq_wait_(MmqCtl * ctl, uint64_t * bar, uint32_t
         if ((++spins & 255) == 0) {
             if (ctl->abort) return false;
             if (clock64() - t0 > PB_WAIT_TIMEOUT_CYCLES) {
-                ctl->abort = 1;                                          // inline on purpose: a call in this kernel costs 7-12 registers
+                ctl->abort = 1;                                          // inline on purpose: a call costs registers the kernel does not have
                 if (abort_flag) *(volatile int *) abort_flag = 1;        // host-mapped; visible at the latest when the launch ends
                 return false;
             }
@@ -113,59 +111,64 @@ __device__ __forceinline__ void bulk_g2s_plain(void * smem_dst, const void * gsr
                  "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
 }
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-    // K-major, SWIZZLE_128B: rows of 128 B, 8-row groups 1024 B apart (cute/arch/mma_sm100_desc.hpp SmemDescriptor)
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr) {
+    // wgmma matrix descriptor, K-major, 128-byte swizzle: rows of 128 B, 8-row groups 1024 B apart (the address must be 1024-B aligned
+    // for a zero base offset; a K step of 16 fp16 inside the swizzle atom advances the start address by 32 B)
     uint64_t d = (uint64_t) ((saddr >> 4) & 0x3FFF);
     d |= (uint64_t) 1 << 16;               // leading byte offset: unused for swizzled K-major, canonical value 1
     d |= (uint64_t) (1024 >> 4) << 32;     // stride byte offset
-    d |= (uint64_t) 1 << 46;               // descriptor version (Blackwell)
-    d |= (uint64_t) 2 << 61;               // SWIZZLE_128B
+    d |= (uint64_t) 1 << 62;               // 128-byte swizzle
     return d;
 }
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] . B[N x 16]^T, both operands K-major in shared memory; accumulate == 0 overwrites D
+template <int N>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate);
+template <> __device__ __forceinline__ void wgmma_f16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %10, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// cta_group::2: the CTA pair of a cluster executes one M = 256 MMA; A rows 0-127 / 128-255 and the two halves of B's N rows come from the two
-// CTAs' shared memory at the same offsets, each CTA's TMEM receives its own 128 rows of D.  Issued by the leader CTA (rank 0) only.
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+template <> __device__ __forceinline__ void wgmma_f16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-// completion of all prior MMAs of the pair -> the barrier at this offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_cg2(uint64_t * bar) {
-    const uint16_t mask = 3;
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
+template <> __device__ __forceinline__ void wgmma_f16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ uint32_t mmq_cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void mmq_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+template <> __device__ __forceinline__ void wgmma_f16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-// arrive on the barrier at the same shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t * bar, uint32_t rank) {
-    uint32_t ra;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(bar)), "r"(rank));
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(ra) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int NPEND>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(NPEND) : "memory"); }
+// keeps the compiler from touching accumulator registers across the asynchronous wgmma (reads before its wait_group)
+__device__ __forceinline__ void reg_fence(float & r) { asm volatile("" : "+f"(r)::"memory"); }
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     __half2 h = __floats2half2_rn(a, b);
@@ -288,128 +291,118 @@ __device__ __forceinline__ void cp_async16(void * smem_dst, const void * gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
 
-template <int TYPE, int CG>
+
+template <int TYPE, int BN>
 __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant__ MmqParams P) {
     extern __shared__ uint8_t smem_raw[];
     // the swizzle-128B atoms (A and B stages) need 1024-byte alignment in the shared window
     uint8_t * smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int BN = P.BN;
-    const int b1 = BN * 128;                                     // one token tile's chunk in the activation image
-    const int b1c = b1 / CG;                                     // this CTA's part of it: BN / CG token rows (a pair splits B's N rows)
-    const int b_bytes = P.nacc * b1c;                            // one B stage
-    const uint32_t rank = CG == 2 ? mmq_cluster_rank() : 0u;     // CTA pairs: rank 0 leads (issues the MMAs), rank 1 expands the tile's other 128 rows
-    uint8_t * a_st = smem;                                       // [A_NST][16 KB]
-    uint8_t * b_st = a_st + P.a_nst * MMQ_A_BYTES;               // [b_nst][nacc][BN/CG*128]
+    constexpr int b1 = BN * 128;                                 // one step of a token tile in the activation image = one B stage
+    uint8_t * a_st = smem;                                       // [a_nst][16 KB]
+    uint8_t * b_st = a_st + P.a_nst * MMQ_A_BYTES;               // [b_nst][BN * 128]
     const int amask = P.a_nst - 1, ashift = P.a_nst == 4 ? 2 : 1;
-    uint8_t * raw = b_st + P.b_nst * b_bytes;                    // [nraw][128 * slot]
+    uint8_t * raw = b_st + P.b_nst * b1;                         // [nraw][128 * slot]
     MmqCtl * ctl = reinterpret_cast<MmqCtl *>(raw + P.nraw * MMQ_BM * P.slot);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nstep_all = P.K / MMQ_BK;                          // 64-element steps of a whole row; group sb holds steps [4 sb, min(4 sb + 4, nstep_all))
-    const int w0 = (int) (blockIdx.x / CG) * P.upc, w1 = min(w0 + P.upc, P.total_units);   // this CTA's (pair's) units
+    const int w0 = (int) blockIdx.x * P.upc, w1 = min(w0 + P.upc, P.total_units);   // this CTA's units
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < 3; i++) { mbar_init(&ctl->raw_full[i], MMQ_DQ_WARPS * 32); mbar_init(&ctl->raw_empty[i], MMQ_DQ_WARPS); }
         for (int i = 0; i < MMQ_A_MAX; i++) mbar_init(&ctl->a_ready[i], MMQ_DQ_WARPS);
-        for (int i = 0; i < MMQ_B_NST; i++) { mbar_init(&ctl->b_full[i], 1); mbar_init(&ctl->step_done[i], 1); }
-        mbar_init(&ctl->acc_ready, 1);
-        mbar_init(&ctl->acc_free, 8 * CG);
-        for (int i = 0; i < MMQ_B_NST; i++) mbar_init(&ctl->peer_ready[i], 1);
+        for (int i = 0; i < MMQ_B_NST; i++) { mbar_init(&ctl->b_full[i], 1); mbar_init(&ctl->step_done[i], MMQ_MMA_WARPS / 4); }
         ctl->abort = 0;
         mbar_fence_init();
     }
-    if (warp == 0) {
-        if (CG == 2) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&ctl->tmem_base)), "r"(P.tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&ctl->tmem_base)), "r"(P.tmem_cols) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tc_fence_before();
     __syncthreads();
-    if (CG == 2) mmq_cluster_sync();   // both CTAs' barriers are initialised before anything arrives on them from the other CTA
-    tc_fence_after();
-    const uint32_t tmem = *(volatile uint32_t *) &ctl->tmem_base;
 
-    // Every role walks the same segments: unit w -> tile w / ngrp (token-tile group tile / rtiles, row tile tile % rtiles), K group w % ngrp.
-    if (warp == 0 && rank != 0) {
-        // ================= peer CTA of a pair: tell the leader when this CTA's stages of step g are filled =================
-        if (lane == 0) {
-            int g = 0;
-            bool ok = true;
-            for (int w = w0; w < w1 && ok;) {
-                const int tile = w / P.ngrp, sbb = w - tile * P.ngrp, sbe = min(P.ngrp, sbb + (w1 - w));
-                const int nsteps = min(4 * sbe, nstep_all) - 4 * sbb;
-                for (int u = 0; u < nsteps; u++, g++) {
-                    if (!mmq_wait(ctl, &ctl->b_full[g % P.b_nst], (g / P.b_nst) & 1)) { ok = false; break; }
-                    if (!mmq_wait(ctl, &ctl->a_ready[g & amask], (g >> ashift) & 1)) { ok = false; break; }
-                    mbar_arrive_cluster(&ctl->peer_ready[g % MMQ_B_NST], 0);
-                }
-                w += sbe - sbb;
-            }
-        }
-        __syncwarp();
-    } else if (warp == 0) {
-        // ================= MMA issuer =================
-        if (lane == 0) {
-            int g = 0, seg = 0;                                  // CTA-wide step and segment counters (barrier phases follow them)
-            bool ok = true;
-            for (int w = w0; w < w1 && ok; seg++) {
-                const int tile = w / P.ngrp, sbb = w - tile * P.ngrp, sbe = min(P.ngrp, sbb + (w1 - w));
-                const int nacc = min(P.nacc, P.ttiles - (tile / P.rtiles) * P.nacc);
-                const int nsteps = min(4 * sbe, nstep_all) - 4 * sbb;
-                if (seg > 0 && !mmq_wait(ctl, &ctl->acc_free, (seg - 1) & 1)) break;   // the previous segment's accumulators have been read out
-                tc_fence_after();
-                for (int u = 0; u < nsteps; u++, g++) {
-                    const int sa = g & amask, sb = g % P.b_nst;
-                    if (!mmq_wait(ctl, &ctl->b_full[sb], (g / P.b_nst) & 1)) { ok = false; break; }
-                    if (!mmq_wait(ctl, &ctl->a_ready[sa], (g >> ashift) & 1)) { ok = false; break; }
-                    if (CG == 2 && !mmq_wait(ctl, &ctl->peer_ready[g % MMQ_B_NST], (g / MMQ_B_NST) & 1)) { ok = false; break; }
-                    tc_fence_after();
-                    const uint64_t da = umma_desc_sw128(smem_u32(a_st + (size_t) sa * MMQ_A_BYTES));
-                    const uint64_t db = umma_desc_sw128(smem_u32(b_st + (size_t) sb * b_bytes));
-                    const uint64_t db2 = umma_desc_sw128(smem_u32(b_st + (size_t) sb * b_bytes + b1c));
+    // Every role walks the same segments: unit w -> tile w / ngrp (token tile tile / rtiles, row tile tile % rtiles), K group w % ngrp.
+    if (warp < MMQ_MMA_WARPS) {
+        // ================= consumers: warpgroup wg multiplies weight rows [64 wg, 64 wg + 64) of the tile =================
+        const int wg = warp >> 2;
+        const bool leader = (threadIdx.x & 127) == 0;
+        float acc[BN / 2];
+        int g = 0;                                               // CTA-wide step counter (barrier phases follow it)
+        bool ok = true;
+        for (int w = w0; w < w1 && ok;) {
+            const int tile = w / P.ngrp, sbb = w - tile * P.ngrp, sbe = min(P.ngrp, sbb + (w1 - w));
+            const int nsteps = min(4 * sbe, nstep_all) - 4 * sbb;
+            for (int u = 0; u < nsteps; u++, g++) {
+                const int sa = g & amask, sb = g % P.b_nst;
+                if (!mmq_wait(ctl, &ctl->b_full[sb], (g / P.b_nst) & 1)) { ok = false; break; }
+                if (!mmq_wait(ctl, &ctl->a_ready[sa], (g >> ashift) & 1)) { ok = false; break; }
+                const uint64_t da = gmma_desc_sw128(smem_u32(a_st + (size_t) sa * MMQ_A_BYTES + wg * (MMQ_A_BYTES / 2)));
+                const uint64_t db = gmma_desc_sw128(smem_u32(b_st + (size_t) sb * b1));
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < MMQ_BK / 16; k++) {
-                        if (CG == 2) {
-                            umma_f16_cg2(tmem, da + 2 * k, db + 2 * k, P.idesc, (u | k) != 0);
-                            if (nacc == 2) umma_f16_cg2(tmem + 256, da + 2 * k, db2 + 2 * k, P.idesc, (u | k) != 0);
-                        } else {
-                            umma_f16(tmem, da + 2 * k, db + 2 * k, P.idesc, (u | k) != 0);
-                            if (nacc == 2) umma_f16(tmem + 256, da + 2 * k, db2 + 2 * k, P.idesc, (u | k) != 0);
-                        }
-                    }
-                    if (CG == 2) umma_commit_cg2(&ctl->step_done[g % MMQ_B_NST]); else umma_commit(&ctl->step_done[g % MMQ_B_NST]);
-                }
-                if (CG == 2) umma_commit_cg2(&ctl->acc_ready); else umma_commit(&ctl->acc_ready);
-                w += sbe - sbb;
+                for (int k = 0; k < MMQ_BK / 16; k++) wgmma_f16<BN>(acc, da + 2 * k, db + 2 * k, (u | k) != 0);
+                wgmma_commit();
+                wgmma_wait<1>();                                 // step g - 1 has read its stages
+                if (u > 0 && leader) mbar_arrive(&ctl->step_done[(g - 1) % MMQ_B_NST]);
             }
+            wgmma_wait<0>();
+#pragma unroll
+            for (int i = 0; i < BN / 2; i++) reg_fence(acc[i]);
+            if (!ok) break;
+            if (leader) mbar_arrive(&ctl->step_done[(g - 1) % MMQ_B_NST]);
+            // ================= epilogue of the segment, straight from the accumulator registers =================
+            // wgmma's D fragment: acc[4 j + 2 i + e] = D[16 (warp % 4) + lane / 4 + 8 i][8 j + 2 (lane % 4) + e]
+            const int t0 = (tile / P.rtiles) * BN + 2 * (lane & 3);
+            const int nrow = (tile % P.rtiles) * MMQ_BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+            const bool first = sbb == 0, whole = first && sbe == P.ngrp;   // bias / residual ride on the K group 0 segment
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+                const int n = nrow + 8 * i;
+                if (n >= P.N) continue;
+                const float bias = (P.bias && first) ? P.bias[n] : 0.f;
+                const float * __restrict__ rp = (P.resid && first) ? P.resid + n : nullptr;
+                // a chunk's residuals are loaded before its stores: written as "load, add, store" per element the loads would serialise
+                // behind the stores / atomics (dst and resid may alias as far as the compiler knows)
+                constexpr int JC = 2;
+#pragma unroll
+                for (int j0 = 0; j0 < BN / 8; j0 += JC) {
+                    float rv[2 * JC];
+#pragma unroll
+                    for (int j = 0; j < JC; j++)
+#pragma unroll
+                        for (int e = 0; e < 2; e++) {
+                            const int t = t0 + 8 * (j0 + j) + e;
+                            rv[2 * j + e] = (rp && t < P.T) ? __ldg(rp + (size_t) t * P.N) : 0.f;
+                        }
+#pragma unroll
+                    for (int j = 0; j < JC; j++)
+#pragma unroll
+                        for (int e = 0; e < 2; e++) {
+                            const int t = t0 + 8 * (j0 + j) + e;
+                            if (t < P.T) {
+                                const float y = __fadd_rn(__fadd_rn(acc[4 * (j0 + j) + 2 * i + e], bias), rv[2 * j + e]);
+                                if (whole) P.dst[(size_t) t * P.N + n] = y;
+                                else atomicAdd(&P.dst[(size_t) t * P.N + n], y);   // <= 3 addends onto 0
+                            }
+                        }
+                }
+            }
+            w += sbe - sbb;
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ================= activation producer: runs up to b_nst steps ahead of the tensor core =================
+    } else if (warp == MMQ_MMA_WARPS) {
+        // ================= activation producer: runs up to b_nst steps ahead of the tensor cores =================
         if (lane == 0) {
             const size_t tile_stride = (size_t) nstep_all * b1;
             int g = 0;
             bool ok = true;
             for (int w = w0; w < w1 && ok;) {
                 const int tile = w / P.ngrp, sbb = w - tile * P.ngrp, sbe = min(P.ngrp, sbb + (w1 - w));
-                const int tt0 = (tile / P.rtiles) * P.nacc;
-                const int nacc = min(P.nacc, P.ttiles - tt0);
                 const int nsteps = min(4 * sbe, nstep_all) - 4 * sbb;
-                const uint8_t * Bt = P.B + (size_t) tt0 * tile_stride + (size_t) sbb * 4 * b1 + (size_t) rank * b1c;
+                const uint8_t * Bt = P.B + (size_t) (tile / P.rtiles) * tile_stride + (size_t) sbb * 4 * b1;
                 for (int u = 0; u < nsteps; u++, g++) {
                     const int sb = g % P.b_nst;
                     if (g >= P.b_nst) {   // step g - b_nst consumed this stage
                         const int f = g - P.b_nst;
                         if (!mmq_wait(ctl, &ctl->step_done[f % MMQ_B_NST], (f / MMQ_B_NST) & 1)) { ok = false; break; }
                     }
-                    mbar_arrive_expect_tx(&ctl->b_full[sb], (uint32_t) (nacc * b1c));
-                    for (int a = 0; a < nacc; a++)
-                        bulk_g2s_plain(b_st + (size_t) sb * b_bytes + (size_t) a * b1c, Bt + (size_t) a * tile_stride + (size_t) u * b1, (uint32_t) b1c,
-                                       &ctl->b_full[sb]);
+                    mbar_arrive_expect_tx(&ctl->b_full[sb], (uint32_t) b1);
+                    bulk_g2s_plain(b_st + (size_t) sb * b1, Bt + (size_t) u * b1, (uint32_t) b1, &ctl->b_full[sb]);
                 }
                 w += sbe - sbb;
             }
@@ -417,18 +410,18 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
         __syncwarp();
     } else {
         // ================= weight expansion =================
-        const int dt = threadIdx.x - MMQ_DQ_WARP0 * 32;        // 0..511
-        const int r = dt >> 2, h = (dt >> 1) & 1, hh = dt & 1;
+        const int dt = threadIdx.x - MMQ_DQ_WARP0 * 32;        // 0..255
+        const int r = dt >> 1, h = dt & 1;
         bool ok = true;
         // this thread fetches its own half of the row's block: 16-byte cp.async pieces of the 16-B aligned window around it
         const int64_t lim = (P.total_bytes + 15) & ~(int64_t) 15;
-        const int cpr = P.slot >> 4, p_lo = cpr * (dt & 3) / 4, p_hi = cpr * ((dt & 3) + 1) / 4;   // this thread's quarter of the row's window
+        const int cpr = P.slot >> 4, p_lo = cpr * h / 2, p_hi = cpr * (h + 1) / 2;
         const int nx = w1 - w0;                                 // groups this CTA walks, x = 0 .. nx-1 across its segments
         // fetch cursor: the group nraw-1 ahead of the one being expanded (tile / K group tracked incrementally: no divisions in the loop)
         int f_x = 0, f_sb, f_rt;
         { const int tile = w0 / P.ngrp; f_sb = w0 - tile * P.ngrp; f_rt = tile % P.rtiles; }
         auto fetch_next = [&](int slot) {                       // issues group f_x of this CTA into raw slot `slot`, advances the cursor
-            const int gr = min((f_rt * CG + (int) rank) * MMQ_BM + r, P.N - 1);
+            const int gr = min(f_rt * MMQ_BM + r, P.N - 1);
             const int64_t src0 = ((int64_t) gr * P.row_bytes + (int64_t) f_sb * P.bpb) & ~(int64_t) 15;
             uint8_t * dst0 = raw + ((size_t) slot * MMQ_BM + r) * P.slot;
             for (int pc = p_lo; pc < p_hi; pc++)
@@ -438,16 +431,17 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
             if (++f_sb == P.ngrp) { f_sb = 0; if (++f_rt == P.rtiles) f_rt = 0; }
         };
         for (int i = 0; i < P.nraw - 1 && i < nx; i++) fetch_next(i);
-        // the four 16-byte pieces this thread writes per step, already swizzled
+        // the four 16-byte pieces (K elements 32h + 8q .. + 8, q = 0..3) this thread writes per step, already swizzled
         const uint32_t arow = r * 128;
-        const uint32_t o0 = arow + (((4 * h + 2 * hh + 0) ^ (r & 7)) << 4), o1 = arow + (((4 * h + 2 * hh + 1) ^ (r & 7)) << 4);
-        int g = 0, seg = 0;
+        uint32_t o[4];
+#pragma unroll
+        for (int q = 0; q < 4; q++) o[q] = arow + (((4 * h + q) ^ (r & 7)) << 4);
+        int g = 0;
         int rs = 0, rph = 0;                                    // raw slot / phase of the group being expanded
         int prs = P.nraw - 1, pph = 1;                          // ... of the group before it (the slot the next fetch goes into)
-        for (int w = w0; w < w1 && ok; seg++) {
+        for (int w = w0; w < w1 && ok;) {
             const int tile = w / P.ngrp, sbb = w - tile * P.ngrp, sbe = min(P.ngrp, sbb + (w1 - w));
-            const int row0 = ((tile % P.rtiles) * CG + (int) rank) * MMQ_BM;
-            const int gr = min(row0 + r, P.N - 1);
+            const int gr = min((tile % P.rtiles) * MMQ_BM + r, P.N - 1);
             for (int sb = sbb; sb < sbe && ok; sb++) {
                 // refill the slot the previous group used, once every expansion warp has left it
                 if (f_x < nx) {
@@ -461,16 +455,20 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
 #pragma unroll
                 for (int c = 0; c < 4; c++) {
                     if (c >= nst) break;
-                    uint32_t v[8];
-                    expand<TYPE>(blk, c, h, hh, v);
+                    uint32_t v[2][8];
+                    expand<TYPE>(blk, c, h, 0, v[0]);
+                    expand<TYPE>(blk, c, h, 1, v[1]);
                     if (g >= P.a_nst) {     // step g - a_nst has consumed this A stage
                         const int f = g - P.a_nst;
                         if (!mmq_wait(ctl, &ctl->step_done[f % MMQ_B_NST], (f / MMQ_B_NST) & 1)) { ok = false; break; }
                     }
                     uint8_t * as = a_st + (size_t) (g & amask) * MMQ_A_BYTES;
-                    *reinterpret_cast<uint4 *>(as + o0) = make_uint4(v[0], v[1], v[2], v[3]);
-                    *reinterpret_cast<uint4 *>(as + o1) = make_uint4(v[4], v[5], v[6], v[7]);
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core's async proxy
+#pragma unroll
+                    for (int hh = 0; hh < 2; hh++) {
+                        *reinterpret_cast<uint4 *>(as + o[2 * hh]) = make_uint4(v[hh][0], v[hh][1], v[hh][2], v[hh][3]);
+                        *reinterpret_cast<uint4 *>(as + o[2 * hh + 1]) = make_uint4(v[hh][4], v[hh][5], v[hh][6], v[hh][7]);
+                    }
+                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma's async proxy
                     __syncwarp();
                     if (lane == 0) mbar_arrive(&ctl->a_ready[g & amask]);
                     g++;
@@ -480,86 +478,12 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
                 prs = rs; pph = rph;
                 if (++rs == P.nraw) { rs = 0; rph ^= 1; }
             }
-            // ================= epilogue of the segment: four consecutive warps cover the four 32-lane quadrants of TMEM =================
-            if (warp < MMQ_DQ_WARP0 + 8) {
-                // 8 epilogue warps: quadrant warp % 4 of the TMEM lanes (a warp may only read its own quadrant), accumulator (warp - 2) / 4
-                const int ehalf = (warp - MMQ_DQ_WARP0) >> 2;
-                const bool acc_ok = ok && mmq_wait(ctl, &ctl->acc_ready, seg & 1);
-                tc_fence_after();
-                const int tt0 = (tile / P.rtiles) * P.nacc;
-                const int nacc = min(P.nacc, P.ttiles - tt0);
-                const bool first = sbb == 0, whole = first && sbe == P.ngrp;   // bias / residual ride on the K group 0 segment
-                const int quad = warp & 3;
-                const int n = row0 + quad * 32 + lane;
-                const float bias = (P.bias && n < P.N && first) ? P.bias[n] : 0.f;
-                // The residual rows are fetched one 16-token chunk AHEAD, all 16 loads in flight at once: written as "load, add, store" per
-                // element the loads serialise behind the stores / atomics (dst and resid may alias as far as the compiler knows), which cost
-                // 220-260 us per launch with a residual (wo, ffn_down: profiles/r2_prefill_launches_streamk_before_resid_fix.csv)
-                const float * __restrict__ rp = (P.resid && first && n < P.N) ? P.resid + n : nullptr;
-                float rcur[16], rnext[16];
-                auto load_resid = [&](float (&rv)[16], int a, int c0) {
-#pragma unroll
-                    for (int i = 0; i < 16; i++) {
-                        const int t = (tt0 + a) * BN + c0 + i;
-                        rv[i] = (rp && t < P.T) ? __ldg(rp + (size_t) t * P.N) : 0.f;
-                    }
-                };
-                // two accumulators: one per warp group; one accumulator: its column halves (when they split into whole 16-column chunks)
-                const bool csplit = nacc == 1 && BN % 32 == 0;
-                const int a_lo = nacc == 2 ? ehalf : 0, a_hi = nacc == 2 ? ehalf + 1 : ((csplit || ehalf == 0) ? 1 : 0);
-                const int c_lo = csplit ? ehalf * (BN / 2) : 0, c_hi = csplit ? c_lo + BN / 2 : BN;
-                if (a_lo < a_hi) load_resid(rcur, a_lo, c_lo);
-                for (int a = a_lo; a < a_hi; a++) {
-                    for (int c0 = c_lo; c0 < c_hi; c0 += 16) {
-                        {   // next chunk's residual
-                            int a2 = a, c2 = c0 + 16;
-                            if (c2 >= c_hi) { a2++; c2 = c_lo; }
-                            if (a2 < a_hi) load_resid(rnext, a2, c2);
-                        }
-                        uint32_t v[16];
-                        const uint32_t taddr = tmem + ((uint32_t) (quad * 32) << 16) + (uint32_t) (a * 256 + c0);
-                        asm volatile(
-                            "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-                            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-                              "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-                            : "r"(taddr)
-                            : "memory");
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                        if (acc_ok && n < P.N) {
-#pragma unroll
-                            for (int i = 0; i < 16; i++) {
-                                const int t = (tt0 + a) * BN + c0 + i;
-                                if (t < P.T) {
-                                    const float y = __fadd_rn(__fadd_rn(__uint_as_float(v[i]), bias), rcur[i]);
-                                    if (whole) P.dst[(size_t) t * P.N + n] = y;
-                                    else atomicAdd(&P.dst[(size_t) t * P.N + n], y);   // <= 3 addends onto 0
-                                }
-                            }
-                        }
-#pragma unroll
-                        for (int i = 0; i < 16; i++) rcur[i] = rnext[i];
-                    }
-                }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {                                 // the issuer (of the leader CTA) may overwrite the accumulators
-                    if (CG == 2) mbar_arrive_cluster(&ctl->acc_free, 0); else mbar_arrive(&ctl->acc_free);
-                }
-            }
             w += sbe - sbb;
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (CG == 2) mmq_cluster_sync();   // the pair leaves together: the leader's MMAs and commits reach into the peer's shared memory
-    if (warp == 0) {
-        tc_fence_after();
-        if (CG == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(P.tmem_cols) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(P.tmem_cols) : "memory");
-    }
 }
 
-// ---- activation rows -> q8_K (exactly as the CPU backend quantizes them) -> fp16, written in the tiled UMMA image ----
+// ---- activation rows -> q8_K (exactly as the CPU backend quantizes them) -> fp16, written in the tiled 128-byte-swizzle image wgmma reads ----
 // blk32: the weight type is Q8_0 / Q5_1, whose CPU dot quantizes the activation per 32 values (q8_0 / q8_1: d = amax / 127 stored
 // as f16, q = round-half-even(x * 127 / amax), quantize_row_q8_0 ggml-quants.c:943-1010) instead of per 256 (q8_K).
 // Fused producers of the activation (pre_kind): 1 = silu(x) * aux[t][k] (llm_build_ffn's SILU + MUL in front of ffn_down, the f32 product never
@@ -658,10 +582,11 @@ __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, 
     }
 }
 
-static int mmq_pick_bn(int T) {
-    if (T >= 256) return 256;
-    int bn = (T + 15) / 16 * 16;
-    return bn < 16 ? 16 : bn;
+
+static int mmq_pick_bn(int T) {   // a power of two: one kernel instance per width
+    int bn = 16;
+    while (bn < T && bn < MMQ_BN_MAX) bn <<= 1;
+    return bn;
 }
 size_t mmq_workspace_bytes(int64_t K, int64_t T) {
     const int BN = mmq_pick_bn((int) T);
@@ -673,26 +598,22 @@ bool mmq_supported(int type, int64_t K) {
     return (type == T_Q8_0 || type == T_Q5_1) && K % 64 == 0 && K >= 256;   // 32-element blocks: two per 64-element step
 }
 
-template <int TYPE, int CG>
-static cudaError_t mmq_launch_typed2(const MmqParams & P, dim3 grid, size_t smem, cudaStream_t st) {
+template <int TYPE, int BN>
+static cudaError_t mmq_launch_bn(const MmqParams & P, dim3 grid, size_t smem, cudaStream_t st) {
     static FuncAttrCache attr_cache;
-    cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_mmq_tc<TYPE, CG>, smem, false);
+    cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_mmq_tc<TYPE, BN>, smem, false);
     if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(MMQ_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = CG > 1 ? 1 : 0;
-    return cudaLaunchKernelEx(&cfg, k_mmq_tc<TYPE, CG>, P);
+    k_mmq_tc<TYPE, BN><<<grid, MMQ_THREADS, smem, st>>>(P);
+    return cudaGetLastError();
 }
 template <int TYPE>
-static cudaError_t mmq_launch_typed(const MmqParams & P, int cg, dim3 grid, size_t smem, cudaStream_t st) {
-    return cg == 2 ? mmq_launch_typed2<TYPE, 2>(P, grid, smem, st) : mmq_launch_typed2<TYPE, 1>(P, grid, smem, st);
+static cudaError_t mmq_launch_typed(const MmqParams & P, int bn, dim3 grid, size_t smem, cudaStream_t st) {
+    switch (bn) {
+        case 16: return mmq_launch_bn<TYPE, 16>(P, grid, smem, st);
+        case 32: return mmq_launch_bn<TYPE, 32>(P, grid, smem, st);
+        case 64: return mmq_launch_bn<TYPE, 64>(P, grid, smem, st);
+        default: return mmq_launch_bn<TYPE, 128>(P, grid, smem, st);
+    }
 }
 
 cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const float * x, int64_t ldx, int64_t T, float * dst, const float * bias,
@@ -714,34 +635,20 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
     P.N = (int) N;
     P.K = (int) K;
     P.T = (int) T;
-    P.BN = BN;
     // bytes of one 256-K group of a row, and the 16-byte aligned window reserved for it (Q6_K and Q8_0 rows are not 16-B aligned)
     P.bpb = type == T_Q4_K ? BYTES_Q4_K : type == T_Q5_K ? BYTES_Q5_K : type == T_Q6_K ? BYTES_Q6_K : type == T_Q8_0 ? 8 * BYTES_Q8_0 : 8 * BYTES_Q5_1;
     P.slot = type == T_Q6_K ? 240 : (type == T_Q8_0 ? 288 : P.bpb);
-    P.ttiles = tpad / BN;
-    // CTA pairs (tcgen05 cta_group::2, PB200_MMQ_CG=2): two row tiles form one M = 256 MMA, each CTA stages only half of the activation tile
-    // (L2 -> SM traffic halves, room for 4 expanded-weight stages).  Built and measured: parity green, but 5-7 % SLOWER than one CTA per
-    // MMA at every shape (profiles/r2_mmq_probe.txt) — neither the activation ring nor the weight-stage depth was the limiter, the
-    // weight-expansion warps were (8 -> 16 warps: +19 %).  The single-CTA form is the default.
-    static const int force_cg = getenv("PB200_MMQ_CG") ? atoi(getenv("PB200_MMQ_CG")) : 0;
-    const int rt1 = (int) ((N + MMQ_BM - 1) / MMQ_BM);
-    const int cg = (force_cg == 2 && rt1 >= 2 && BN % 32 == 0) ? 2 : 1;
-    P.rtiles = (rt1 + cg - 1) / cg;            // row-tile groups (pairs)
-    // two accumulators per output tile halve the weight-expansion work per FLOP (measured 1040 vs 590 TFLOP/s at full occupancy)
-    static const int force_nacc = getenv("PB200_MMQ_NACC") ? atoi(getenv("PB200_MMQ_NACC")) : 0;
-    P.nacc = (P.ttiles >= 2 && force_nacc != 1) ? 2 : 1;
-    // ... if the shared-memory budget allows it: Q8_0's 288-byte raw slots leave no room for two 64-KB activation stages
-    if (P.nacc == 2 && 1024 + (size_t) 2 * MMQ_A_BYTES + (size_t) 2 * 2 * (BN / cg) * 128 + (size_t) 2 * MMQ_BM * P.slot + MMQ_CTL_BYTES > 232448) P.nacc = 1;
-    const int tgroups = (P.ttiles + P.nacc - 1) / P.nacc;
+    P.rtiles = (int) ((N + MMQ_BM - 1) / MMQ_BM);
+    const int ttiles = tpad / BN;
     P.ngrp = (int) ((K / MMQ_BK + 3) / 4);
     // stream-K: the tiles' K groups, tile after tile, in equal contiguous shares; a share is at least MMQ_MIN_UNITS groups (a segment's
-    // pipeline fill + 128 x 512 epilogue must stay small against its MMA steps) unless the whole launch is smaller than that
+    // pipeline fill + epilogue must stay small against its MMA steps) unless the whole launch is smaller than that
     static const int min_units = getenv("PB200_MMQ_MIN_UNITS") ? std::max(1, atoi(getenv("PB200_MMQ_MIN_UNITS"))) : 8;
-    static const bool whole_tiles = getenv("PB200_MMQ_WHOLE_TILES") != nullptr;   // A/B: round 1's one tile per CTA (no split, no atomics)
-    const int64_t total = (int64_t) P.rtiles * tgroups * P.ngrp;
+    static const bool whole_tiles = getenv("PB200_MMQ_WHOLE_TILES") != nullptr;   // A/B: one tile per CTA (no split, no atomics)
+    const int64_t total = (int64_t) P.rtiles * ttiles * P.ngrp;
     if (total > 0x7fffffff) return cudaErrorInvalidValue;
     P.total_units = (int) total;
-    const int nsm = sm_count() / cg;           // CTAs (pairs) that can be resident: one CTA per SM
+    const int nsm = sm_count();                // CTAs that can be resident: one CTA per SM
     int upc = (int) ((total + nsm - 1) / nsm);
     upc = std::max(upc, std::min(min_units, P.ngrp));
     if (whole_tiles) upc = P.ngrp;
@@ -758,19 +665,12 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
         cudaError_t e0 = cudaMemsetAsync(dst, 0, (size_t) T * (size_t) N * sizeof(float), st);
         if (e0 != cudaSuccess) return e0;
     }
-    uint32_t cols = 32;
-    while ((int) cols < BN) cols <<= 1;
-    P.tmem_cols = P.nacc == 2 ? 512 : cols;
-    // kind::f16 instruction descriptor (cute/arch/mma_sm100_desc.hpp InstrDescriptor): D=f32, A=B=f16, both K-major, N>>3, M>>4
-    P.idesc = (1u << 4) | ((uint32_t) (BN >> 3) << 17) | ((uint32_t) ((MMQ_BM * cg) >> 4) << 24);
-    // ring depths: 3 raw super-block slots (HBM latency) if they fit, and as many activation stages (2..4) as the 227 KB budget leaves
     auto smem_for = [&](int nraw, int b_nst) {
-        return 1024 + (size_t) P.a_nst * MMQ_A_BYTES + (size_t) b_nst * P.nacc * (BN / cg) * 128 + (size_t) nraw * MMQ_BM * P.slot + MMQ_CTL_BYTES;
+        return 1024 + (size_t) P.a_nst * MMQ_A_BYTES + (size_t) b_nst * BN * 128 + (size_t) nraw * MMQ_BM * P.slot + MMQ_CTL_BYTES;
     };
-    // 4 expanded-weight stages when a CTA pair halves the activation stages (the handshake "MMA done -> store the next tile -> MMA" then
-    // has three MMA steps of slack instead of one), else 2; 3 raw slots if they fit; then as many activation stages (2..4) as are left
+    // 2 expanded-weight stages (4 on request), 3 raw slots if they fit, then as many activation stages (2..4) as the 227 KB budget leaves
     static const int force_a = getenv("PB200_MMQ_A_NST") ? atoi(getenv("PB200_MMQ_A_NST")) : 0;
-    P.a_nst = force_a == 2 || force_a == 4 ? force_a : (cg == 2 ? 4 : 2);
+    P.a_nst = force_a == 4 ? 4 : 2;
     P.nraw = 3;
     if (smem_for(3, 2) > 232448) P.nraw = 2;
     if (smem_for(P.nraw, 2) > 232448) P.a_nst = 2;
@@ -778,12 +678,12 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
     while (P.b_nst > 2 && smem_for(P.nraw, P.b_nst) > 232448) P.b_nst--;
     const size_t smem = smem_for(P.nraw, P.b_nst);
     if (smem > 232448) return cudaErrorInvalidConfiguration;
-    dim3 grid((unsigned) (grid_x * cg), 1, 1);
-    if (type == T_Q4_K) return mmq_launch_typed<T_Q4_K>(P, cg, grid, smem, st);
-    if (type == T_Q5_K) return mmq_launch_typed<T_Q5_K>(P, cg, grid, smem, st);
-    if (type == T_Q6_K) return mmq_launch_typed<T_Q6_K>(P, cg, grid, smem, st);
-    if (type == T_Q8_0) return mmq_launch_typed<T_Q8_0>(P, cg, grid, smem, st);
-    return mmq_launch_typed<T_Q5_1>(P, cg, grid, smem, st);
+    dim3 grid((unsigned) grid_x, 1, 1);
+    if (type == T_Q4_K) return mmq_launch_typed<T_Q4_K>(P, BN, grid, smem, st);
+    if (type == T_Q5_K) return mmq_launch_typed<T_Q5_K>(P, BN, grid, smem, st);
+    if (type == T_Q6_K) return mmq_launch_typed<T_Q6_K>(P, BN, grid, smem, st);
+    if (type == T_Q8_0) return mmq_launch_typed<T_Q8_0>(P, BN, grid, smem, st);
+    return mmq_launch_typed<T_Q5_1>(P, BN, grid, smem, st);
 }
 
 }  // namespace pb

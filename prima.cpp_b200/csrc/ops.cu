@@ -1,6 +1,6 @@
-// prima.cpp_b200/csrc/ops.cu — the non-GEMV ops of the decode graph, fused the way the B200 decode loop needs them.
+// prima.cpp_b200/csrc/ops.cu — the non-GEMV ops of the decode graph, fused the way the decode loop needs them.
 //
-// Reference ops replaced (file:line under /root/reference/ggml/src/ggml-cuda): quantize.cu:4-38 (activation quant),
+// Reference ops replaced (file:line under the reference's ggml/src/ggml-cuda): quantize.cu:4-38 (activation quant),
 // norm.cu:100-132 (rms_norm_f32) + binbcast.cu (MUL by the norm weight), rope.cu:32-109, cpy.cu:34 (f32->f16 KV store),
 // softmax.cu:14-116, the FA-off attention chain ggml-cuda.cu:1737-1881 (batched cuBLAS KQ / KQV), unary.cu (silu),
 // getrows.cu.  Numerics follow the CPU backend (ggml.c:11950, 14143, 13783, 12377), see each kernel.
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(1024) k_rmsnorm_quant(const float * __restrict
 // Decode-path variant: q8_K( rms_norm(x) * w ) of one vector, ONE CTA of 16 warps.  The vector is read once (128-bit loads, all
 // issued before anything is used) and stays in registers between the sum of squares and the quantization.  Under PDL the GEMV
 // that consumes the result is already resident and streaming its weights while this runs; doing the same work in the prologue
-// of each of its 296 CTAs cost ~7 us per launch (profiles/r2_token_trace_v1.txt: 19 MB of redundant L2 reads).
+// of each of its CTAs would read the whole vector from L2 once per CTA.
 constexpr int RQ_WARPS = 16;   // RQ_B super-blocks per warp in registers: 2 (n <= 8192, ~64 registers: fits beside a resident GEMV CTA) or 4
 template <int RQ_B>
 __global__ void __launch_bounds__(RQ_WARPS * 32) k_rmsnorm_q8K(const float * __restrict__ x, const float * __restrict__ w, int n, float eps, ActQ out) {
@@ -617,7 +617,7 @@ __global__ void __launch_bounds__(256) k_attn_fused(const float * __restrict__ q
 // kernel sits between the q|k|v GEMV and the wo GEMV, and every microsecond of it is a bubble in the weight stream:
 //   * one CTA of 16 warps per q head, launched as CLUSTERS OF 2 (heads 2j, 2j+1 = one 256-value q8_K super-block of the output):
 //     the pair agrees on the block's arg-max through distributed shared memory and writes the QUANTIZED activation itself,
-//     so the wo GEMV needs no quantize prologue (4 us per layer in profiles/r2_token_trace_v1.txt);
+//     so the wo GEMV needs no quantize prologue;
 //   * everything that does not depend on the q|k|v GEMV happens BEFORE griddepcontrol.wait: the position, the RoPE angles and
 //     the K/V cache rows [0, pos) (written by earlier tokens) — up to 256 rows each are in flight as cp.async copies into
 //     shared memory (completion on mbarriers) while the GEMV drains.  Round 1's kernel chained ~10 dependent L2 round trips

@@ -18,7 +18,7 @@ def lib_path() -> Path:
 
 
 def build(force: bool = False) -> Path:
-    """Compile libprima_b200.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libprima_b200.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     if force:
         subprocess.check_call(["make", "-C", str(PKG / "csrc"), "clean"], stdout=subprocess.DEVNULL)
     subprocess.check_call(["make", "-C", str(PKG / "csrc"), "-j4"], stdout=subprocess.DEVNULL)
@@ -43,7 +43,7 @@ class Lib:
     def __init__(self):
         p = lib_path()
         if not p.exists():
-            raise Pb200Error(f"{p} is missing: run __graft_entry__.build() (nvcc, sm_100a); no CPU fallback exists")
+            raise Pb200Error(f"{p} is missing: run __graft_entry__.build() (nvcc, sm_90a); no CPU fallback exists")
         self.c = C.CDLL(str(p))
         c = self.c
         vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float

@@ -27,7 +27,7 @@ def _entered(stream):
 
 
 def layer_windows(n_layer: int, world: int) -> list[int]:
-    """Uniform contiguous windows (8 identical B200s need no ILP scheduler, common/common.cpp:860-1594): bounds[r]..bounds[r+1]."""
+    """Uniform contiguous windows (8 identical GPUs need no ILP scheduler, common/common.cpp:860-1594): bounds[r]..bounds[r+1]."""
     if world < 1 or n_layer < world:
         raise ValueError("need 1 <= world <= n_layer")
     return [round(r * n_layer / world) for r in range(world + 1)]

@@ -9,7 +9,7 @@ sys.path.insert(0, str(ROOT / "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -24,7 +24,7 @@ def ref():
     if not O.have_ref():
         O.build_ref()
     if not O.have_ref():
-        pytest.skip("oracle/_ref not built and /root/reference absent")
+        pytest.skip("oracle/_ref not built and the reference source tree is not readable")
     return O.Ref()
 
 

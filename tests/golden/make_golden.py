@@ -1,6 +1,5 @@
-"""Generates tests/golden/*.npz from the UNMODIFIED reference compiled into oracle/_ref (run in the build container where
-/root/reference exists:  python tests/golden/make_golden.py).  The fixtures travel with the repo; the GPU box never needs
-/root/reference."""
+"""Generates tests/golden/*.npz from the UNMODIFIED reference compiled into oracle/_ref (run where the reference source tree is
+readable:  python tests/golden/make_golden.py).  The fixtures are committed; the tests never need the reference tree."""
 import sys
 from pathlib import Path
 
@@ -13,7 +12,7 @@ from tiny_model import TinyModel  # noqa: E402
 
 
 def main():
-    assert O.build_ref(), "needs /root/reference to build oracle/_ref"
+    assert O.build_ref(), "needs the reference source tree to build oracle/_ref"
     r = O.Ref(4)
     # 1) per-type kernels on the analytic input of tests/test-quantize-fns.cpp:30-34 (0.1 + 2 cos(i + off))
     N, K = 6, 1024

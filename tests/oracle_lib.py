@@ -2,7 +2,7 @@
 
 * ``port``  : oracle/liboracle_port.so — our plain-C restatement (oracle/kquants_port.c).
 * ``ref``   : oracle/_ref/{v3,v4}/libggml_ref.so + libgraph_ref.so — the UNMODIFIED reference CPU ggml
-              compiled from /root/reference (oracle/Makefile); travels to the GPU box pre-built.
+              compiled from the reference source tree (oracle/Makefile).
 Also: synthetic GGUF-block generators shared by the tests and bench.py's cpu legs.
 """
 from __future__ import annotations
@@ -64,9 +64,14 @@ def build_port() -> Path:
     return so
 
 
+def have_reference_tree() -> bool:
+    """Whether the reference source tree oracle/Makefile points at (REF) is present and readable by this user."""
+    return subprocess.call(["make", "-s", "-C", str(ORACLE), "have-ref"], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL) == 0
+
+
 def build_ref() -> bool:
-    """(Re)build oracle/_ref from /root/reference when that tree is present (this container only)."""
-    if not Path("/root/reference/ggml/src/ggml.c").exists():
+    """(Re)build oracle/_ref from the reference source tree when that tree is readable."""
+    if not have_reference_tree():
         return have_ref()
     subprocess.check_call(["make", "-C", str(ORACLE), "-j8", "ref"], stdout=subprocess.DEVNULL)
     return have_ref()

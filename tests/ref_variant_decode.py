@@ -8,14 +8,12 @@ import numpy as np
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT / "tests"))
 import oracle_lib as O          # noqa: E402
-from tiny_model import TinyModel  # noqa: E402
+from golden.make_reference_golden import divergence_model  # noqa: E402
 
 arch, n_tok, out = sys.argv[1], int(sys.argv[2]), sys.argv[3]
-branch = float(sys.argv[4]) if len(sys.argv) > 4 else 0.1
-tm = TinyModel(n_layer=3, n_embd=1024, n_head=8, n_head_kv=2, n_ff=2816 if arch == "llama" else 3104, n_vocab=384, n_ctx=96, arch=arch,
-               ftype="q4_K_M" if arch == "llama" else "q5_K_M", freq_factors=(arch == "llama"), seed=11, branch_scale=branch)
+tm, toks = divergence_model(arch)
+toks = toks[:n_tok]
 ref = O.Ref(4)
-toks = [(i * 7919 + 13) % 384 for i in range(n_tok)]
 logits, _ = tm.ref_decode(ref, toks)
 np.save(out, logits)
 print(O.ref_variant())

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 import oracle_lib as O
+from golden import make_reference_golden as RG
 from tiny_model import TinyModel, from_golden
 
 pytestmark = pytest.mark.gpu
@@ -67,11 +68,10 @@ def test_engine_vs_port_longer_decode(cuda, pkg, port, arch, ftype, ff):
     eng.close()
 
 
-def test_engine_vs_compiled_reference(cuda, pkg, ref):
-    tm = TinyModel(n_layer=2, n_embd=512, n_head=4, n_head_kv=2, n_ff=1024, n_vocab=320, n_ctx=64, arch="llama", quantizer=ref.quantize, seed=5,
-                   branch_scale=0.1)
-    toks = [(i * 7919 + 13) % 320 for i in range(12)]
-    want, _ = tm.ref_decode(ref, toks)
+def test_engine_vs_compiled_reference(cuda, pkg):
+    # the reference CPU graph's logits on these weights are recorded in golden/reference_golden.npz (golden/make_reference_golden.py)
+    tm, toks = RG.engine_model()
+    want = np.load(G / "reference_golden.npz")["engine_logits"]
     eng = tm.load_engine(pkg)
     got = np.zeros_like(want)
     for i, t in enumerate(toks):
@@ -80,20 +80,34 @@ def test_engine_vs_compiled_reference(cuda, pkg, ref):
     eng.close()
 
 
-def test_engine_llama3_70b_layer_shapes_vs_compiled_reference(cuda, pkg, ref):
+@pytest.mark.parametrize("arch", ["llama", "qwen2"])
+def test_engine_40_tokens_vs_reference_graph(cuda, pkg, arch):
+    """40 tokens of a 3-layer Llama (rope freq factors, Q4_K_M) / Qwen2 (q/k/v biases, Q5_K_M, ffn_down on Q5_1 / Q8_0) decoded by the
+    engine against the reference CPU graph on the same bytes (its AVX2 build's logits, recorded in golden/reference_golden.npz):
+    the multi-token bar, whose noise the reference's own AVX2 and AVX-512 builds show against each other on exactly these runs."""
+    tm, toks = RG.divergence_model(arch)
+    want = np.load(G / "reference_golden.npz")[f"selfdiv_{arch}_v3"]
+    eng = tm.load_engine(pkg)
+    got = np.zeros_like(want)
+    for i, t in enumerate(toks):
+        eng.decode(int(t), i, got[i])
+    check_decode_parity(got, want)
+    eng.close()
+
+
+def test_engine_llama3_70b_layer_shapes_vs_compiled_reference(cuda, pkg):
     """Whole-engine parity at the BASELINE config's layer shapes (VERDICT r1 #9): 2 full-size Llama-3-70B layers (n_embd 8192, 64/8 heads,
     n_ff 28672: the split-row ffn_down kernel, the 3-matrix q|k|v launch, the Q5_K / Q6_K v and down of the Q4_K_M mixture) + a
     small vocabulary, decoded token by token against the UNMODIFIED reference CPU backend (oracle/_ref) on the same quantized bytes."""
-    tm = TinyModel(n_layer=2, n_embd=8192, n_head=64, n_head_kv=8, n_ff=28672, n_vocab=512, n_ctx=32, arch="llama", ftype="q4_K_M", seed=21,
-                   branch_scale=0.1)
-    toks = [(i * 7919 + 13) % 512 for i in range(8)]
-    want, hid = tm.ref_decode(ref, toks)
+    tm, toks = RG.engine_70b_model()
+    z = np.load(G / "reference_golden.npz")
+    want, hid0 = z["engine_70b_logits"], z["engine_70b_hidden0"]
     eng = tm.load_engine(pkg)
     got = np.zeros_like(want)
     for i, t in enumerate(toks):
         eng.decode(int(t), i, got[i])
         if i == 0:
-            assert np.max(np.abs(eng.hidden() - hid[0])) < TOL
+            assert np.max(np.abs(eng.hidden() - hid0)) < TOL
     check_decode_parity(got, want)
     assert np.max(np.abs(got[0] - want[0])) < TOL
     eng.close()

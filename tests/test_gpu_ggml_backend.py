@@ -20,7 +20,7 @@ OPS = ["MUL_MAT", "RMS_NORM", "ROPE", "SOFT_MAX", "ADD", "MUL", "CPY", "CONT", "
 def run_tbo(args, timeout=900):
     exe = O.ORACLE / "_ref" / "v3" / "test-backend-ops"
     if not exe.exists() or not PLUGIN.exists():
-        pytest.skip("oracle/_ref/v3/test-backend-ops or libggml-b200.so not built (run __graft_entry__.build() where /root/reference exists)")
+        pytest.skip("oracle/_ref/v3/test-backend-ops or libggml-b200.so not built (build() builds them only where the reference source tree is readable)")
     env = dict(os.environ, LD_PRELOAD=str(PLUGIN))
     p = subprocess.run([str(exe)] + args, env=env, capture_output=True, text=True, timeout=timeout)
     return p.returncode, re.sub(r"\x1b\[[0-9;]*m", "", p.stdout + p.stderr)
@@ -41,10 +41,9 @@ def test_reference_test_backend_ops(cuda, op):
 
 
 def test_backend_perf_mode_mul_mat(cuda):
-    """test-backend-ops perf (m=4096, k=14336, n=1: tests/test-backend-ops.cpp:3703-3709) runs on the B200 backend and prints GB/s."""
+    """test-backend-ops perf (m=4096, k=14336, n=1: tests/test-backend-ops.cpp:3703-3709) runs on the "B200" ggml backend and prints GB/s."""
     rc, out = run_tbo(["perf", "-b", "B200_0", "-o", "MUL_MAT"], timeout=600)
     assert rc == 0, out[-2000:]
     lines = [l for l in out.splitlines() if "q4_K" in l and "n=1," in l]
     assert lines, out[-2000:]
-    (ROOT / "gpurun_out").mkdir(exist_ok=True)
-    (ROOT / "gpurun_out" / "test_backend_ops_perf.txt").write_text(out)
+    print("\n".join(lines))

@@ -16,7 +16,7 @@ ROOT = Path(__file__).resolve().parent.parent
 def run(arch, n_tok, dims=None, env=None):
     import os
     if not (ROOT / "host" / "_ggml" / "libllama_graph_host.so").exists() or not (ROOT / "prima.cpp_b200" / "libggml-b200.so").exists():
-        pytest.skip("host/_ggml or the plugin is not built (run __graft_entry__.build() where /root/reference exists)")
+        pytest.skip("host/_ggml or the plugin is not built (build() builds them only where the reference source tree is readable)")
     cmd = [sys.executable, str(ROOT / "tests" / "ggml_graph_parity.py"), arch, str(n_tok)] + ([str(d) for d in dims] if dims else [])
     p = subprocess.run(cmd, capture_output=True, text=True, timeout=900, env=dict(os.environ, **(env or {})))
     assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-4000:]

@@ -1,4 +1,4 @@
-"""-m gpu: the batched (prefill) k-quant product pb200_mul_mat_q — tcgen05 tensor cores — against the CPU oracle.
+"""-m gpu: the batched (prefill) k-quant product pb200_mul_mat_q — wgmma tensor cores — against the CPU oracle.
 
 Numerics bar (floating point, stated here): the kernel quantizes every activation row to q8_K exactly as the CPU backend
 does and expands the weights with the reference's dequantization formulas evaluated in fp16: the integer q is exact, the
@@ -35,7 +35,7 @@ def run_mmq(lib, t, W, N, K, X, bias=None, ldx=None, resid=None):
     lib.check(lib.c.pb200_mul_mat_q(t, ptr(Wd), N, K, ptr(xd), ldx, T, ptr(y), ptr(bd) if bd is not None else None,
                                     ptr(rd) if rd is not None else None, ptr(ws), None), "mul_mat_q")
     sync()
-    assert lib.c.pb200_aborted() == 0, "tcgen05 pipeline gave up (watchdog)"
+    assert lib.c.pb200_aborted() == 0, "tensor-core pipeline gave up (watchdog)"
     return y.cpu().numpy()
 
 

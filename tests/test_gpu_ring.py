@@ -139,7 +139,7 @@ def _ring_rank(rank, world, port, rounds, q):
 def test_ring_across_nccl_ranks_bit_identical_to_single_process(cuda, pkg):
     world = 2
     if torch.cuda.device_count() < world:
-        pytest.skip("needs 2 GPUs (run with gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     rounds = 5
     want = greedy_reference(_model(), pkg, [(5 + 9 * s, s) for s in range(world)], rounds)

@@ -1,6 +1,6 @@
 """GPU: the k-quant GEMV at the Llama-3-70B launch shapes, back to back through the C ABI (events), and the target of the ncu captures:
 
-    ncu --set full --clock-control none --import-source on -k regex:k_gemv_kquant -s 10 -c 5 -o gpurun_out/gemv python tools/gemv_probe.py 1
+    ncu --set full --clock-control none --import-source on -k regex:k_gemv_kquant -s 10 -c 5 -o gemv python tools/gemv_probe.py 1
 """
 import sys, ctypes as C
 from pathlib import Path
