@@ -15,16 +15,6 @@ using namespace pb;
 extern std::atomic<uint64_t> g_launches;
 
 namespace {
-ActQ act_from_ws(void * ws, int64_t k) {
-    const int64_t kp = (k + 255) / 256 * 256;
-    ActQ a{};
-    uint8_t * p = (uint8_t *) ws;
-    a.qs = (int8_t *) p;
-    a.d = (float *) (p + kp);
-    a.s = (float *) (p + kp + kp / 32 * 4);
-    a.bsums = (int16_t *) (p + kp + kp / 32 * 8);
-    return a;
-}
 bool type_ok(int t) { return t == T_Q4_K || t == T_Q5_K || t == T_Q6_K || t == T_Q8_0 || t == T_Q5_1; }
 }  // namespace
 
@@ -54,10 +44,7 @@ int64_t pb200_row_bytes(int type, int64_t k) { return row_bytes(type, k); }
 uint64_t pb200_kernel_launches(void) { return g_launches.load(); }
 void pb200_kernel_launches_add(uint64_t n) { g_launches += n; }
 
-size_t pb200_act_workspace_bytes(int64_t k) {
-    const int64_t kp = (k + 255) / 256 * 256;
-    return (size_t) kp + (size_t) kp / 32 * 8 + (size_t) kp / 16 * 2;
-}
+size_t pb200_act_workspace_bytes(int64_t k) { return act_ws_bytes(k); }
 
 int pb200_quantize_act(int wtype, const float * x, int64_t k, void * act_ws, void * stream) {
     if (!type_ok(wtype) || !x || !act_ws || k <= 0 || k % block_elems(wtype) != 0) return PB200_EINVAL;
@@ -69,8 +56,10 @@ int pb200_mul_mat_vec_q(int type, const void * W, int64_t n, int64_t k, const vo
                         void * stream) {
     if (!type_ok(type) || !W || !act_ws || !y || n <= 0 || k <= 0 || k % block_elems(type) != 0) return PB200_EINVAL;
     GemvDesc d = {W, y, bias, resid, type, (int) n};
-    g_launches++;
-    return launch_gemv(&d, 1, (int) k, act_from_ws(const_cast<void *>(act_ws), k), (cudaStream_t) stream, false);
+    uint64_t nl = 0;
+    const int rc = launch_gemv(&d, 1, (int) k, act_from_ws(const_cast<void *>(act_ws), k), GemvPrologue{}, (cudaStream_t) stream, false, nl);
+    g_launches += nl;
+    return rc;
 }
 
 int pb200_mul_mat_vec(int type, const void * W, int64_t n, int64_t k, const float * x, float * y, void * act_ws, void * stream) {
@@ -85,10 +74,13 @@ int pb200_mul_mat_vec_fused(int nmat, const int * types, const void * const * W,
     GemvDesc d[3];
     for (int i = 0; i < nmat; i++) {
         if (!type_ok(types[i]) || k % block_elems(types[i]) != 0) return PB200_EINVAL;
+        if (act_mode_for(types[i]) != act_mode_for(types[0])) return PB200_EINVAL;   // one activation: one quantization format
         d[i] = GemvDesc{W[i], y[i], nullptr, nullptr, types[i], (int) n[i]};
     }
-    g_launches++;
-    return launch_gemv(d, nmat, (int) k, act_from_ws(const_cast<void *>(act_ws), k), (cudaStream_t) stream, false);
+    uint64_t nl = 0;
+    const int rc = launch_gemv(d, nmat, (int) k, act_from_ws(const_cast<void *>(act_ws), k), GemvPrologue{}, (cudaStream_t) stream, false, nl);
+    g_launches += nl;
+    return rc;
 }
 
 int pb200_mul_mat_vec_host(int type, const void * W_dev, int64_t n, int64_t k, const float * x_host, float * y_host) {
@@ -154,11 +146,7 @@ int pb200_soft_max(const float * x, const float * mask, float * y, int64_t ncols
 
 int pb200_silu_mul(const float * gate, const float * up, float * y, int64_t n, void * stream) {
     if (!gate || !up || !y || n <= 0) return PB200_EINVAL;
-    ActQ none{};
-    // the fused kernel writes the f32 product and skips quantization when no workspace is given
-    ActQ scratch = none;
     g_launches++;
-    // quantization needs a workspace; use the f32-only path: silu then mul
     int e = launch_silu(gate, y, n, (cudaStream_t) stream);
     if (e) return e;
     g_launches++;
@@ -211,7 +199,7 @@ int pb200_attn_decode(const float * q, const void * k_cache_f16, const void * v_
     if (!q || !k_cache_f16 || !v_cache_f16 || !out || !pos_dev || head_dim != 128 || n_head_kv <= 0 || n_head <= 0 || n_head % n_head_kv) return PB200_EINVAL;
     g_launches++;
     return launch_attn_decode(q, (const __half *) k_cache_f16, (const __half *) v_cache_f16, out, n_head, n_head_kv, head_dim, pos_dev, n_ctx, scale,
-                              nullptr, (cudaStream_t) stream, false);
+                              (cudaStream_t) stream, false);
 }
 
 int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * act_ws, int prologue, const float * in0, const float * in1, float eps,
@@ -225,23 +213,12 @@ int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * ac
         if (!is_kquant(mats[i].type) || ((uintptr_t) mats[i].W & 15)) return PB200_ENOTSUP;
         d[i] = GemvDesc{mats[i].W, mats[i].y, nullptr, mats[i].add, mats[i].type, (int) mats[i].n};
     }
-    cudaStream_t st = (cudaStream_t) stream;
-    const ActQ act = act_from_ws(act_ws, k);
-    GemvFused pro;
-    bool gemv_pdl = pdl != 0;
-    if (prologue != 0) {
-        if (sync_ws && gemv_dist_prologue_ok()) {
-            pro.kind = prologue == 1 ? 4 : 5; pro.in0 = in0; pro.in1 = in1; pro.eps = eps; pro.gbar = (unsigned int *) sync_ws;
-        } else {   // the grid cannot be made co-resident on this device: produce the activation with a small kernel in front
-            g_launches++;
-            int e = prologue == 1 ? launch_rmsnorm_quant(in0, in1, (int) k, eps, ACT_Q8_K, act, nullptr, st, gemv_pdl)
-                                  : launch_silu_mul_quant(in0, in1, (int) k, ACT_Q8_K, act, nullptr, st, gemv_pdl);
-            if (e) return e;
-            gemv_pdl = true;
-        }
-    }
-    g_launches++;
-    return launch_gemv_kquant_fused(d, nmat, (int) k, act, pro, st, gemv_pdl);
+    static const int kind[3] = {PRO_NONE, PRO_RMSNORM, PRO_SILU_MUL};   // the ABI's prologue codes
+    const GemvPrologue pro{kind[prologue], in0, in1, eps, (unsigned int *) sync_ws, nullptr};
+    uint64_t nl = 0;
+    const int rc = launch_gemv(d, nmat, (int) k, act_from_ws(act_ws, k), pro, (cudaStream_t) stream, pdl != 0, nl);
+    g_launches += nl;
+    return rc;
 }
 
 int pb200_attn_ggml(const float * q, const float * k, const float * v, void * k_cache_f16, void * v_cache_t_f16, int64_t vt_stride, float * out,

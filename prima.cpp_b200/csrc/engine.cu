@@ -63,22 +63,6 @@ struct ActBuf {
     int64_t K = 0;
 };
 
-size_t act_ws_bytes(int64_t k) {
-    const int64_t kp = (k + 255) / 256 * 256;
-    // qs[kp] | d[kp/32] f32 | s[kp/32] f32 | bsums[kp/16] i16     (all 16-B aligned since kp % 256 == 0)
-    return (size_t) kp + (size_t) kp / 32 * 4 * 2 + (size_t) kp / 16 * 2;
-}
-ActQ act_from_ws(void * ws, int64_t k) {
-    const int64_t kp = (k + 255) / 256 * 256;
-    ActQ a{};
-    uint8_t * p = (uint8_t *) ws;
-    a.qs = (int8_t *) p;
-    a.d = (float *) (p + kp);
-    a.s = (float *) (p + kp + kp / 32 * 4);
-    a.bsums = (int16_t *) (p + kp + kp / 32 * 8);
-    return a;
-}
-
 }  // namespace
 
 struct pb200_model {
@@ -343,8 +327,10 @@ int pb200_model_synth(pb200_model * m, int ftype, uint64_t seed) {
     return (int) cudaStreamSynchronize(m->stream);
 }
 
-// profile pass: CUDA events around every GEMV launch (direct launches, no graph) -> per-launch durations for the roofline
-static int prof_begin(pb200_model * m, int64_t bytes) {
+// profile pass: CUDA events around every GEMV group (direct launches, no graph) -> per-group durations for the roofline.  The start
+// event is handed to launch_gemv, which records it after any producer kernel, right in front of the GEMV kernels.
+static int prof_begin(pb200_model * m, int64_t bytes, cudaEvent_t & start) {
+    start = nullptr;
     if (!m->profiling) return 0;
     if (m->prof_ev.size() < 2 * (m->prof_n + 1)) {
         cudaEvent_t a, b;
@@ -353,7 +339,8 @@ static int prof_begin(pb200_model * m, int64_t bytes) {
         m->prof_bytes.push_back(0);
     }
     m->prof_bytes[m->prof_n] = bytes;
-    return (int) cudaEventRecord(m->prof_ev[2 * m->prof_n], m->stream);
+    start = m->prof_ev[2 * m->prof_n];
+    return 0;
 }
 static int prof_end(pb200_model * m) {
     if (!m->profiling) return 0;
@@ -363,22 +350,19 @@ static int prof_end(pb200_model * m) {
 }
 static int64_t tbytes(const Tensor & t) { return (int64_t) t.bytes; }
 
-// one decode step enqueued on m->stream (captured into the CUDA graph by finalize)
+// one decode step enqueued on m->stream (captured into the CUDA graph by finalize); every kernel is PDL-chained to the previous one
 static int enqueue_step(pb200_model * m, int seq, uint64_t * nlaunch) {
     const pb200_hparams & hp = m->hp;
     const int E = hp.n_embd, H = hp.n_head, HK = hp.n_head_kv, D = hp.head_dim, F = hp.n_ff;
     const int QD = H * D, EK = HK * D;
     cudaStream_t st = m->stream;
-    static const bool pdl = getenv("PB200_NO_PDL") == nullptr;   // programmatic dependent launch on every kernel of the step
-    static const bool attn_v2 = getenv("PB200_ATTN_V1") == nullptr;   // A/B: round 1's attention kernel + quantize prologue in wo
-    static const bool dist_env = getenv("PB200_NO_DIST") == nullptr;   // A/B: single-CTA rmsnorm / silu kernels in front of the GEMVs instead
-    const bool dist = dist_env && gemv_dist_prologue_ok();
     uint64_t n = 0;
+    cudaEvent_t ev = nullptr;   // profiling: start event of the next GEMV group
     const int32_t * tok_dev = m->tokpos_dev + 4 * seq, * pos_dev = m->tokpos_dev + 4 * seq + 1;
     const size_t nl_ = m->layers.size();
     float * x = m->x_in;
     if (m->with_embd) {
-        CK(launch_get_rows(m->tok_embd.data, m->tok_embd.type, E, tok_dev, 1, m->x_a, st, pdl)); n++; CK(dbg_sync(st, "get_rows"));
+        CK(launch_get_rows(m->tok_embd.data, m->tok_embd.type, E, tok_dev, 1, m->x_a, st, true)); n++; CK(dbg_sync(st, "get_rows"));
         x = m->x_a;
     }
     const float kq_scale = 1.0f / sqrtf((float) D);
@@ -393,84 +377,38 @@ static int enqueue_step(pb200_model * m, int seq, uint64_t * nlaunch) {
             if (bufs[i] != x) { if (!x1) x1 = bufs[i]; else x2 = bufs[i]; }
         if (il + 1 == m->l1) x2 = m->x_out;   // the last layer writes hidden_out in place (a copy node would break the PDL chain)
         // --- attention block ---
-        const bool qkv_k = is_kquant(L.wq.type) && is_kquant(L.wk.type) && is_kquant(L.wv.type) && gemv_fused_prologue_ok(E);
-        if (qkv_k) {
+        {
             GemvDesc d[3] = {{L.wq.data, m->q, L.bq, nullptr, L.wq.type, QD},
                              {L.wk.data, m->k, L.bk, nullptr, L.wk.type, EK},
                              {L.wv.data, m->v, L.bv, nullptr, L.wv.type, EK}};
-            GemvFused pro;
-            if (dist) {   // rms_norm * attn_norm -> q8_K inside the GEMV: CTA c produces super-block c, one grid barrier
-                pro.kind = 4; pro.in0 = x; pro.in1 = L.attn_norm; pro.eps = hp.rms_eps; pro.gbar = m->gbar;
-            } else {      // ... or once by a single-CTA kernel in front of it
-                CK(launch_rmsnorm_quant(x, L.attn_norm, E, hp.rms_eps, ACT_Q8_K, m->actE.q, nullptr, st, pdl)); n++;
-            }
-            CK(prof_begin(m, tbytes(L.wq) + tbytes(L.wk) + tbytes(L.wv)));
-            CK(launch_gemv_kquant_fused(d, 3, E, m->actE.q, pro, st, pdl)); n++; CK(dbg_sync(st, "gemv qkv"));
+            const GemvPrologue pro{PRO_RMSNORM, x, L.attn_norm, hp.rms_eps, m->gbar, m->g};   // g: scratch
+            CK(prof_begin(m, tbytes(L.wq) + tbytes(L.wk) + tbytes(L.wv), ev));
+            CK(launch_gemv(d, 3, E, m->actE.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv qkv"));
             CK(prof_end(m));
-        } else {
-            ActQ none{};
-            CK(launch_rmsnorm_quant(x, L.attn_norm, E, hp.rms_eps, ACT_Q8_K, none, m->g, st, pdl)); n++;   // f32 normalized -> g (scratch)
-            Tensor * ws[3] = {&L.wq, &L.wk, &L.wv};
-            float * ys[3] = {m->q, m->k, m->v};
-            const float * bs[3] = {L.bq, L.bk, L.bv};
-            for (int i = 0; i < 3; i++) {
-                CK(launch_quantize_act(m->g, E, act_mode_for(ws[i]->type), m->actE.q, st, pdl)); n++;
-                GemvDesc d1 = {ws[i]->data, ys[i], bs[i], nullptr, ws[i]->type, (int) ws[i]->N};
-                CK(launch_gemv(&d1, 1, E, m->actE.q, st, pdl)); n++;
-            }
         }
-        const bool wo_k = is_kquant(L.wo.type) && gemv_fused_prologue_ok(QD);
-        bool att_quantized = false;
-        if (wo_k && attn_v2) {   // clustered attention writes the q8_K activation of wo itself
-            const int rc = launch_attn_fused2(m->q, m->k, m->v, kc, vc, m->att, m->actQD.q, H, HK, D, pos_dev, hp.n_ctx, m->rp, m->rope_ff, kq_scale, st, pdl);
-            if (rc == 0) { att_quantized = true; n++; }
-            else if (rc != (int) cudaErrorNotSupported) return rc;
-        }
-        if (!att_quantized) { CK(launch_attn_fused(m->q, m->k, m->v, kc, vc, m->att, H, HK, D, pos_dev, hp.n_ctx, m->rp, m->rope_ff, kq_scale, st, pdl)); n++; }
-        CK(dbg_sync(st, "attn"));
+        bool att_quantized = false;   // the attention kernel also wrote wo's activation
+        CK(launch_attn_step(m->q, m->k, m->v, kc, vc, m->att, m->actQD.q, act_mode_for(L.wo.type), H, HK, D, pos_dev, hp.n_ctx, m->rp, m->rope_ff,
+                            kq_scale, st, true, att_quantized)); n++; CK(dbg_sync(st, "attn"));
         {
             GemvDesc d1 = {L.wo.data, x1, nullptr, x, L.wo.type, E};   // ffn_inp = wo.att + inpSA
-            if (!att_quantized) { CK(launch_quantize_act(m->att, QD, act_mode_for(L.wo.type), m->actQD.q, st, pdl)); n++; }
-            CK(prof_begin(m, tbytes(L.wo)));
-            CK(launch_gemv(&d1, 1, QD, m->actQD.q, st, pdl)); n++; CK(dbg_sync(st, "gemv wo"));
+            const GemvPrologue pro = att_quantized ? GemvPrologue{} : GemvPrologue{PRO_QUANTIZE, m->att};
+            CK(prof_begin(m, tbytes(L.wo), ev));
+            CK(launch_gemv(&d1, 1, QD, m->actQD.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv wo"));
             CK(prof_end(m));
         }
         // --- FFN block ---
-        const bool gu_k = is_kquant(L.gate.type) && is_kquant(L.up.type) && gemv_fused_prologue_ok(E);
-        if (gu_k) {
+        {
             GemvDesc d[2] = {{L.gate.data, m->g, nullptr, nullptr, L.gate.type, F}, {L.up.data, m->u, nullptr, nullptr, L.up.type, F}};
-            GemvFused pro;
-            if (dist) {
-                pro.kind = 4; pro.in0 = x1; pro.in1 = L.ffn_norm; pro.eps = hp.rms_eps; pro.gbar = m->gbar;
-            } else {
-                CK(launch_rmsnorm_quant(x1, L.ffn_norm, E, hp.rms_eps, ACT_Q8_K, m->actE.q, nullptr, st, pdl)); n++;
-            }
-            CK(prof_begin(m, tbytes(L.gate) + tbytes(L.up)));
-            CK(launch_gemv_kquant_fused(d, 2, E, m->actE.q, pro, st, pdl)); n++; CK(dbg_sync(st, "gemv gate|up"));
+            const GemvPrologue pro{PRO_RMSNORM, x1, L.ffn_norm, hp.rms_eps, m->gbar, m->att};   // att: scratch
+            CK(prof_begin(m, tbytes(L.gate) + tbytes(L.up), ev));
+            CK(launch_gemv(d, 2, E, m->actE.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv gate|up"));
             CK(prof_end(m));
-        } else {
-            ActQ none{};
-            CK(launch_rmsnorm_quant(x1, L.ffn_norm, E, hp.rms_eps, ACT_Q8_K, none, m->att, st, pdl)); n++;
-            Tensor * ws[2] = {&L.gate, &L.up};
-            float * ys[2] = {m->g, m->u};
-            for (int i = 0; i < 2; i++) {
-                CK(launch_quantize_act(m->att, E, act_mode_for(ws[i]->type), m->actE.q, st, pdl)); n++;
-                GemvDesc d1 = {ws[i]->data, ys[i], nullptr, nullptr, ws[i]->type, (int) ws[i]->N};
-                CK(launch_gemv(&d1, 1, E, m->actE.q, st, pdl)); n++;
-            }
         }
         {
             GemvDesc d1 = {L.down.data, x2, nullptr, x1, L.down.type, E};   // l_out = down.act + ffn_inp
-            const bool down_k = is_kquant(L.down.type) && gemv_fused_prologue_ok(F);
-            if (down_k && dist) {   // silu(g)*u -> q8_K inside the GEMV, distributed over the grid
-                GemvFused pro; pro.kind = 5; pro.in0 = m->g; pro.in1 = m->u; pro.gbar = m->gbar;
-                CK(prof_begin(m, tbytes(L.down)));
-                CK(launch_gemv_kquant_fused(&d1, 1, F, m->actF.q, pro, st, pdl)); n++; CK(dbg_sync(st, "gemv down"));
-            } else {
-                CK(launch_silu_mul_quant(m->g, m->u, F, act_mode_for(L.down.type), m->actF.q, nullptr, st, pdl)); n++; CK(dbg_sync(st, "silu"));
-                CK(prof_begin(m, tbytes(L.down)));
-                CK(launch_gemv(&d1, 1, F, m->actF.q, st, pdl)); n++; CK(dbg_sync(st, "gemv down"));
-            }
+            const GemvPrologue pro{PRO_SILU_MUL, m->g, m->u, 0.f, m->gbar};
+            CK(prof_begin(m, tbytes(L.down), ev));
+            CK(launch_gemv(&d1, 1, F, m->actF.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv down"));
             CK(prof_end(m));
         }
         x = x2;
@@ -479,15 +417,10 @@ static int enqueue_step(pb200_model * m, int seq, uint64_t * nlaunch) {
     if (x != m->x_out) { CK(cudaMemcpyAsync(m->x_out, x, (size_t) E * 4, cudaMemcpyDeviceToDevice, st)); }
     if (m->with_head) {
         GemvDesc d1 = {m->output.data, m->logits, nullptr, nullptr, m->output.type, hp.n_vocab};
-        CK(prof_begin(m, tbytes(m->output)));
-        const bool head_pdl = pdl && m->l1 > m->l0;   // a stage without layers starts with a copy node: no programmatic edge
-        if (is_kquant(m->output.type) && gemv_fused_prologue_ok(E) && dist) {
-            GemvFused pro; pro.kind = 4; pro.in0 = m->x_out; pro.in1 = m->output_norm; pro.eps = hp.rms_eps; pro.gbar = m->gbar;
-            CK(launch_gemv_kquant_fused(&d1, 1, E, m->actE.q, pro, st, head_pdl)); n++;
-        } else {
-            CK(launch_rmsnorm_quant(m->x_out, m->output_norm, E, hp.rms_eps, act_mode_for(m->output.type), m->actE.q, nullptr, st, head_pdl)); n++;
-            CK(launch_gemv(&d1, 1, E, m->actE.q, st, pdl)); n++;
-        }
+        const GemvPrologue pro{PRO_RMSNORM, m->x_out, m->output_norm, hp.rms_eps, m->gbar};
+        const bool head_pdl = m->l1 > m->l0;   // a stage without layers starts with a copy node: no programmatic edge
+        CK(prof_begin(m, tbytes(m->output), ev));
+        CK(launch_gemv(&d1, 1, E, m->actE.q, pro, st, head_pdl, n, ev));
         CK(prof_end(m));
     }
     if (nlaunch) *nlaunch = n;
@@ -644,10 +577,8 @@ static int pf_matmul(pb200_model * m, const Tensor & W, const float * x, int T, 
     if (pre) return (int) cudaErrorInvalidValue;   // callers fuse a producer only when pf_tc(W, T) && is_kquant(W.type)
     ActQ act = act_from_ws(m->actF.base, W.K);
     for (int t = 0; t < T; t++) {
-        CK(launch_quantize_act(x + (size_t) t * W.K, (int) W.K, act_mode_for(W.type), act, st, false));
         GemvDesc d1 = {W.data, y + (size_t) t * W.N, bias, resid ? resid + (size_t) t * W.N : nullptr, W.type, (int) W.N};
-        CK(launch_gemv(&d1, 1, (int) W.K, act, st, false));
-        n += 2;
+        CK(launch_gemv(&d1, 1, (int) W.K, act, GemvPrologue{PRO_QUANTIZE, x + (size_t) t * W.K}, st, false, n));
     }
     return 0;
 }
@@ -718,7 +649,7 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
         // rms_norm * attn_norm rides in the activation pass of q (k and v reuse its image) when all three take the tensor-core path
         const bool qkv_fused = pf_tc(L.wq, T) && pf_tc(L.wk, T) && pf_tc(L.wv, T) && is_kquant(L.wq.type) && is_kquant(L.wk.type) && is_kquant(L.wv.type);
         if (qkv_fused) {
-            MmqPre pre; pre.kind = 2; pre.aux = L.attn_norm; pre.eps = hp.rms_eps;
+            MmqPre pre; pre.kind = PRO_RMSNORM; pre.aux = L.attn_norm; pre.eps = hp.rms_eps;
             CK(pf_matmul(m, L.wq, x, T, P.q, L.bq, nullptr, n, nullptr, &pre));
             CK(pf_matmul(m, L.wk, x, T, P.k, L.bk, nullptr, n, &L.wq));
             CK(pf_matmul(m, L.wv, x, T, P.v, L.bv, nullptr, n, &L.wk));
@@ -736,7 +667,7 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
         CK(pf_matmul(m, L.wo, P.att, T, y, nullptr, x, n));                  // ffn_inp = wo.att + inpSA (residual in the epilogue)
         // --- FFN block ---
         if (pf_tc(L.gate, T) && pf_tc(L.up, T) && is_kquant(L.gate.type) && is_kquant(L.up.type)) {
-            MmqPre pre; pre.kind = 2; pre.aux = L.ffn_norm; pre.eps = hp.rms_eps;
+            MmqPre pre; pre.kind = PRO_RMSNORM; pre.aux = L.ffn_norm; pre.eps = hp.rms_eps;
             CK(pf_matmul(m, L.gate, y, T, P.g, nullptr, nullptr, n, nullptr, &pre));
             CK(pf_matmul(m, L.up, y, T, P.u, nullptr, nullptr, n, &L.gate));
         } else {
@@ -745,7 +676,7 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
             CK(pf_matmul(m, L.up, P.xn, T, P.u, nullptr, nullptr, n, &L.gate));
         }
         if (pf_tc(L.down, T) && is_kquant(L.down.type)) {                     // silu(g) * u inside ffn_down's activation pass
-            MmqPre pre; pre.kind = 1; pre.aux = P.u; pre.ld_aux = F;
+            MmqPre pre; pre.kind = PRO_SILU_MUL; pre.aux = P.u; pre.ld_aux = F;
             CK(pf_matmul(m, L.down, P.g, T, x, nullptr, y, n, nullptr, &pre));   // l_out = down.act + ffn_inp   (x is free: y holds ffn_inp)
         } else {
             CK(launch_silu_mul(P.g, P.u, P.g, (int64_t) T * F, st)); n++;
@@ -756,8 +687,7 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
     CK(cudaMemcpyAsync(m->x_out, x + (size_t) (T - 1) * E, (size_t) E * 4, cudaMemcpyDeviceToDevice, st));
     if (m->with_head) {
         GemvDesc d1 = {m->output.data, m->logits, nullptr, nullptr, m->output.type, hp.n_vocab};
-        CK(launch_rmsnorm_quant(m->x_out, m->output_norm, E, hp.rms_eps, act_mode_for(m->output.type), m->actE.q, nullptr, st, false)); n++;
-        CK(launch_gemv(&d1, 1, E, m->actE.q, st, false)); n++;
+        CK(launch_gemv(&d1, 1, E, m->actE.q, GemvPrologue{PRO_RMSNORM, m->x_out, m->output_norm, hp.rms_eps}, st, false, n));
     }
     g_launches += n;
     if (!sync) return 0;
@@ -891,14 +821,9 @@ int pb200_argmax_seq(pb200_model * m, int seq, int feed_back) {
     if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
     if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
     cudaSetDevice(m->device);
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(1); cfg.blockDim = dim3(1024); cfg.stream = m->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
+    LaunchCfg lc(dim3(1), dim3(1024), 0, m->stream, true);
     g_launches++;
-    return (int) cudaLaunchKernelEx(&cfg, k_argmax, (const float *) m->logits, (int) m->hp.n_vocab, m->sample_dev + seq,
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_argmax, (const float *) m->logits, (int) m->hp.n_vocab, m->sample_dev + seq,
                                     (int32_t *) (feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr));
 }
 int32_t * pb200_token_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->tokpos_dev + 4 * seq : nullptr; }

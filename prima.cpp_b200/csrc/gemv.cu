@@ -4,7 +4,6 @@
 #include "quantize.cuh"
 
 #include <algorithm>
-#include <cstdlib>
 
 namespace pb {
 
@@ -81,16 +80,6 @@ __device__ __forceinline__ void release_stage(const GemvParams & P, GemvSmemCtl 
     }
 }
 
-// initial stages that were held back until the activation loads had been issued (P.prefill < P.nstage_init)
-__device__ __forceinline__ void fill_rest(const GemvParams & P, GemvSmemCtl * ctl, uint8_t * stages, uint64_t pol) {
-    if (threadIdx.x == 0) {
-        for (int it = P.prefill; it < P.nstage_init; it++) {
-            const int t = blockIdx.x + it * gridDim.x;
-            if (t < P.ntiles) issue_tile(P, ctl, stages, it, t, pol);
-        }
-    }
-}
-
 // TYPE = weight type of every matrix of the launch (one dot routine in the hot loop: the three unrolled routines together are
 // ~126 KB of SASS, more than the instruction cache holds), or 0 = mixed (q|k|v with a Q5_K / Q6_K v)
 template <int TYPE>
@@ -105,7 +94,7 @@ __device__ __forceinline__ float dot_block(int type, const uint8_t * bp, const A
     return dot_q5K(bp, r);
 }
 
-// ---- distributed prologue (PRO_*_DIST): CTA c produces super-blocks c, c + grid, ... of the q8_K activation in P.act ----
+// ---- distributed prologue (PRO_RMSNORM / PRO_SILU_MUL): CTA c produces super-blocks c, c + grid, ... of the q8_K activation in P.act ----
 __device__ __forceinline__ void dist_prologue(const GemvParams & P, GemvSmemCtl * ctl, int warp, int lane) {
     const int nblk = P.nblk;
     if ((int) blockIdx.x >= nblk) return;                       // nothing to produce: straight to the barrier
@@ -117,7 +106,7 @@ __device__ __forceinline__ void dist_prologue(const GemvParams & P, GemvSmemCtl 
         load8(P.in1 + myblk * 256 + lane * 8, bw);
     }
     float scale = 1.f;
-    if (P.prologue == PRO_RMSNORM_DIST) {
+    if (P.prologue == PRO_RMSNORM) {
         // every producing CTA needs the whole sum of squares (one extra read of the vector per producer: 32 x 32 KB at K = 8192)
         double sum = 0.0;
         if (nblk <= GEMV_NW * PRO_B) {
@@ -148,7 +137,7 @@ __device__ __forceinline__ void dist_prologue(const GemvParams & P, GemvSmemCtl 
     }
     for (int b = myblk; b < nblk; b += GEMV_NW * (int) gridDim.x) {
         if (b != myblk) { load8(P.in0 + b * 256 + lane * 8, bx); load8(P.in1 + b * 256 + lane * 8, bw); }   // tiny grids only
-        if (P.prologue == PRO_RMSNORM_DIST) {
+        if (P.prologue == PRO_RMSNORM) {
 #pragma unroll
             for (int i = 0; i < 8; i++) bx[i] = __fmul_rn(__fmul_rn(bx[i], scale), bw[i]);
         } else {
@@ -227,7 +216,7 @@ __global__ void __launch_bounds__(GEMV_THREADS, GEMV_CTAS_PER_SM) k_gemv_kquant(
     // Weights never depend on the previous kernel: start streaming BEFORE griddepcontrol.wait.  Under PDL this CTA is resident
     // while the tail of the previous GEMV (or a whole small kernel: attention, silu-quant) still runs on other SMs.
     if (threadIdx.x == 0) {
-        for (int it = 0; it < P.prefill; it++) {
+        for (int it = 0; it < P.nstage_init; it++) {
             const int t = blockIdx.x + it * gridDim.x;
             if (t < P.ntiles) issue_tile(P, ctl, stages, it, t, pol);
         }
@@ -254,8 +243,7 @@ __global__ void __launch_bounds__(GEMV_THREADS, GEMV_CTAS_PER_SM) k_gemv_kquant(
     sa.s = nullptr;
     sa.qs_stride = ACT_SMEM_QS_STRIDE;
     sa.bs_stride = ACT_SMEM_BS_STRIDE;
-    const bool dist = P.prologue == PRO_RMSNORM_DIST || P.prologue == PRO_SILU_DIST;
-    if (dist) {
+    if (P.prologue != PRO_NONE) {
         dist_prologue(P, ctl, warp, lane);
         grid_barrier(P, ctl);
     }
@@ -272,7 +260,6 @@ __global__ void __launch_bounds__(GEMV_THREADS, GEMV_CTAS_PER_SM) k_gemv_kquant(
             sd[i] = i < nb32 ? __ldcg(P.act.d + i) : 0.f;
             if (TYPE == T_Q5_1) ss[i] = i < nb32 ? __ldcg(P.act.s + i) : 0.f;
         }
-        fill_rest(P, ctl, stages, pol);
         __syncthreads();
         r.nb = valid ? min(8, nb32 - 8 * blk) : 0;
         if (valid) {
@@ -300,7 +287,6 @@ __global__ void __launch_bounds__(GEMV_THREADS, GEMV_CTAS_PER_SM) k_gemv_kquant(
         }
         if ((int) threadIdx.x < nb16) cb = __ldcg(reinterpret_cast<const int4 *>(P.act.bsums) + threadIdx.x);
         if ((int) threadIdx.x < P.nblk) cd = __ldcg(P.act.d + threadIdx.x);
-        fill_rest(P, ctl, stages, pol);   // the small activation loads are out: they do not queue behind the rest of the ring fill
 #pragma unroll
         for (int j = 0; j < NQ_MAX; j++) {
             const int i = threadIdx.x + j * GEMV_THREADS;
@@ -721,19 +707,13 @@ bool gemv_fused_prologue_ok(int K) { return K > 0 && K % 256 == 0 && K / 256 <= 
 
 // ring geometry of one launch: rows per tile of each matrix, stage size, depth — everything that must fit 2 CTAs on an SM
 struct GemvPlan { int wpr, nblk_p2, nstage, nstage_init, stage_bytes, smem, owner_only, rel_count, rows[GEMV_MAX_MAT]; };
-// tunables (environment, read once): ring geometry experiments without a rebuild
-struct GemvTune { int stage_target, max_stage, prefill; };
-static const GemvTune tune = [] {
-    GemvTune t{GEMV_STAGE_TARGET, GEMV_MAX_STAGE, GEMV_MAX_STAGE};
-    if (const char * e = getenv("PB200_GEMV_STAGE_KB")) t.stage_target = std::max(4, atoi(e)) * 1024;
-    if (const char * e = getenv("PB200_GEMV_PREFILL")) t.prefill = std::max(0, atoi(e));
-    if (const char * e = getenv("PB200_GEMV_MAX_STAGE")) t.max_stage = std::min(GEMV_MAX_STAGE, std::max(2, atoi(e)));
-    return t;
-}();
 static bool is_blk32(int t) { return t == T_Q8_0 || t == T_Q5_1; }
-static bool gemv_plan(const int * types, const int * Ns, int nmat, int K, GemvPlan & pl) {
+// false: the group does not fit the ring kernel
+static bool gemv_plan(const GemvDesc * d, int nmat, int K, GemvPlan & pl) {
+    for (int i = 0; i < nmat; i++)
+        if ((uintptr_t) d[i].W & 15) return false;    // bulk copies need 16-byte aligned sources
     // k-quants: K a multiple of 256; 32-element block types (one matrix per launch): K a multiple of 32, columns of 8 blocks
-    const bool b32 = nmat == 1 && is_blk32(types[0]);
+    const bool b32 = nmat == 1 && is_blk32(d[0].type);
     if (b32 ? !(K > 0 && K % 32 == 0 && (K + 255) / 256 <= GEMV_ACT_MAX_NBLK) : !gemv_fused_prologue_ok(K)) return false;
     const int nblk = (K + 255) / 256;
     int wpr = 1;
@@ -745,16 +725,16 @@ static bool gemv_plan(const int * types, const int * Ns, int nmat, int K, GemvPl
     pl.nblk_p2 = nbp;
     int64_t biggest = 0;
     for (int i = 0; i < nmat; i++) {
-        if (!(is_kquant(types[i]) || b32) || Ns[i] < 1) return false;
-        const int64_t rb = row_bytes(types[i], K);
+        if (!(is_kquant(d[i].type) || b32) || d[i].N < 1) return false;
+        const int64_t rb = row_bytes(d[i].type, K);
         if (b32 && rb % 8 != 0) return false;          // the column dots read 64-bit words
-        int R = (int) std::max<int64_t>(1, tune.stage_target / rb);
+        int R = (int) std::max<int64_t>(1, GEMV_STAGE_TARGET / rb);
         R = std::max(rpw, R / rpw * rpw);              // whole slots
         if (wpr > 1) {                             // split rows: at most one row per warp group and stage, and a ring of >= 4 stages
             R = std::min(R, ngroups);
             while (R > 1 && (GEMV_SMEM_LIMIT - GEMV_CTL_BYTES) / ((R * rb + 16 + 127) / 128 * 128) < 5) R--;
         }
-        if (R > Ns[i]) R = (Ns[i] + rpw - 1) / rpw * rpw;   // (ragged rows of the last slot are masked in the kernel)
+        if (R > d[i].N) R = (d[i].N + rpw - 1) / rpw * rpw;   // (ragged rows of the last slot are masked in the kernel)
         pl.rows[i] = R;
         biggest = std::max<int64_t>(biggest, R * rb);
     }
@@ -763,7 +743,7 @@ static bool gemv_plan(const int * types, const int * Ns, int nmat, int K, GemvPl
     // the activation staging area overlays the last stages of the ring (they are filled once the activation is in registers)
     const int act = gemv_act_smem_bytes(nblk);
     const int act_stages = (act + pl.stage_bytes - 1) / pl.stage_bytes;
-    pl.nstage = std::min(tune.max_stage, (GEMV_SMEM_LIMIT - GEMV_CTL_BYTES) / pl.stage_bytes);
+    pl.nstage = std::min(GEMV_MAX_STAGE, (GEMV_SMEM_LIMIT - GEMV_CTL_BYTES) / pl.stage_bytes);
     if (pl.nstage >= GEMV_ROWQ) pl.nstage = GEMV_ROWQ - 1;   // split rows reuse their partial-sum slots GEMV_ROWQ rows later (see the kernel)
     // Owner-only visits: row slot j of iteration it belongs to group (it * R + j) mod ngroups; with a common R that pattern has
     // period ngroups / gcd(ngroups, R) in `it`, so if the ring depth is a multiple of it every stage is always consumed by the same
@@ -774,7 +754,7 @@ static bool gemv_plan(const int * types, const int * Ns, int nmat, int K, GemvPl
         bool same = true;
         for (int i = 1; i < nmat; i++) same = same && pl.rows[i] == pl.rows[0];
         const int R = pl.rows[0] / rpw;          // row slots per tile
-        if (same && R < ngroups && !getenv("PB200_GEMV_VISIT_ALL")) {
+        if (same && R < ngroups) {
             int g = R, b = ngroups;
             while (b) { const int t = g % b; g = b; b = t; }
             const int period = ngroups / g;
@@ -805,39 +785,10 @@ bool gemv_dist_prologue_ok() {
     }
     return cache[dev] == 1;
 }
-int gemv_smem_bytes(int type, int K, int N) {
-    GemvPlan pl;
-    return gemv_plan(&type, &N, 1, K, pl) ? pl.smem : 0;
-}
 
-// Fused launch of up to 3 k-quant matrices sharing one q8_K activation.  Returns cudaError_t as int.
-int launch_gemv_kquant(const GemvDesc * d, int nmat, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
-    GemvFused none{};
-    return launch_gemv_kquant_fused(d, nmat, K, act, none, stream, pdl);
-}
-
-int launch_gemv_kquant_fused(const GemvDesc * d, int nmat, int K, const ActQ & act, const GemvFused & pro, cudaStream_t stream, bool pdl) {
-    const bool b32 = nmat == 1 && is_blk32(d[0].type);   // Q8_0 / Q5_1 (act: q8_0 / q8_1): same ring, columns of 8 blocks, no fused prologue
-    if (nmat < 1 || nmat > GEMV_MAX_MAT || K <= 0 || (b32 ? K % 32 != 0 : K % 256 != 0)) return (int) cudaErrorInvalidValue;
-    if (b32 && pro.kind != PRO_NONE) return (int) cudaErrorInvalidValue;
-    int types[GEMV_MAX_MAT], Ns[GEMV_MAX_MAT];
-    bool fast = true;
-    for (int i = 0; i < nmat; i++) {
-        types[i] = d[i].type; Ns[i] = d[i].N;
-        if (!is_kquant(d[i].type) && !b32) return (int) cudaErrorInvalidValue;
-        if ((uintptr_t) d[i].W & 15) fast = false;      // bulk copies need 16-byte aligned sources
-    }
-    GemvPlan pl;
-    fast = fast && gemv_plan(types, Ns, nmat, K, pl);
-    if (!fast) {
-        if (pro.kind != PRO_NONE) return (int) cudaErrorInvalidValue;   // callers must check gemv_fused_prologue_ok / alignment
-        if (b32) return (int) cudaErrorNotSupported;                     // launch_gemv_generic falls back to its own kernels
-        for (int i = 0; i < nmat; i++) {
-            int e = launch_gemv_generic(d[i], K, act, stream, pdl);
-            if (e) return e;
-        }
-        return 0;
-    }
+// the ring kernel on a group gemv_plan accepted; pro: PRO_NONE (act is ready) or a distributed prologue
+static int launch_ring(const GemvDesc * d, int nmat, int K, const ActQ & act, const GemvPlan & pl, const GemvPrologue & pro, cudaStream_t stream,
+                       bool pdl) {
     GemvParams P{};
     P.wpr = pl.wpr;
     P.nblk_p2 = pl.nblk_p2;
@@ -848,13 +799,13 @@ int launch_gemv_kquant_fused(const GemvDesc * d, int nmat, int K, const ActQ & a
     P.nstage_init = pl.nstage_init;
     P.owner_only = pl.owner_only;
     P.rel_count = pl.rel_count;
-    P.prefill = std::min(pl.nstage_init, tune.prefill);
     P.stage_bytes = pl.stage_bytes;
     P.act = act;
     P.prologue = pro.kind;
     P.in0 = pro.in0;
     P.in1 = pro.in1;
     P.eps = pro.eps;
+    P.gbar = pro.gbar;
     P.abort_flag = abort_flag();
     P.trace = g_trace_buf ? g_trace_buf + (size_t) (g_trace_idx++ % (uint64_t) g_trace_slots) * GEMV_TRACE_ROW : nullptr;
     int tiles = 0;
@@ -873,11 +824,9 @@ int launch_gemv_kquant_fused(const GemvDesc * d, int nmat, int K, const ActQ & a
         tiles += (d[i].N + M.rows_per_tile - 1) / M.rows_per_tile;
     }
     P.ntiles = tiles;
-    P.gbar = pro.gbar;
-    if ((pro.kind == PRO_RMSNORM_DIST || pro.kind == PRO_SILU_DIST) && (!pro.gbar || !gemv_dist_prologue_ok())) return (int) cudaErrorInvalidValue;
     // instantiation: weight type (0 = mixed) x split rows x instrumented
-    int ty = types[0];
-    for (int i = 1; i < nmat; i++) if (types[i] != ty) ty = 0;
+    int ty = d[0].type;
+    for (int i = 1; i < nmat; i++) if (d[i].type != ty) ty = 0;
     const int ti = ty == T_Q4_K ? 1 : ty == T_Q5_K ? 2 : ty == T_Q6_K ? 3 : ty == T_Q8_0 ? 4 : ty == T_Q5_1 ? 5 : 0;
     const bool tr = g_trace_buf != nullptr;
     typedef void (*kern_t)(const GemvParams);
@@ -895,19 +844,14 @@ int launch_gemv_kquant_fused(const GemvDesc * d, int nmat, int K, const ActQ & a
     if (e != cudaSuccess) return (int) e;
     int grid = sm_count() * GEMV_CTAS_PER_SM;
     if (grid > P.ntiles) grid = P.ntiles;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(GEMV_THREADS);
-    cfg.dynamicSmemBytes = pl.smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return (int) cudaLaunchKernelEx(&cfg, fn, P);
+    LaunchCfg lc(dim3(grid), dim3(GEMV_THREADS), pl.smem, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, fn, P);
 }
 
+// Q8_0 / Q5_1 with 8-byte aligned rows and an activation that fits in shared memory: the per-warp cp.async streaming kernel
+static bool blk32_ok(const GemvDesc & d, int K) {
+    return is_blk32(d.type) && K % 32 == 0 && row_bytes(d.type, K) % 8 == 0 && K <= 131072 && ((uintptr_t) d.W & 7) == 0;
+}
 static int launch_gemv_blk32(const GemvDesc & d, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
     GemvB32Params P{};
     P.W = (const uint8_t *) d.W;
@@ -929,32 +873,11 @@ static int launch_gemv_blk32(const GemvDesc & d, int K, const ActQ & act, cudaSt
         if (e != cudaSuccess) return (int) e;
     }
     const int per_sm = (int) std::max<size_t>(1, std::min<size_t>(4, (224 * 1024) / (smem + 1024)));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(std::min((d.N + 7) / 8, sm_count() * per_sm));
-    cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return (int) cudaLaunchKernelEx(&cfg, k_gemv_blk32, P);
+    LaunchCfg lc(dim3(std::min((d.N + 7) / 8, sm_count() * per_sm)), dim3(256), smem, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_gemv_blk32, P);
 }
 
-int launch_gemv_generic(const GemvDesc & d, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
-    // 32-element block types: the bulk-copy ring of the k-quant kernel (columns of 8 blocks) when the shape fits it ...
-    static const bool no_ring32 = getenv("PB200_NO_BLK32_RING") != nullptr;
-    if (!no_ring32 && (d.type == T_Q8_0 || d.type == T_Q5_1)) {
-        GemvFused none{};
-        const int rc = launch_gemv_kquant_fused(&d, 1, K, act, none, stream, pdl);
-        if (rc != (int) cudaErrorNotSupported && rc != (int) cudaErrorInvalidValue) return rc;
-    }
-    // ... else, with 8-byte aligned rows and an activation that fits in shared memory, the per-warp cp.async streaming kernel
-    static const bool no_b32 = getenv("PB200_NO_BLK32") != nullptr;
-    if (!no_b32 && (d.type == T_Q8_0 || d.type == T_Q5_1) && K % 32 == 0 && row_bytes(d.type, K) % 8 == 0 && K % 16 == 0 && K <= 131072 &&
-        ((uintptr_t) d.W & 7) == 0)
-        return launch_gemv_blk32(d, K, act, stream, pdl);
+static int launch_gemv_generic(const GemvDesc & d, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
     GemvGenericParams P{};
     P.W = (const uint8_t *) d.W;
     P.y = d.y;
@@ -965,16 +888,97 @@ int launch_gemv_generic(const GemvDesc & d, int K, const ActQ & act, cudaStream_
     P.K = K;
     P.row_bytes = row_bytes(d.type, K);
     P.act = act;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((d.N + 7) / 8);
-    cfg.blockDim = dim3(256);
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return (int) cudaLaunchKernelEx(&cfg, k_gemv_generic, P);
+    LaunchCfg lc(dim3((d.N + 7) / 8), dim3(256), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_gemv_generic, P);
+}
+
+// The GEMV kernels of a group whose activation is in `act`: the ring kernel when the group fits it, else one kernel per matrix.
+// pdl: the flag of the next launch; every launch made here sets it for the one after.  start (optional): recorded in front of the
+// first kernel, then cleared.
+static int gemv_kernels(const GemvDesc * d, int nmat, int K, const ActQ & act, cudaStream_t stream, bool & pdl, uint64_t & nlaunch,
+                        cudaEvent_t & start) {
+    if (start) {
+        const cudaError_t e = cudaEventRecord(start, stream);
+        if (e != cudaSuccess) return (int) e;
+        start = nullptr;
+    }
+    GemvPlan pl;
+    if (gemv_plan(d, nmat, K, pl)) {
+        const int e = launch_ring(d, nmat, K, act, pl, GemvPrologue{}, stream, pdl);
+        if (e) return e;
+        nlaunch++;
+        pdl = true;
+        return 0;
+    }
+    for (int i = 0; i < nmat; i++) {
+        int e;
+        // gemv_plan takes a Q8_0 / Q5_1 matrix only on its own: each of a group of them still gets the ring when it fits
+        if (is_blk32(d[i].type) && gemv_plan(&d[i], 1, K, pl)) e = launch_ring(&d[i], 1, K, act, pl, GemvPrologue{}, stream, pdl);
+        else if (blk32_ok(d[i], K)) e = launch_gemv_blk32(d[i], K, act, stream, pdl);
+        else e = launch_gemv_generic(d[i], K, act, stream, pdl);
+        if (e) return e;
+        nlaunch++;
+        pdl = true;
+    }
+    return 0;
+}
+
+int launch_gemv(const GemvDesc * d, int nmat, int K, const ActQ & act, const GemvPrologue & pro, cudaStream_t stream, bool pdl, uint64_t & nlaunch,
+                cudaEvent_t start) {
+    if (nmat < 1 || nmat > GEMV_MAX_MAT || K <= 0) return (int) cudaErrorInvalidValue;
+    if (pro.kind != PRO_NONE && !pro.in0) return (int) cudaErrorInvalidValue;
+    bool kq = true;
+    for (int i = 0; i < nmat; i++) kq = kq && is_kquant(d[i].type);
+    // 1. the activation inside the ring kernel: each CTA quantizes its share, one grid barrier (the ring plan implies gemv_fused_prologue_ok)
+    GemvPlan pl;
+    if ((pro.kind == PRO_RMSNORM || pro.kind == PRO_SILU_MUL) && kq && pro.gbar && gemv_plan(d, nmat, K, pl) && gemv_dist_prologue_ok()) {
+        if (start) {
+            const cudaError_t e = cudaEventRecord(start, stream);
+            if (e != cudaSuccess) return (int) e;
+        }
+        const int e = launch_ring(d, nmat, K, act, pl, pro, stream, pdl);
+        if (e == 0) nlaunch++;
+        return e;
+    }
+    // 2. or a producer kernel in front: per activation mode the matrices need
+    int modes[GEMV_MAX_MAT], nmode = 0;
+    for (int i = 0; i < nmat; i++) {
+        const int m = act_mode_for(d[i].type);
+        if (std::find(modes, modes + nmode, m) == modes + nmode) modes[nmode++] = m;
+    }
+    int e = 0;
+    if (nmode == 1) {
+        if (pro.kind == PRO_QUANTIZE) e = launch_quantize_act(pro.in0, K, modes[0], act, stream, pdl);
+        else if (pro.kind == PRO_RMSNORM) e = launch_rmsnorm_quant(pro.in0, pro.in1, K, pro.eps, modes[0], act, nullptr, stream, pdl);
+        else if (pro.kind == PRO_SILU_MUL) e = launch_silu_mul_quant(pro.in0, pro.in1, K, modes[0], act, nullptr, stream, pdl);
+        if (e) return e;
+        if (pro.kind != PRO_NONE) { nlaunch++; pdl = true; }
+        return gemv_kernels(d, nmat, K, act, stream, pdl, nlaunch, start);
+    }
+    // several modes (e.g. a Q8_0 matrix beside k-quants): the f32 vector once, then per mode its quantization and that mode's matrices
+    const float * x = pro.in0;
+    if (pro.kind == PRO_RMSNORM && pro.f32) {
+        e = launch_rmsnorm_quant(pro.in0, pro.in1, K, pro.eps, ACT_Q8_K, ActQ{}, pro.f32, stream, pdl);
+        if (e) return e;
+        nlaunch++;
+        pdl = true;
+        x = pro.f32;
+    } else if (pro.kind != PRO_QUANTIZE) {
+        return (int) cudaErrorInvalidValue;   // one activation buffer cannot hold several modes; no caller materialises silu(g) * u
+    }
+    for (int j = 0; j < nmode; j++) {
+        GemvDesc sub[GEMV_MAX_MAT];
+        int ns = 0;
+        for (int i = 0; i < nmat; i++)
+            if (act_mode_for(d[i].type) == modes[j]) sub[ns++] = d[i];
+        e = launch_quantize_act(x, K, modes[j], act, stream, pdl);
+        if (e) return e;
+        nlaunch++;
+        pdl = true;
+        e = gemv_kernels(sub, ns, K, act, stream, pdl, nlaunch, start);
+        if (e) return e;
+    }
+    return 0;
 }
 
 }  // namespace pb

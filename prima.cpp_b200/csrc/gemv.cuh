@@ -53,15 +53,13 @@ struct GemvMat {
     int tile0;             // index of this matrix' first tile in the launch-wide tile list
 };
 
-// Prologue: how the launch gets its q8_K activation.
+// Prologue (Prologue in launch.h): how the launch gets its q8_K activation.
 //   PRO_NONE          already quantized in HBM (`act`): one coalesced copy per CTA into shared memory, then registers
-//   PRO_RMSNORM_DIST  act = q8_K( rms_norm(in0) * in1 )     llm_build_norm + quantize_row_q8_K   (in1 = norm weight)
-//   PRO_SILU_DIST     act = q8_K( silu(in0) * in1 )         llm_build_ffn LLM_FFN_SILU / LLM_FFN_PAR -> ffn_down
-//   Distributed: CTA c quantizes super-block c into `act` (HBM/L2), ONE grid barrier (all CTAs of the persistent grid are
-//   co-resident), then every CTA stages the finished vector like PRO_NONE.  No tiny kernel + launch boundary in front of the GEMV,
-//   and each CTA quantizes one super-block instead of every CTA recomputing the whole vector from L2.
-enum : int { PRO_NONE = 0, PRO_RMSNORM_DIST = 4, PRO_SILU_DIST = 5 };
-
+//   PRO_RMSNORM       act = q8_K( rms_norm(in0) * in1 )     llm_build_norm + quantize_row_q8_K   (in1 = norm weight)
+//   PRO_SILU_MUL      act = q8_K( silu(in0) * in1 )         llm_build_ffn LLM_FFN_SILU / LLM_FFN_PAR -> ffn_down
+//   The last two are distributed: CTA c quantizes super-block c into `act` (HBM/L2), ONE grid barrier (all CTAs of the persistent
+//   grid are co-resident), then every CTA stages the finished vector like PRO_NONE.  No tiny kernel + launch boundary in front of the
+//   GEMV, and each CTA quantizes one super-block instead of every CTA recomputing the whole vector from L2.
 struct GemvParams {
     GemvMat mat[GEMV_MAX_MAT];
     int nmat;
@@ -71,10 +69,10 @@ struct GemvParams {
     int wpr;           // warps per row: 1, 2 or 4
     int nblk_p2;       // lanes per row: nblk rounded up to a power of two, at most 32.  Short rows (K <= 4096) put 32 / nblk_p2 rows in one warp
     int nstage;        // ring depth of this launch
-    int nstage_init;   // stages [nstage_init, nstage) overlay the activation staging area: they join the ring once the activation is in registers
+    int nstage_init;   // stages requested before griddepcontrol.wait; stages [nstage_init, nstage) overlay the activation staging area: they
+                       // join the ring once the activation is in registers
     int rel_count;     // warps that hand a stage back before it is refilled: all 8, or only its owners (owner_only)
     int owner_only;    // a stage is always consumed by the same warps: the others skip it entirely (no wait, no release)
-    int prefill;       // stages requested before griddepcontrol.wait; the other initial stages follow once the activation loads are out
     int stage_bytes;   // bytes reserved per stage (multiple of 128)
     ActQ act;          // q8_K activation (PRO_NONE)
     int prologue;

@@ -33,7 +33,6 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "launch.h"
@@ -45,6 +44,7 @@ constexpr int MMQ_BK = 64;
 constexpr int MMQ_BN_MAX = 128;   // token columns of a tile: 64 accumulator registers per consumer thread
 constexpr int MMQ_A_MAX = 4;      // expanded-weight stages: P.a_nst = 2 or 4 (a power of two) of 16 KB, chosen at launch from the shared-memory budget
 constexpr int MMQ_B_NST = 4;      // activation stages (L2 loads: the deep ring)
+constexpr int MMQ_MIN_UNITS = 8;  // smallest stream-K share of a CTA, in K groups
 constexpr int MMQ_MMA_WARPS = 8;  // two consumer warpgroups, 64 weight rows each
 constexpr int MMQ_DQ_WARPS = 8;   // expansion warps: 2 threads per weight row, 32 weights per thread and step
 constexpr int MMQ_DQ_WARP0 = MMQ_MMA_WARPS + 1;   // warp MMQ_MMA_WARPS = activation producer
@@ -486,8 +486,8 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
 // ---- activation rows -> q8_K (exactly as the CPU backend quantizes them) -> fp16, written in the tiled 128-byte-swizzle image wgmma reads ----
 // blk32: the weight type is Q8_0 / Q5_1, whose CPU dot quantizes the activation per 32 values (q8_0 / q8_1: d = amax / 127 stored
 // as f16, q = round-half-even(x * 127 / amax), quantize_row_q8_0 ggml-quants.c:943-1010) instead of per 256 (q8_K).
-// Fused producers of the activation (pre_kind): 1 = silu(x) * aux[t][k] (llm_build_ffn's SILU + MUL in front of ffn_down, the f32 product never
-// goes to HBM), 2 = rms_norm(x) * aux[k] (llm_build_norm in front of q|k|v and gate|up): the same arithmetic, rounding for rounding, as
+// Fused producers of the activation (pre_kind): PRO_SILU_MUL = silu(x) * aux[t][k] (llm_build_ffn's SILU + MUL in front of ffn_down, the f32
+// product never goes to HBM), PRO_RMSNORM = rms_norm(x) * aux[k] (llm_build_norm in front of q|k|v and gate|up): the same arithmetic, rounding for rounding, as
 // k_silu_mul / k_rms_norm_rows followed by the plain pass.
 __device__ __forceinline__ float mmq_silu(float x) { return __fdiv_rn(x, 1.0f + expf(-x)); }   // ggml.c:2560
 __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, int64_t ldx, int T, int K, int BN, uint8_t * __restrict__ out,
@@ -497,7 +497,7 @@ __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, 
     const int t = blockIdx.x;                       // 0 .. Tpad-1
     const int b_bytes = BN * 128;
     float nscale = 1.f;
-    if (pre_kind == 2 && t < T) {                   // k_rms_norm_rows' sum, in its order (ggml.c:11950-11996: double-precision sum of squares)
+    if (pre_kind == PRO_RMSNORM && t < T) {                   // k_rms_norm_rows' sum, in its order (ggml.c:11950-11996: double-precision sum of squares)
         __shared__ double red[8];
         __shared__ float s_scale;
         const float * xr = x + (size_t) t * ldx;
@@ -523,11 +523,11 @@ __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, 
             const float4 a = p[0], c = p[1];
             v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = c.x; v[5] = c.y; v[6] = c.z; v[7] = c.w;
             if (pre_kind) {
-                const float4 * q = reinterpret_cast<const float4 *>(aux + (pre_kind == 1 ? (size_t) t * ld_aux : (size_t) 0) + (size_t) b * 256 + lane * 8);
+                const float4 * q = reinterpret_cast<const float4 *>(aux + (pre_kind == PRO_SILU_MUL ? (size_t) t * ld_aux : (size_t) 0) + (size_t) b * 256 + lane * 8);
                 const float4 e = q[0], f = q[1];
                 const float w[8] = {e.x, e.y, e.z, e.w, f.x, f.y, f.z, f.w};
 #pragma unroll
-                for (int i = 0; i < 8; i++) v[i] = pre_kind == 1 ? __fmul_rn(mmq_silu(v[i]), w[i]) : __fmul_rn(__fmul_rn(v[i], nscale), w[i]);
+                for (int i = 0; i < 8; i++) v[i] = pre_kind == PRO_SILU_MUL ? __fmul_rn(mmq_silu(v[i]), w[i]) : __fmul_rn(__fmul_rn(v[i], nscale), w[i]);
             }
         } else {
 #pragma unroll
@@ -618,7 +618,7 @@ static cudaError_t mmq_launch_typed(const MmqParams & P, int bn, dim3 grid, size
 
 cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const float * x, int64_t ldx, int64_t T, float * dst, const float * bias,
                        const float * resid, void * ws, cudaStream_t st, bool reuse_prep, const MmqPre * pre) {
-    if (pre && pre->kind != 0 && (!pre->aux || K % 256 != 0 || pre->kind < 0 || pre->kind > 2)) return cudaErrorInvalidValue;
+    if (pre && pre->kind != PRO_NONE && (!pre->aux || K % 256 != 0 || (pre->kind != PRO_RMSNORM && pre->kind != PRO_SILU_MUL))) return cudaErrorInvalidValue;
     if (!mmq_supported(type, K) || N <= 0 || T <= 0) return cudaErrorInvalidValue;
     const int BN = mmq_pick_bn((int) T);
     const int tpad = (int) ((T + BN - 1) / BN * BN);
@@ -643,20 +643,17 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
     P.ngrp = (int) ((K / MMQ_BK + 3) / 4);
     // stream-K: the tiles' K groups, tile after tile, in equal contiguous shares; a share is at least MMQ_MIN_UNITS groups (a segment's
     // pipeline fill + epilogue must stay small against its MMA steps) unless the whole launch is smaller than that
-    static const int min_units = getenv("PB200_MMQ_MIN_UNITS") ? std::max(1, atoi(getenv("PB200_MMQ_MIN_UNITS"))) : 8;
-    static const bool whole_tiles = getenv("PB200_MMQ_WHOLE_TILES") != nullptr;   // A/B: one tile per CTA (no split, no atomics)
     const int64_t total = (int64_t) P.rtiles * ttiles * P.ngrp;
     if (total > 0x7fffffff) return cudaErrorInvalidValue;
     P.total_units = (int) total;
     const int nsm = sm_count();                // CTAs that can be resident: one CTA per SM
     int upc = (int) ((total + nsm - 1) / nsm);
-    upc = std::max(upc, std::min(min_units, P.ngrp));
-    if (whole_tiles) upc = P.ngrp;
+    upc = std::max(upc, std::min(MMQ_MIN_UNITS, P.ngrp));
     P.upc = upc;
     const int grid_x = (int) ((total + upc - 1) / upc);
     const bool split = upc % P.ngrp != 0;      // some tile is shared by two CTAs: partial results meet in dst by atomic add
     if (!reuse_prep) {
-        k_mmq_prep<<<tpad, 256, 0, st>>>(x, ldx, (int) T, (int) K, BN, (uint8_t *) ws, is_kquant(type) ? 0 : 1, pre ? pre->kind : 0,
+        k_mmq_prep<<<tpad, 256, 0, st>>>(x, ldx, (int) T, (int) K, BN, (uint8_t *) ws, is_kquant(type) ? 0 : 1, pre ? pre->kind : PRO_NONE,
                                          pre ? pre->aux : nullptr, pre ? pre->ld_aux : 0, pre ? pre->eps : 0.f);
         cudaError_t e0 = cudaGetLastError();
         if (e0 != cudaSuccess) return e0;
@@ -668,12 +665,10 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
     auto smem_for = [&](int nraw, int b_nst) {
         return 1024 + (size_t) P.a_nst * MMQ_A_BYTES + (size_t) b_nst * BN * 128 + (size_t) nraw * MMQ_BM * P.slot + MMQ_CTL_BYTES;
     };
-    // 2 expanded-weight stages (4 on request), 3 raw slots if they fit, then as many activation stages (2..4) as the 227 KB budget leaves
-    static const int force_a = getenv("PB200_MMQ_A_NST") ? atoi(getenv("PB200_MMQ_A_NST")) : 0;
-    P.a_nst = force_a == 4 ? 4 : 2;
+    // 2 expanded-weight stages, 3 raw slots if they fit, then as many activation stages (2..4) as the 227 KB budget leaves
+    P.a_nst = 2;
     P.nraw = 3;
     if (smem_for(3, 2) > 232448) P.nraw = 2;
-    if (smem_for(P.nraw, 2) > 232448) P.a_nst = 2;
     P.b_nst = MMQ_B_NST;
     while (P.b_nst > 2 && smem_for(P.nraw, P.b_nst) > 232448) P.b_nst--;
     const size_t smem = smem_for(P.nraw, P.b_nst);

@@ -12,20 +12,6 @@
 
 namespace pb {
 
-static inline int launch_cfg(cudaLaunchConfig_t & cfg, cudaLaunchAttribute * attr, dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                             bool pdl) {
-    cfg = cudaLaunchConfig_t{};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return 0;
-}
-
 // ------------------------------------------------------------------------------------------------
 // activation quantization: one warp per 256 values
 __global__ void __launch_bounds__(256) k_quantize_act(const float * __restrict__ x, int K, int mode, ActQ out) {
@@ -199,46 +185,6 @@ __global__ void __launch_bounds__(256) k_rms_norm_rows(const float * __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------
-// RoPE (ggml.c:14087-14266).  theta for pair i is pos * theta_scale^i computed by i sequential fp32 multiplies, exactly
-// like ggml_rope_cache_init's running product, so the angle is bit-identical to the CPU's.
-// grid = n_head + n_head_kv CTAs of D/2 threads: q heads rotate in place; k heads rotate into the f16 K cache and carry
-// the matching v head into the f16 V cache.
-__global__ void k_rope_kvstore(float * __restrict__ q, const float * __restrict__ k, const float * __restrict__ v, __half * __restrict__ kc,
-                               __half * __restrict__ vc, int n_head, int n_head_kv, int D, const int32_t * __restrict__ pos_dev, RopeParams rp,
-                               const float * __restrict__ freq_factors) {
-    pdl_trigger();   // dependents may launch now; they still wait for this grid's completion in their own pdl_wait()
-    pdl_wait();
-    const int32_t pos = *pos_dev;
-    const int h = blockIdx.x, pair = threadIdx.x;
-    const int half_dims = rp.n_dims / 2;
-    const bool neox = rp.mode & 2;
-    float c = 1.f, s = 0.f;
-    if (pair < half_dims) rope_cos_sin(rp, pos, pair, freq_factors, c, s);
-    const int i0 = neox ? pair : 2 * pair, i1 = neox ? pair + half_dims : 2 * pair + 1;
-    if (h < n_head) {
-        if (pair < half_dims) {
-            float * x = q + (int64_t) h * D;
-            float y0, y1;
-            rope_rotate(x[i0], x[i1], c, s, y0, y1);
-            x[i0] = y0; x[i1] = y1;
-        }
-    } else {
-        const int hk = h - n_head;
-        const int64_t EK = (int64_t) n_head_kv * D;
-        const float * x = k + (int64_t) hk * D;
-        __half * kd = kc + (int64_t) pos * EK + (int64_t) hk * D;
-        __half * vd = vc + (int64_t) pos * EK + (int64_t) hk * D;
-        const float * vs = v + (int64_t) hk * D;
-        if (pair < half_dims) {
-            float y0, y1;
-            rope_rotate(x[i0], x[i1], c, s, y0, y1);
-            kd[i0] = __float2half_rn(y0); kd[i1] = __float2half_rn(y1);
-        }
-        for (int i = rp.n_dims + pair; i < D; i += blockDim.x) kd[i] = __float2half_rn(x[i]);   // un-rotated tail (n_dims < D)
-        for (int i = pair; i < D; i += blockDim.x) vd[i] = __float2half_rn(vs[i]);
-    }
-}
-
 // generic rope for the plugin: one CTA per (token, head)
 __global__ void k_rope(const float * __restrict__ x, float * __restrict__ y, int n_head, int D, int64_t tok_stride, int64_t head_stride,
                        const int32_t * __restrict__ pos, RopeParams rp, const float * __restrict__ freq_factors) {
@@ -468,8 +414,8 @@ __global__ void __launch_bounds__(256) k_attn_prefill_tiled(const float * __rest
 }
 
 // ------------------------------------------------------------------------------------------------
-// Fused RoPE + KV store + decode attention: one CTA (8 warps) per q head.  Replaces k_rope_kvstore + k_attn_decode in the
-// engine's per-token loop (same arithmetic, one launch): the CTA rotates its q head and its kv head's k in shared memory,
+// Fused RoPE + KV store + decode attention: one CTA (8 warps) per q head.  RoPE (ggml.c:14087-14266), the f16 cache store and
+// k_attn_decode's arithmetic in one launch: the CTA rotates its q head and its kv head's k in shared memory,
 // rounds k / v to f16 exactly like the cache store does, attends over cache rows [0, pos) plus the fresh row from shared
 // memory, and the first q head of each GQA group writes the fresh K/V row to the cache for later tokens.
 __global__ void __launch_bounds__(256) k_attn_fused(const float * __restrict__ q, const float * __restrict__ k, const float * __restrict__ v,
@@ -1239,26 +1185,23 @@ int launch_mul_mat_f16(const void * A, const void * B, void * D, int64_t K, cons
 }
 
 int launch_quantize_act(const float * x, int K, int mode, const ActQ & out, cudaStream_t stream, bool pdl) {
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
     const int ngroups = (K + 255) / 256;
-    launch_cfg(cfg, attr, dim3((ngroups + 7) / 8), dim3(256), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_quantize_act, x, K, mode, out);
+    LaunchCfg lc(dim3((ngroups + 7) / 8), dim3(256), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_quantize_act, x, K, mode, out);
 }
 int launch_silu_mul_quant(const float * gate, const float * up, int K, int mode, const ActQ & out, float * f32_out, cudaStream_t stream, bool pdl) {
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
     const int ngroups = (K + 255) / 256;
-    launch_cfg(cfg, attr, dim3((ngroups + 7) / 8), dim3(256), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_silu_mul_quant, gate, up, K, mode, out, f32_out);
+    LaunchCfg lc(dim3((ngroups + 7) / 8), dim3(256), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_silu_mul_quant, gate, up, K, mode, out, f32_out);
 }
 int launch_rmsnorm_quant(const float * x, const float * w, int n, float eps, int mode, const ActQ & out, float * f32_out, cudaStream_t stream, bool pdl) {
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
     if (mode == ACT_Q8_K && w && !f32_out && out.qs && n % 256 == 0 && n / 256 <= RQ_WARPS * 4 && ((uintptr_t) x & 15) == 0 && ((uintptr_t) w & 15) == 0) {
-        launch_cfg(cfg, attr, dim3(1), dim3(RQ_WARPS * 32), 0, stream, pdl);
-        if (n / 256 <= RQ_WARPS * 2) return (int) cudaLaunchKernelEx(&cfg, k_rmsnorm_q8K<2>, x, w, n, eps, out);
-        return (int) cudaLaunchKernelEx(&cfg, k_rmsnorm_q8K<4>, x, w, n, eps, out);
+        LaunchCfg lc(dim3(1), dim3(RQ_WARPS * 32), 0, stream, pdl);
+        if (n / 256 <= RQ_WARPS * 2) return (int) cudaLaunchKernelEx(&lc.cfg, k_rmsnorm_q8K<2>, x, w, n, eps, out);
+        return (int) cudaLaunchKernelEx(&lc.cfg, k_rmsnorm_q8K<4>, x, w, n, eps, out);
     }
-    launch_cfg(cfg, attr, dim3(1), dim3(1024), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_rmsnorm_quant, x, w, n, eps, mode, out, f32_out);
+    LaunchCfg lc(dim3(1), dim3(1024), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_rmsnorm_quant, x, w, n, eps, mode, out, f32_out);
 }
 int launch_rms_norm(const float * x, float * y, int n, int64_t nrows, float eps, cudaStream_t stream, const float * w) {
     k_rms_norm_rows<<<(unsigned) nrows, 256, 0, stream>>>(x, y, n, eps, w);
@@ -1280,38 +1223,29 @@ void rope_params_init(RopeParams & rp, int n_dims, int mode, int n_ctx_orig, flo
     rp.corr_dims[1] = fminf((float) n_dims - 1, end);
 }
 
-int launch_rope_kvstore(float * q, const float * k, const float * v, __half * kcache, __half * vcache, int n_head, int n_head_kv, int D,
-                        const int32_t * pos_dev, const RopeParams & rp, const float * freq_factors, cudaStream_t stream, bool pdl) {
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, dim3(n_head + n_head_kv), dim3(D / 2), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_rope_kvstore, q, k, v, kcache, vcache, n_head, n_head_kv, D, pos_dev, rp, freq_factors);
-}
 int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int64_t tok_stride, int64_t head_stride, const int32_t * pos,
                 const RopeParams & rp, const float * freq_factors, cudaStream_t stream) {
     k_rope<<<(unsigned) (ntok * n_head), 64, 0, stream>>>(x, y, n_head, D, tok_stride, head_stride, pos, rp, freq_factors);
     return (int) cudaGetLastError();
 }
 
-int attn_scratch_floats(int, int) { return 0; }
 static FuncAttrCache g_attn_attr;
 int launch_attn_decode(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
-                       const int32_t * pos_dev, int n_ctx, float scale, float *, cudaStream_t stream, bool pdl) {
+                       const int32_t * pos_dev, int n_ctx, float scale, cudaStream_t stream, bool pdl) {
     if (D != 128) return (int) cudaErrorInvalidValue;
     const size_t smem = ((size_t) ((n_ctx + 31) & ~31) + 8 * 128) * sizeof(float);
     {
         cudaError_t e = ensure_dyn_smem(g_attn_attr, (const void *) k_attn_decode, smem, false);
         if (e != cudaSuccess) return (int) e;
     }
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, dim3(n_head), dim3(256), smem, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_attn_decode, q, kcache, vcache, out, n_head, n_head_kv, D, pos_dev, scale, (int64_t) 0, (int64_t) 0);
+    LaunchCfg lc(dim3(n_head), dim3(256), smem, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_decode, q, kcache, vcache, out, n_head, n_head_kv, D, pos_dev, scale, (int64_t) 0, (int64_t) 0);
 }
 // prefill: n_tok query rows (strides in floats), token t attends to cache rows [0, pos_dev[t]]
 int launch_attn_batch(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
                       const int32_t * pos_dev, int n_tok, int n_kv_max, float scale, cudaStream_t stream) {
     if (D != 128 || n_tok <= 0 || n_tok > 65535) return (int) cudaErrorInvalidValue;
-    static const int attn_mode = getenv("PB200_ATTN_MODE") ? atoi(getenv("PB200_ATTN_MODE")) : 0;   // A/B switch: 1 = the per-(head, token) grid of k_attn_decode
-    if (attn_mode == 0 && n_head % n_head_kv == 0) {   // tiled kernel: all score rows of gqa x TQ queries in shared memory
+    if (n_head % n_head_kv == 0) {   // tiled kernel: all score rows of gqa x TQ queries in shared memory
         const int gqa = n_head / n_head_kv;
         const int n_kv_pad = (n_kv_max + 31) & ~31;
         auto smem_for = [&](int tq) { return (size_t) gqa * tq * n_kv_pad * 4 + (size_t) gqa * tq * D * 4 + (size_t) ATT_TK * ATT_KSTRIDE * 2; };
@@ -1336,28 +1270,12 @@ int launch_attn_batch(const float * q, const __half * kcache, const __half * vca
         cudaError_t e = ensure_dyn_smem(g_attn_attr, (const void *) k_attn_decode, smem, false);
         if (e != cudaSuccess) return (int) e;
     }
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, dim3(n_head, n_tok), dim3(256), smem, stream, false);
-    return (int) cudaLaunchKernelEx(&cfg, k_attn_decode, q, kcache, vcache, out, n_head, n_head_kv, D, pos_dev, scale, (int64_t) n_head * D,
+    LaunchCfg lc(dim3(n_head, n_tok), dim3(256), smem, stream, false);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_decode, q, kcache, vcache, out, n_head, n_head_kv, D, pos_dev, scale, (int64_t) n_head * D,
                                     (int64_t) n_head * D);
 }
 
-static FuncAttrCache g_attnf_attr;
-int launch_attn_fused(const float * q, const float * k, const float * v, __half * kcache, __half * vcache, float * out, int n_head, int n_head_kv,
-                      int D, const int32_t * pos_dev, int n_ctx, const RopeParams & rp, const float * freq_factors, float scale, cudaStream_t stream,
-                      bool pdl) {
-    if (D != 128) return (int) cudaErrorInvalidValue;
-    const size_t smem = ((size_t) ((n_ctx + 31) & ~31) + 8 * 128) * sizeof(float);
-    {
-        cudaError_t e = ensure_dyn_smem(g_attnf_attr, (const void *) k_attn_fused, smem, false);
-        if (e != cudaSuccess) return (int) e;
-    }
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, dim3(n_head), dim3(256), smem, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_attn_fused, q, k, v, kcache, vcache, out, n_head, n_head_kv, pos_dev, rp, freq_factors, scale);
-}
-
-// v2: returns cudaErrorNotSupported when the shape is outside what the clustered kernel handles (caller uses launch_attn_fused + a quantize kernel)
+// k_attn2: cudaErrorNotSupported for shapes the clustered kernel does not take (odd n_head, scores beyond its shared memory)
 template <bool GGML>
 static int launch_attn2(Attn2Params & P, int n_score_slots, cudaStream_t stream, bool pdl) {
     const size_t smem = sizeof(Attn2Smem) + (size_t) ((n_score_slots + 31) & ~31) * sizeof(float);
@@ -1368,28 +1286,33 @@ static int launch_attn2(Attn2Params & P, int n_score_slots, cudaStream_t stream,
         if (e != cudaSuccess) return (int) e;
     }
     P.abort_flag = abort_flag();
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(P.n_head);
-    cfg.blockDim = dim3(A2_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    attr[1].id = cudaLaunchAttributeClusterDimension;
-    attr[1].val.clusterDim.x = 2; attr[1].val.clusterDim.y = 1; attr[1].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
-    return (int) cudaLaunchKernelEx(&cfg, k_attn2<GGML>, P);
+    LaunchCfg lc(dim3(P.n_head), dim3(A2_THREADS), smem, stream, pdl, 2);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn2<GGML>, P);
 }
-int launch_attn_fused2(const float * q, const float * k, const float * v, __half * kcache, __half * vcache, float * out, const ActQ & outq, int n_head,
-                       int n_head_kv, int D, const int32_t * pos_dev, int n_ctx, const RopeParams & rp, const float * freq_factors, float scale,
-                       cudaStream_t stream, bool pdl) {
-    if (D != 128) return (int) cudaErrorNotSupported;
-    Attn2Params P{};
-    P.q = q; P.k = k; P.v = v; P.kc = kcache; P.vc = vcache; P.out = out; P.outq = outq; P.n_head = n_head; P.n_head_kv = n_head_kv;
-    P.pos_dev = pos_dev; P.rp = rp; P.freq_factors = freq_factors; P.scale = scale;
-    return launch_attn2<false>(P, n_ctx, stream, pdl);
+int launch_attn_step(const float * q, const float * k, const float * v, __half * kcache, __half * vcache, float * out, const ActQ & outq,
+                     int outq_mode, int n_head, int n_head_kv, int D, const int32_t * pos_dev, int n_ctx, const RopeParams & rp,
+                     const float * freq_factors, float scale, cudaStream_t stream, bool pdl, bool & quantized) {
+    quantized = false;
+    if (D != 128) return (int) cudaErrorInvalidValue;
+    // k_attn2 when the output feeds a q8_K GEMV whose ring kernel can stage it
+    if (outq_mode == ACT_Q8_K && gemv_fused_prologue_ok(n_head * D)) {
+        Attn2Params P{};
+        P.q = q; P.k = k; P.v = v; P.kc = kcache; P.vc = vcache; P.out = out; P.outq = outq; P.n_head = n_head; P.n_head_kv = n_head_kv;
+        P.pos_dev = pos_dev; P.rp = rp; P.freq_factors = freq_factors; P.scale = scale;
+        const int rc = launch_attn2<false>(P, n_ctx, stream, pdl);
+        if (rc != (int) cudaErrorNotSupported) {
+            quantized = rc == 0;
+            return rc;
+        }
+    }
+    static FuncAttrCache attr_cache;
+    const size_t smem = ((size_t) ((n_ctx + 31) & ~31) + 8 * 128) * sizeof(float);
+    {
+        cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_attn_fused, smem, false);
+        if (e != cudaSuccess) return (int) e;
+    }
+    LaunchCfg lc(dim3(n_head), dim3(256), smem, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_fused, q, k, v, kcache, vcache, out, n_head, n_head_kv, pos_dev, rp, freq_factors, scale);
 }
 // the reference graph's tensors (FA off): K cache rows, transposed V cache, explicit mask row and destination cell
 int launch_attn_ggml(const float * q, const float * k, const float * v, __half * kcache, __half * vcache_t, int64_t vt_stride, float * out, const ActQ & outq,
@@ -1435,9 +1358,8 @@ int launch_soft_max(const float * x, const float * mask, float * y, int ncols, i
 }
 
 int launch_get_rows(const void * table, int type, int K, const int32_t * ids, int n_ids, float * y, cudaStream_t stream, bool pdl) {
-    cudaLaunchConfig_t cfg; cudaLaunchAttribute attr[1];
-    launch_cfg(cfg, attr, dim3((K + 255) / 256, n_ids), dim3(256), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&cfg, k_get_rows, (const uint8_t *) table, type, K, row_bytes(type, K), ids, y);
+    LaunchCfg lc(dim3((K + 255) / 256, n_ids), dim3(256), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_get_rows, (const uint8_t *) table, type, K, row_bytes(type, K), ids, y);
 }
 
 int launch_binary(int op, const float * a, const float * b, float * y, int64_t n, int64_t nb, cudaStream_t stream) {
@@ -1455,17 +1377,6 @@ int launch_silu_mul(const float * g, const float * u, float * y, int64_t n, cuda
 int launch_cpy_f32_f16(const float * x, __half * y, int64_t n, cudaStream_t stream) {
     k_cpy_f32_f16<<<(unsigned) ((n + 255) / 256), 256, 0, stream>>>(x, y, n);
     return (int) cudaGetLastError();
-}
-
-int launch_gemv(const GemvDesc * d, int nmat, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
-    bool allk = true;
-    for (int i = 0; i < nmat; i++) allk = allk && is_kquant(d[i].type);
-    if (allk) return launch_gemv_kquant(d, nmat, K, act, stream, pdl);
-    for (int i = 0; i < nmat; i++) {
-        int e = launch_gemv_generic(d[i], K, act, stream, pdl);
-        if (e) return e;
-    }
-    return 0;
 }
 
 }  // namespace pb

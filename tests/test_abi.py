@@ -38,6 +38,9 @@ def test_argument_validation_no_gpu(lib, pkg):
     c = lib.c
     assert c.pb200_quantize_act(12, None, 256, None, None) == -1
     assert c.pb200_mul_mat_vec_q(3, None, 1, 256, None, None, None, None, None) == -1
+    # matrices that need different activation formats (q8_K for Q4_K, q8_0 for Q8_0) cannot share one activation
+    fake = (C.c_void_p * 2)(256, 512)
+    assert c.pb200_mul_mat_vec_fused(2, (C.c_int * 2)(12, 8), fake, (C.c_int64 * 2)(16, 16), 256, C.c_void_p(1024), fake, None) == -1
     hp = pkg.HParams(n_layer=2, n_embd=250, n_head=2, n_head_kv=1, head_dim=128, n_ff=512, n_vocab=100, n_ctx=16, rope_mode=0,
                      n_ctx_orig=8192, rope_freq_base=5e5, rope_freq_scale=1.0, rms_eps=1e-5)
     assert not c.pb200_model_create(C.byref(hp), 0, 0, 2, 1, 1)   # n_embd % 256 != 0 -> NULL, no abort
