@@ -102,6 +102,27 @@ __device__ __forceinline__ double warp_sum_d(double v) {
     return v;
 }
 
+// First-occurrence arg-max, the CPU backend's rule (its loops compare with a strict '>'): a larger key wins, an equal key keeps the
+// smaller index.  Folds the candidate (okey, oidx) into (key, idx); the optional payload *val travels with the winner.  Every
+// arg-max that must agree bit for bit with the CPU (the q8_K scale, greedy sampling) decides here.
+__device__ __forceinline__ void argmax_combine(float & key, int & idx, float okey, int oidx, float * val = nullptr, float oval = 0.f) {
+    if (okey > key || (okey == key && oidx < idx)) {
+        key = okey;
+        idx = oidx;
+        if (val) *val = oval;
+    }
+}
+// the same over a warp: every lane ends with the warp's winner
+__device__ __forceinline__ void warp_argmax(float & key, int & idx, float * val = nullptr) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float okey = __shfl_xor_sync(0xffffffffu, key, o);
+        const float oval = val ? __shfl_xor_sync(0xffffffffu, *val, o) : 0.f;
+        const int oidx = __shfl_xor_sync(0xffffffffu, idx, o);
+        argmax_combine(key, idx, okey, oidx, val, oval);
+    }
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void * p) { return (uint32_t) __cvta_generic_to_shared(p); }
 
 // ---- mbarrier + bulk async copy (TMA 1-D, SASS UBLKCP) ----

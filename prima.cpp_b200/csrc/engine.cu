@@ -731,22 +731,12 @@ __global__ void __launch_bounds__(1024) k_argmax(const float * __restrict__ x, i
         if (v > best) { best = v; bi = i; }       // ascending i per thread: strict '>' keeps the first occurrence
     }
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-    }
+    warp_argmax(best, bi);
     if (lane == 0) { sv[warp] = best; si[warp] = bi; }
     __syncthreads();
     if (warp == 0) {
         best = sv[lane]; bi = si[lane];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
-        }
+        warp_argmax(best, bi);
         if (lane == 0) { *out = bi; if (out2) *out2 = bi; }
     }
 }

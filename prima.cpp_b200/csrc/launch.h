@@ -122,17 +122,18 @@ void rope_params_init(RopeParams & rp, int n_dims, int mode, int n_ctx_orig, flo
 int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int64_t tok_stride, int64_t head_stride, const int32_t * pos,
                 const RopeParams & rp, const float * freq_factors, cudaStream_t stream);
 
-// decode attention, FA-off numerics of the CPU backend (f16-rounded q and probabilities, f32 accumulation):
+// decode attention (k_attn_rows), FA-off numerics of the CPU backend (f16-rounded q and probabilities, f32 accumulation):
 //   out[h][:] = softmax(scale * K[0..n_kv) . q_h) . V   — GQA-aware, K/V read once per kv head.  n_kv = *pos_dev + 1.
 int launch_attn_decode(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
                        const int32_t * pos_dev, int n_ctx, float scale, cudaStream_t stream, bool pdl);
-// batched form for prompt processing: token t (q row t, out row t) attends to cache rows [0, pos_dev[t]]
+// batched form for prompt processing: token t (q row t, out row t) attends to cache rows [0, pos_dev[t]].  The tiled kernel when its
+// scores fit shared memory, else k_attn_rows per (head, token)
 int launch_attn_batch(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
                       const int32_t * pos_dev, int n_tok, int n_kv_max, float scale, cudaStream_t stream);
 // The engine's per-token attention, one launch: rope(q), rope(k) -> f16 K row, v -> f16 V row, cache store and attention.  When the
 // consumer of `out` wants it in mode ACT_Q8_K (outq_mode) and the shape allows, the clustered k_attn2 also writes that activation
-// into outq and `quantized` is set; otherwise (odd n_head, scores beyond its shared memory at long n_ctx, other modes) k_attn_fused
-// writes `out` only and `quantized` is cleared.
+// into outq and `quantized` is set; otherwise (odd n_head, scores beyond its shared memory at long n_ctx, other modes)
+// k_attn_rows<true> writes `out` only and `quantized` is cleared.
 int launch_attn_step(const float * q, const float * k, const float * v, __half * kcache, __half * vcache, float * out, const ActQ & outq,
                      int outq_mode, int n_head, int n_head_kv, int D, const int32_t * pos_dev, int n_ctx, const RopeParams & rp,
                      const float * freq_factors, float scale, cudaStream_t stream, bool pdl, bool & quantized);

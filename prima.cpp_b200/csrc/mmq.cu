@@ -540,13 +540,7 @@ __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, 
             const float ax = fabsf(v[i]);
             if (ax > amax) { amax = ax; vmax = v[i]; idx = lane * 8 + i; }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float oa = __shfl_xor_sync(0xffffffffu, amax, o);
-            const float ov = __shfl_xor_sync(0xffffffffu, vmax, o);
-            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-            if (oa > amax || (oa == amax && oi < idx)) { amax = oa; vmax = ov; idx = oi; }
-        }
+        warp_argmax(amax, idx, &vmax);
         uint32_t h[4] = {0u, 0u, 0u, 0u};
         if (blk32) {
             float am = 0.f;

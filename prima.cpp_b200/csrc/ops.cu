@@ -205,80 +205,168 @@ __global__ void k_rope(const float * __restrict__ x, float * __restrict__ y, int
 }
 
 // ------------------------------------------------------------------------------------------------
-// Decode attention, one CTA (8 warps) per q head.  D == 128 (4 values per lane).
-//   s[p] = sum_d f32(K16[p][d]) * f32(f16(q[d]))            (CPU: mul_mat with f16 src0 rounds src1 to f16, ggml.c:12445)
-//   w    = softmax(s * scale)                               (ggml.c:13783; double sum, p = e * float(1/sum))
-//   o[d] = sum_p f32(V16[p][d]) * f32(f16(w[p]))            (second mul_mat, probabilities rounded to f16)
-__global__ void __launch_bounds__(256) k_attn_decode(const float * __restrict__ q, const __half * __restrict__ kc, const __half * __restrict__ vc,
-                                                     float * __restrict__ out, int n_head, int n_head_kv, int D, const int32_t * __restrict__ pos_dev,
-                                                     float scale, int64_t q_tok_stride, int64_t out_tok_stride) {
-    extern __shared__ float sm[];   // S[n_kv_pad] | red[8][128]
-    pdl_trigger();   // dependents may launch now; they still wait for this grid's completion in their own pdl_wait()
-    pdl_wait();
-    // blockIdx.y = token of a batch (prefill): its own position, q row and out row; K/V rows [0, pos] are already in the cache
-    const int n_kv = pos_dev[blockIdx.y] + 1;
-    q += (int64_t) blockIdx.y * q_tok_stride;
-    out += (int64_t) blockIdx.y * out_tok_stride;
-    const int h = blockIdx.x, hk = h / (n_head / n_head_kv);
+// Softmax of one row S[0..n) in shared memory by a CTA of WARPS warps, in the order of the FA-off chain's CPU soft_max
+// (ggml.c:13783): per-thread strided fmaxf, warp max, thread 0 folds the warps in order; e = expf(s - max) written back in place
+// (MASKED: a -inf score gives 0); per-thread double sum, warp sum, thread 0 adds the warps in order.  Returns inv = float(1 / sum)
+// to every thread, S then holds e.  Every thread calls it; S may have been written by any of them.  red / redd hold WARPS values
+// and bc one, all in shared memory.
+template <int WARPS, bool MASKED>
+__device__ __forceinline__ float block_softmax(float * S, int n, float * red, double * redd, float * bc) {
+    constexpr int NT = WARPS * 32;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t EK = (int64_t) n_head_kv * D;
-    float * S = sm;
-    float * red = sm + ((n_kv + 31) & ~31);
-    __shared__ float s_red[8];
-    __shared__ double s_redd[8];
-    __shared__ float s_max, s_inv;
-
-    const float4 qv = *reinterpret_cast<const float4 *>(q + (int64_t) h * D + 4 * lane);
-    const float q0 = __half2float(__float2half_rn(qv.x)), q1 = __half2float(__float2half_rn(qv.y));
-    const float q2 = __half2float(__float2half_rn(qv.z)), q3 = __half2float(__float2half_rn(qv.w));
-    for (int p = warp; p < n_kv; p += 8) {
-        const uint2 kraw = *reinterpret_cast<const uint2 *>(kc + (int64_t) p * EK + (int64_t) hk * D + 4 * lane);
-        const float2 k01 = __half22float2(*reinterpret_cast<const __half2 *>(&kraw.x));
-        const float2 k23 = __half22float2(*reinterpret_cast<const __half2 *>(&kraw.y));
-        float s = k01.x * q0;
-        s = fmaf(k01.y, q1, s);
-        s = fmaf(k23.x, q2, s);
-        s = fmaf(k23.y, q3, s);
-        s = warp_sum(s);
-        if (lane == 0) S[p] = __fmul_rn(s, scale);
-    }
     __syncthreads();
-    // max
     float m = -INFINITY;
-    for (int p = threadIdx.x; p < n_kv; p += 256) m = fmaxf(m, S[p]);
+    for (int p = threadIdx.x; p < n; p += NT) m = fmaxf(m, S[p]);
     m = warp_max(m);
-    if (lane == 0) s_red[warp] = m;
+    if (lane == 0) red[warp] = m;
     __syncthreads();
     if (threadIdx.x == 0) {
-        float t = s_red[0];
-        for (int i = 1; i < 8; i++) t = fmaxf(t, s_red[i]);
-        s_max = t;
+        float t = red[0];
+        for (int i = 1; i < WARPS; i++) t = fmaxf(t, red[i]);
+        *bc = t;
     }
     __syncthreads();
-    const float mx = s_max;
+    const float mx = *bc;
     double dsum = 0.0;
-    for (int p = threadIdx.x; p < n_kv; p += 256) {
-        const float e = expf(__fsub_rn(S[p], mx));
+    for (int p = threadIdx.x; p < n; p += NT) {
+        const float s = S[p];
+        const float e = (MASKED && s == -INFINITY) ? 0.f : expf(__fsub_rn(s, mx));
         S[p] = e;
         dsum += (double) e;
     }
     dsum = warp_sum_d(dsum);
-    if (lane == 0) s_redd[warp] = dsum;
-    __syncthreads();
+    if (lane == 0) redd[warp] = dsum;
+    __syncthreads();   // also: every thread has read the max, bc is free
     if (threadIdx.x == 0) {
         double t = 0;
-        for (int i = 0; i < 8; i++) t += s_redd[i];
-        s_inv = (float) (1.0 / t);
+        for (int i = 0; i < WARPS; i++) t += redd[i];
+        *bc = (float) (1.0 / t);
     }
     __syncthreads();
-    const float inv = s_inv;
+    return *bc;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Attention over the engine's cache, one CTA (8 warps) per (q head, token).  D == 128 (4 values per lane).
+//   s[p] = sum_d f32(K16[p][d]) * f32(f16(q[d]))            (CPU: mul_mat with f16 src0 rounds src1 to f16, ggml.c:12445)
+//   w    = softmax(s * scale)                               (ggml.c:13783; double sum, p = e * float(1/sum))
+//   o[d] = sum_p f32(V16[p][d]) * f32(f16(w[p]))            (second mul_mat, probabilities rounded to f16)
+// Token blockIdx.y attends to cache rows [0, pos], pos = pos_dev[blockIdx.y]; its q and out rows are tok_stride floats after the
+// previous token's.  Warp w visits rows w, w + 8, ... in that order, four rows' loads in flight before any is used.
+// FRESH = false: q is already rotated and every row is in the cache.
+// FRESH = true (one token, pre-RoPE q / k / v of it): RoPE (ggml.c:14087-14266) of the CTA's q head and its kv head's k into shared
+// memory, k / v rounded to f16 exactly like the cache store; row pos is read from there, and the first q head of each GQA group
+// writes it to the cache for later tokens.
+template <bool FRESH>
+__global__ void __launch_bounds__(256) k_attn_rows(const float * __restrict__ q, const float * __restrict__ k, const float * __restrict__ v,
+                                                   __half * __restrict__ kc, __half * __restrict__ vc, float * __restrict__ out, int n_head,
+                                                   int n_head_kv, const int32_t * __restrict__ pos_dev, RopeParams rp,
+                                                   const float * __restrict__ freq_factors, float scale, int64_t tok_stride) {
+    constexpr int D = 128;
+    extern __shared__ float sm[];   // S[n_kv_pad] | red[8][128]
+    __shared__ float q_s[D];
+    __shared__ __align__(16) __half k_s[D];
+    __shared__ __align__(16) __half v_s[D];
+    __shared__ float s_red[8];
+    __shared__ double s_redd[8];
+    __shared__ float s_bc;
+    pdl_trigger();   // dependents may launch now; they still wait for this grid's completion in their own pdl_wait()
+    pdl_wait();
+    const int pos = pos_dev[blockIdx.y];
+    const int n_kv = pos + 1;
+    const int gqa = n_head / n_head_kv;
+    const int h = blockIdx.x, hk = h / gqa;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t EK = (int64_t) n_head_kv * D;
+    q += (int64_t) blockIdx.y * tok_stride + (int64_t) h * D;
+    out += (int64_t) blockIdx.y * tok_stride + (int64_t) h * D;
+    float * S = sm;
+    float * red = sm + ((n_kv + 31) & ~31);
+
+    float q0, q1, q2, q3;
+    if constexpr (FRESH) {
+        // RoPE: threads 0..63 rotate q (pair = tid), threads 64..127 rotate k, threads 128..255 convert v
+        const int half_dims = rp.n_dims / 2;
+        const bool neox = rp.mode & 2;
+        if (threadIdx.x < 128) {
+            const int pair = threadIdx.x & 63;
+            const bool is_q = threadIdx.x < 64;
+            const float * src = is_q ? q : k + (int64_t) hk * D;
+            if (pair < half_dims) {
+                float c, s;
+                rope_cos_sin(rp, pos, pair, freq_factors, c, s);
+                const int i0 = neox ? pair : 2 * pair, i1 = neox ? pair + half_dims : 2 * pair + 1;
+                float y0, y1;
+                rope_rotate(src[i0], src[i1], c, s, y0, y1);
+                if (is_q) { q_s[i0] = __half2float(__float2half_rn(y0)); q_s[i1] = __half2float(__float2half_rn(y1)); }
+                else { k_s[i0] = __float2half_rn(y0); k_s[i1] = __float2half_rn(y1); }
+            }
+            for (int i = rp.n_dims + pair; i < D; i += 64) {   // un-rotated tail when n_dims < D
+                if (is_q) q_s[i] = __half2float(__float2half_rn(src[i]));
+                else k_s[i] = __float2half_rn(src[i]);
+            }
+        } else {
+            const int i = threadIdx.x - 128;
+            v_s[i] = __float2half_rn(v[(int64_t) hk * D + i]);
+        }
+        __syncthreads();
+        if (h % gqa == 0 && threadIdx.x < 32) {   // one CTA per kv head publishes the fresh row (8 B per lane, coalesced)
+            *reinterpret_cast<uint2 *>(kc + (int64_t) pos * EK + (int64_t) hk * D + 4 * lane) = *reinterpret_cast<const uint2 *>(k_s + 4 * lane);
+            *reinterpret_cast<uint2 *>(vc + (int64_t) pos * EK + (int64_t) hk * D + 4 * lane) = *reinterpret_cast<const uint2 *>(v_s + 4 * lane);
+        }
+        q0 = q_s[4 * lane]; q1 = q_s[4 * lane + 1]; q2 = q_s[4 * lane + 2]; q3 = q_s[4 * lane + 3];
+    } else {
+        const float4 qv = *reinterpret_cast<const float4 *>(q + 4 * lane);
+        q0 = __half2float(__float2half_rn(qv.x)); q1 = __half2float(__float2half_rn(qv.y));
+        q2 = __half2float(__float2half_rn(qv.z)); q3 = __half2float(__float2half_rn(qv.w));
+    }
+    for (int p0 = warp; p0 < n_kv; p0 += 32) {     // 4 positions per warp in flight: all K rows requested before any is used
+        uint2 kraw[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int p = p0 + 8 * j;
+            if (p < n_kv) {
+                const __half * krow = FRESH && p == pos ? k_s : kc + (int64_t) p * EK + (int64_t) hk * D;
+                kraw[j] = *reinterpret_cast<const uint2 *>(krow + 4 * lane);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int p = p0 + 8 * j;
+            if (p < n_kv) {
+                const float2 k01 = __half22float2(*reinterpret_cast<const __half2 *>(&kraw[j].x));
+                const float2 k23 = __half22float2(*reinterpret_cast<const __half2 *>(&kraw[j].y));
+                float s = k01.x * q0;
+                s = fmaf(k01.y, q1, s);
+                s = fmaf(k23.x, q2, s);
+                s = fmaf(k23.y, q3, s);
+                s = warp_sum(s);
+                if (lane == 0) S[p] = __fmul_rn(s, scale);
+            }
+        }
+    }
+    const float inv = block_softmax<8, false>(S, n_kv, s_red, s_redd, &s_bc);
     float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-    for (int p = warp; p < n_kv; p += 8) {
-        const float w = __half2float(__float2half_rn(__fmul_rn(S[p], inv)));
-        const uint2 vraw = *reinterpret_cast<const uint2 *>(vc + (int64_t) p * EK + (int64_t) hk * D + 4 * lane);
-        const float2 v01 = __half22float2(*reinterpret_cast<const __half2 *>(&vraw.x));
-        const float2 v23 = __half22float2(*reinterpret_cast<const __half2 *>(&vraw.y));
-        a0 = fmaf(v01.x, w, a0); a1 = fmaf(v01.y, w, a1); a2 = fmaf(v23.x, w, a2); a3 = fmaf(v23.y, w, a3);
+    for (int p0 = warp; p0 < n_kv; p0 += 32) {
+        uint2 vraw[4];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int p = p0 + 8 * j;
+            if (p < n_kv) {
+                const __half * vrow = FRESH && p == pos ? v_s : vc + (int64_t) p * EK + (int64_t) hk * D;
+                vraw[j] = *reinterpret_cast<const uint2 *>(vrow + 4 * lane);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int p = p0 + 8 * j;
+            if (p < n_kv) {
+                const float w = __half2float(__float2half_rn(__fmul_rn(S[p], inv)));
+                const float2 v01 = __half22float2(*reinterpret_cast<const __half2 *>(&vraw[j].x));
+                const float2 v23 = __half22float2(*reinterpret_cast<const __half2 *>(&vraw[j].y));
+                a0 = fmaf(v01.x, w, a0); a1 = fmaf(v01.y, w, a1); a2 = fmaf(v23.x, w, a2); a3 = fmaf(v23.y, w, a3);
+            }
+        }
     }
     *reinterpret_cast<float4 *>(red + warp * 128 + 4 * lane) = make_float4(a0, a1, a2, a3);
     __syncthreads();
@@ -286,7 +374,7 @@ __global__ void __launch_bounds__(256) k_attn_decode(const float * __restrict__ 
         float t = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; i++) t += red[i * 128 + threadIdx.x];
-        out[(int64_t) h * D + threadIdx.x] = t;
+        out[threadIdx.x] = t;
     }
 }
 
@@ -414,152 +502,7 @@ __global__ void __launch_bounds__(256) k_attn_prefill_tiled(const float * __rest
 }
 
 // ------------------------------------------------------------------------------------------------
-// Fused RoPE + KV store + decode attention: one CTA (8 warps) per q head.  RoPE (ggml.c:14087-14266), the f16 cache store and
-// k_attn_decode's arithmetic in one launch: the CTA rotates its q head and its kv head's k in shared memory,
-// rounds k / v to f16 exactly like the cache store does, attends over cache rows [0, pos) plus the fresh row from shared
-// memory, and the first q head of each GQA group writes the fresh K/V row to the cache for later tokens.
-__global__ void __launch_bounds__(256) k_attn_fused(const float * __restrict__ q, const float * __restrict__ k, const float * __restrict__ v,
-                                                    __half * __restrict__ kc, __half * __restrict__ vc, float * __restrict__ out, int n_head,
-                                                    int n_head_kv, const int32_t * __restrict__ pos_dev, RopeParams rp,
-                                                    const float * __restrict__ freq_factors, float scale) {
-    constexpr int D = 128;
-    extern __shared__ float sm[];   // S[n_kv_pad] | red[8][128]
-    __shared__ float q_s[D];
-    __shared__ __align__(16) __half k_s[D];
-    __shared__ __align__(16) __half v_s[D];
-    __shared__ float s_red[8];
-    __shared__ double s_redd[8];
-    __shared__ float s_max, s_inv;
-    pdl_trigger();
-    pdl_wait();
-    const int pos = *pos_dev;
-    const int n_kv = pos + 1;
-    const int gqa = n_head / n_head_kv;
-    const int h = blockIdx.x, hk = h / gqa;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t EK = (int64_t) n_head_kv * D;
-    float * S = sm;
-    float * red = sm + ((n_kv + 31) & ~31);
-
-    {   // RoPE: threads 0..63 rotate q (pair = tid), threads 64..127 rotate k, threads 128..255 convert v
-        const int half_dims = rp.n_dims / 2;
-        const bool neox = rp.mode & 2;
-        if (threadIdx.x < 128) {
-            const int pair = threadIdx.x & 63;
-            const bool is_q = threadIdx.x < 64;
-            const float * src = is_q ? q + (int64_t) h * D : k + (int64_t) hk * D;
-            if (pair < half_dims) {
-                float c, s;
-                rope_cos_sin(rp, pos, pair, freq_factors, c, s);
-                const int i0 = neox ? pair : 2 * pair, i1 = neox ? pair + half_dims : 2 * pair + 1;
-                float y0, y1;
-                rope_rotate(src[i0], src[i1], c, s, y0, y1);
-                if (is_q) { q_s[i0] = __half2float(__float2half_rn(y0)); q_s[i1] = __half2float(__float2half_rn(y1)); }
-                else { k_s[i0] = __float2half_rn(y0); k_s[i1] = __float2half_rn(y1); }
-            }
-            for (int i = rp.n_dims + pair; i < D; i += 64) {   // un-rotated tail when n_dims < D
-                if (is_q) q_s[i] = __half2float(__float2half_rn(src[i]));
-                else k_s[i] = __float2half_rn(src[i]);
-            }
-        } else {
-            const int i = threadIdx.x - 128;
-            v_s[i] = __float2half_rn(v[(int64_t) hk * D + i]);
-        }
-    }
-    __syncthreads();
-    if (h % gqa == 0 && threadIdx.x < 32) {   // one CTA per kv head publishes the fresh row (8 B per lane, coalesced)
-        *reinterpret_cast<uint2 *>(kc + (int64_t) pos * EK + (int64_t) hk * D + 4 * lane) = *reinterpret_cast<const uint2 *>(k_s + 4 * lane);
-        *reinterpret_cast<uint2 *>(vc + (int64_t) pos * EK + (int64_t) hk * D + 4 * lane) = *reinterpret_cast<const uint2 *>(v_s + 4 * lane);
-    }
-    const float q0 = q_s[4 * lane], q1 = q_s[4 * lane + 1], q2 = q_s[4 * lane + 2], q3 = q_s[4 * lane + 3];
-    for (int p0 = warp; p0 < n_kv; p0 += 32) {     // 4 positions per warp in flight: all K rows requested before any is used
-        uint2 kraw[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int p = p0 + 8 * j;
-            if (p < n_kv) {
-                const __half * krow = p == pos ? k_s : kc + (int64_t) p * EK + (int64_t) hk * D;
-                kraw[j] = *reinterpret_cast<const uint2 *>(krow + 4 * lane);
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int p = p0 + 8 * j;
-            if (p < n_kv) {
-                const float2 k01 = __half22float2(*reinterpret_cast<const __half2 *>(&kraw[j].x));
-                const float2 k23 = __half22float2(*reinterpret_cast<const __half2 *>(&kraw[j].y));
-                float s = k01.x * q0;
-                s = fmaf(k01.y, q1, s);
-                s = fmaf(k23.x, q2, s);
-                s = fmaf(k23.y, q3, s);
-                s = warp_sum(s);
-                if (lane == 0) S[p] = __fmul_rn(s, scale);
-            }
-        }
-    }
-    __syncthreads();
-    float m = -INFINITY;
-    for (int p = threadIdx.x; p < n_kv; p += 256) m = fmaxf(m, S[p]);
-    m = warp_max(m);
-    if (lane == 0) s_red[warp] = m;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float t = s_red[0];
-        for (int i = 1; i < 8; i++) t = fmaxf(t, s_red[i]);
-        s_max = t;
-    }
-    __syncthreads();
-    const float mx = s_max;
-    double dsum = 0.0;
-    for (int p = threadIdx.x; p < n_kv; p += 256) {
-        const float e = expf(__fsub_rn(S[p], mx));
-        S[p] = e;
-        dsum += (double) e;
-    }
-    dsum = warp_sum_d(dsum);
-    if (lane == 0) s_redd[warp] = dsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0;
-        for (int i = 0; i < 8; i++) t += s_redd[i];
-        s_inv = (float) (1.0 / t);
-    }
-    __syncthreads();
-    const float inv = s_inv;
-    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-    for (int p0 = warp; p0 < n_kv; p0 += 32) {
-        uint2 vraw[4];
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int p = p0 + 8 * j;
-            if (p < n_kv) {
-                const __half * vrow = p == pos ? v_s : vc + (int64_t) p * EK + (int64_t) hk * D;
-                vraw[j] = *reinterpret_cast<const uint2 *>(vrow + 4 * lane);
-            }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const int p = p0 + 8 * j;
-            if (p < n_kv) {
-                const float w = __half2float(__float2half_rn(__fmul_rn(S[p], inv)));
-                const float2 v01 = __half22float2(*reinterpret_cast<const __half2 *>(&vraw[j].x));
-                const float2 v23 = __half22float2(*reinterpret_cast<const __half2 *>(&vraw[j].y));
-                a0 = fmaf(v01.x, w, a0); a1 = fmaf(v01.y, w, a1); a2 = fmaf(v23.x, w, a2); a3 = fmaf(v23.y, w, a3);
-            }
-        }
-    }
-    *reinterpret_cast<float4 *>(red + warp * 128 + 4 * lane) = make_float4(a0, a1, a2, a3);
-    __syncthreads();
-    if (threadIdx.x < 128) {
-        float t = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; i++) t += red[i * 128 + threadIdx.x];
-        out[(int64_t) h * D + threadIdx.x] = t;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Decode attention v2 (the engine's per-token path): same arithmetic as k_attn_fused, restructured for LATENCY — under PDL this
+// Decode attention v2 (the engine's per-token path): same arithmetic as k_attn_rows<true>, restructured for LATENCY — under PDL this
 // kernel sits between the q|k|v GEMV and the wo GEMV, and every microsecond of it is a bubble in the weight stream:
 //   * one CTA of 16 warps per q head, launched as CLUSTERS OF 2 (heads 2j, 2j+1 = one 256-value q8_K super-block of the output):
 //     the pair agrees on the block's arg-max through distributed shared memory and writes the QUANTIZED activation itself,
@@ -573,7 +516,7 @@ constexpr int A2_THREADS = 512, A2_WARPS = 16, A2_CHUNK = 128;
 struct __align__(128) Attn2Smem {   // fixed part; dynamic tail: S[n_ctx padded to 32] floats
     uint64_t kbar[2], vbar[2];
     float cand[4];                 // this CTA's arg-max candidate {amax, vmax, idx, -} for the cluster exchange
-    float s_bc[3];
+    float s_bc;                    // block_softmax broadcast
     volatile int aborted;          // wait watchdog (common.cuh)
     float s_red[A2_WARPS];
     double s_redd[A2_WARPS];
@@ -767,37 +710,8 @@ __global__ void __launch_bounds__(A2_THREADS, 1) k_attn2(const __grid_constant__
             a2_issue_chunk(sm->kbuf[b], kc, EK, hk, c + 2, ncell, &sm->kbar[b]);
         }
     }
-    __syncthreads();
-    // ---- softmax (max, expf, double sum, p = e * float(1/sum))
-    float m = -INFINITY;
-    for (int p = threadIdx.x; p < ncell; p += A2_THREADS) m = fmaxf(m, S[p]);
-    m = warp_max(m);
-    if (lane == 0) sm->s_red[warp] = m;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        float t = sm->s_red[0];
-        for (int i = 1; i < A2_WARPS; i++) t = fmaxf(t, sm->s_red[i]);
-        sm->s_bc[0] = t;
-    }
-    __syncthreads();
-    const float mx = sm->s_bc[0];
-    double dsum = 0.0;
-    for (int p = threadIdx.x; p < ncell; p += A2_THREADS) {
-        const float sv = S[p];
-        const float e = (GGML && sv == -INFINITY) ? 0.f : expf(__fsub_rn(sv, mx));
-        S[p] = e;
-        dsum += (double) e;
-    }
-    dsum = warp_sum_d(dsum);
-    if (lane == 0) sm->s_redd[warp] = dsum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0;
-        for (int i = 0; i < A2_WARPS; i++) t += sm->s_redd[i];
-        sm->s_bc[1] = (float) (1.0 / t);
-    }
-    __syncthreads();
-    const float inv = sm->s_bc[1];
+    // ---- softmax (max, expf, double sum, p = e * float(1/sum)); the GGML mask's -inf cells get 0
+    const float inv = block_softmax<A2_WARPS, GGML>(S, ncell, sm->s_red, sm->s_redd, &sm->s_bc);
     if (GGML) {
         // ---- P.V over the transposed cache: warp w owns channels w, w+16, ...; lane l owns cells 2l, 2l+1, 64+2l, 64+2l+1 of a chunk
         for (int p = threadIdx.x; p < ncell; p += A2_THREADS) S[p] = __half2float(__float2half_rn(__fmul_rn(S[p], inv)));   // f16-rounded probabilities
@@ -884,19 +798,14 @@ __global__ void __launch_bounds__(A2_THREADS, 1) k_attn2(const __grid_constant__
                 const float ax = fabsf(xv[i]);
                 if (ax > amax) { amax = ax; vmax = xv[i]; idx = (int) rank * 128 + 4 * lane + i; }   // strict '>': first occurrence
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float oa = __shfl_xor_sync(0xffffffffu, amax, o), ov = __shfl_xor_sync(0xffffffffu, vmax, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-                if (oa > amax || (oa == amax && oi < idx)) { amax = oa; vmax = ov; idx = oi; }
-            }
+            warp_argmax(amax, idx, &vmax);
             if (lane == 0) { sm->cand[0] = amax; sm->cand[1] = vmax; sm->cand[2] = __int_as_float(idx); }
         }
         cluster_sync_all();
         if (warp == 0) {
             const float oa = ld_dsmem_f32(&sm->cand[0], rank ^ 1u), ov = ld_dsmem_f32(&sm->cand[1], rank ^ 1u);
             const int oi = __float_as_int(ld_dsmem_f32(&sm->cand[2], rank ^ 1u));
-            if (oa > amax || (oa == amax && oi < idx)) { amax = oa; vmax = ov; idx = oi; }
+            argmax_combine(amax, idx, oa, oi, &vmax, ov);
             const int64_t blk = h >> 1;
             uint32_t packed = 0u;
             int sum = 0;
@@ -934,33 +843,12 @@ __global__ void __launch_bounds__(256) k_soft_max(const float * __restrict__ x, 
     const float * xr = x + row * ncols;
     const float * mr = mask ? mask + (row % rows_per_mask_cycle) * ncols : nullptr;
     float * yr = y + row * ncols;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    float m = -INFINITY;
     for (int i = threadIdx.x; i < ncols; i += 256) {
         float v = __fmul_rn(xr[i], scale);
         if (mr) v = __fadd_rn(v, mr[i]);
         sm[i] = v;
-        m = fmaxf(m, v);
     }
-    m = warp_max(m);
-    if (lane == 0) s_red[warp] = m;
-    __syncthreads();
-    if (threadIdx.x == 0) { float t = s_red[0]; for (int i = 1; i < 8; i++) t = fmaxf(t, s_red[i]); s_b = t; }
-    __syncthreads();
-    const float mx = s_b;
-    double dsum = 0.0;
-    for (int i = threadIdx.x; i < ncols; i += 256) {
-        const float v = sm[i];
-        const float e = v == -INFINITY ? 0.f : expf(__fsub_rn(v, mx));
-        sm[i] = e;
-        dsum += (double) e;
-    }
-    dsum = warp_sum_d(dsum);
-    if (lane == 0) s_redd[warp] = dsum;
-    __syncthreads();
-    if (threadIdx.x == 0) { double t = 0; for (int i = 0; i < 8; i++) t += s_redd[i]; s_b = (float) (1.0 / t); }
-    __syncthreads();
-    const float inv = s_b;
+    const float inv = block_softmax<8, true>(sm, ncols, s_red, s_redd, &s_b);
     for (int i = threadIdx.x; i < ncols; i += 256) yr[i] = __fmul_rn(sm[i], inv);
 }
 
@@ -1229,17 +1117,26 @@ int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int
     return (int) cudaGetLastError();
 }
 
-static FuncAttrCache g_attn_attr;
+// k_attn_rows<FRESH> for n_head heads x n_tok tokens (q / out rows tok_stride floats apart), scores of up to n_kv_max cells
+template <bool FRESH>
+static int launch_attn_rows(const float * q, const float * k, const float * v, __half * kc, __half * vc, float * out, int n_head, int n_head_kv,
+                            const int32_t * pos_dev, const RopeParams & rp, const float * freq_factors, float scale, int n_tok, int64_t tok_stride,
+                            int n_kv_max, cudaStream_t stream, bool pdl) {
+    const size_t smem = ((size_t) ((n_kv_max + 31) & ~31) + 8 * 128) * sizeof(float);
+    static FuncAttrCache attr_cache;
+    {
+        cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_attn_rows<FRESH>, smem, false);
+        if (e != cudaSuccess) return (int) e;
+    }
+    LaunchCfg lc(dim3(n_head, n_tok), dim3(256), smem, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_rows<FRESH>, q, k, v, kc, vc, out, n_head, n_head_kv, pos_dev, rp, freq_factors, scale, tok_stride);
+}
+// k_attn_rows<false> only reads the caches
 int launch_attn_decode(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
                        const int32_t * pos_dev, int n_ctx, float scale, cudaStream_t stream, bool pdl) {
     if (D != 128) return (int) cudaErrorInvalidValue;
-    const size_t smem = ((size_t) ((n_ctx + 31) & ~31) + 8 * 128) * sizeof(float);
-    {
-        cudaError_t e = ensure_dyn_smem(g_attn_attr, (const void *) k_attn_decode, smem, false);
-        if (e != cudaSuccess) return (int) e;
-    }
-    LaunchCfg lc(dim3(n_head), dim3(256), smem, stream, pdl);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_decode, q, kcache, vcache, out, n_head, n_head_kv, D, pos_dev, scale, (int64_t) 0, (int64_t) 0);
+    return launch_attn_rows<false>(q, nullptr, nullptr, const_cast<__half *>(kcache), const_cast<__half *>(vcache), out, n_head, n_head_kv, pos_dev,
+                                   RopeParams{}, nullptr, scale, 1, 0, n_ctx, stream, pdl);
 }
 // prefill: n_tok query rows (strides in floats), token t attends to cache rows [0, pos_dev[t]]
 int launch_attn_batch(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
@@ -1265,14 +1162,8 @@ int launch_attn_batch(const float * q, const __half * kcache, const __half * vca
             return (int) cudaGetLastError();
         }
     }
-    const size_t smem = ((size_t) ((n_kv_max + 31) & ~31) + 8 * 128) * sizeof(float);
-    {
-        cudaError_t e = ensure_dyn_smem(g_attn_attr, (const void *) k_attn_decode, smem, false);
-        if (e != cudaSuccess) return (int) e;
-    }
-    LaunchCfg lc(dim3(n_head, n_tok), dim3(256), smem, stream, false);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_decode, q, kcache, vcache, out, n_head, n_head_kv, D, pos_dev, scale, (int64_t) n_head * D,
-                                    (int64_t) n_head * D);
+    return launch_attn_rows<false>(q, nullptr, nullptr, const_cast<__half *>(kcache), const_cast<__half *>(vcache), out, n_head, n_head_kv, pos_dev,
+                                   RopeParams{}, nullptr, scale, n_tok, (int64_t) n_head * D, n_kv_max, stream, false);
 }
 
 // k_attn2: cudaErrorNotSupported for shapes the clustered kernel does not take (odd n_head, scores beyond its shared memory)
@@ -1305,14 +1196,7 @@ int launch_attn_step(const float * q, const float * k, const float * v, __half *
             return rc;
         }
     }
-    static FuncAttrCache attr_cache;
-    const size_t smem = ((size_t) ((n_ctx + 31) & ~31) + 8 * 128) * sizeof(float);
-    {
-        cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_attn_fused, smem, false);
-        if (e != cudaSuccess) return (int) e;
-    }
-    LaunchCfg lc(dim3(n_head), dim3(256), smem, stream, pdl);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_attn_fused, q, k, v, kcache, vcache, out, n_head, n_head_kv, pos_dev, rp, freq_factors, scale);
+    return launch_attn_rows<true>(q, k, v, kcache, vcache, out, n_head, n_head_kv, pos_dev, rp, freq_factors, scale, 1, 0, n_ctx, stream, pdl);
 }
 // the reference graph's tensors (FA off): K cache rows, transposed V cache, explicit mask row and destination cell
 int launch_attn_ggml(const float * q, const float * k, const float * v, __half * kcache, __half * vcache_t, int64_t vt_stride, float * out, const ActQ & outq,

@@ -19,13 +19,7 @@ __device__ __forceinline__ void quantize_warp_q8K(const float (&v)[8], int lane,
         float ax = fabsf(v[i]);
         if (ax > amax) { amax = ax; vmax = v[i]; idx = lane * 8 + i; }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        float oa = __shfl_xor_sync(0xffffffffu, amax, o);
-        float ov = __shfl_xor_sync(0xffffffffu, vmax, o);
-        int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-        if (oa > amax || (oa == amax && oi < idx)) { amax = oa; vmax = ov; idx = oi; }
-    }
+    warp_argmax(amax, idx, &vmax);
     uint32_t packed[2] = {0u, 0u};
     int sum = 0;
     float d = 0.f;

@@ -1,5 +1,5 @@
 """-m gpu: the fallback rungs of the decode launchers, each against the oracle: attention past the clustered kernel's context
-limit (k_attn_fused + a quantize kernel in front of wo), the fused GEMV's producer kernel in front instead of the distributed
+limit (k_attn_rows<true> + a quantize kernel in front of wo), the fused GEMV's producer kernel in front instead of the distributed
 prologue, and the per-matrix GEMV kernels for weights the bulk-copy ring cannot read."""
 import ctypes as C
 
@@ -21,7 +21,7 @@ def rel_tol(ref, r=4e-6):
 
 def test_engine_long_context_attention_fallback(cuda, pkg, lib, port):
     """n_ctx 16384: the scores no longer fit k_attn2's shared memory (about 15k positions at head_dim 128), so every layer runs
-    k_attn_fused and quantizes wo's input in a kernel of its own: one launch per layer more than the same model at a short context."""
+    k_attn_rows<true> and quantizes wo's input in a kernel of its own: one launch per layer more than the same model at a short context."""
     kw = dict(n_layer=2, n_embd=512, n_head=4, n_head_kv=2, n_ff=1024, n_vocab=320, arch="llama", ftype="q4_K_M", seed=9, branch_scale=0.1)
     toks = [(i * 7919 + 13) % 320 for i in range(8)]
     launches = {}
