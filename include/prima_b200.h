@@ -103,7 +103,9 @@ PB200_API size_t pb200_mul_mat_q_workspace_bytes(int64_t k, int64_t t);
 PB200_API int pb200_mul_mat_q(int type, const void * W, int64_t n, int64_t k, const float * x, int64_t ldx, int64_t t, float * dst,
                               const float * bias, const float * resid, void * ws, void * stream);
 PB200_API int pb200_get_rows(int type, const void * table, int64_t k, const int32_t * ids, int64_t n_ids, float * y, void * stream);
-/* decode attention over an f16 KV cache laid out [n_ctx][n_head_kv*head_dim]; n_kv = *pos_dev + 1 */
+/* decode attention over an f16 KV cache laid out [n_ctx][n_head_kv*head_dim]; n_kv = *pos_dev + 1.  The kernel keeps a score row of
+ * n_ctx floats in shared memory: PB200_ENOTSUP when that exceeds the device's limit (n_ctx above 57 056 on an H100); likewise
+ * pb200_attn_prefill for n_kv_max. */
 PB200_API int pb200_attn_decode(const float * q, const void * k_cache_f16, const void * v_cache_f16, float * out, int n_head, int n_head_kv,
                                 int head_dim, const int32_t * pos_dev, int n_ctx, float scale, void * stream);
 /* prompt-processing attention: n_tok query rows q[t][n_head][head_dim]; token t attends to cache rows [0, pos_dev[t]] (its own
@@ -160,7 +162,9 @@ typedef struct pb200_hparams {
 typedef struct pb200_model pb200_model;
 
 /* layers [layer_begin, layer_end) live on this device (prima's layer window, src/llama.cpp:3838-3883);
- * with_embd / with_head: whether token_embd and output_norm+output live here (first / last pipeline stage) */
+ * with_embd / with_head: whether token_embd and output_norm+output live here (first / last pipeline stage).
+ * NULL for an n_ctx longer than the attention kernels can hold: beyond about 15k cells the decode step keeps a whole score row of
+ * n_ctx floats in shared memory, which limits n_ctx to 56 800 on an H100 (the device's opt-in shared memory per block). */
 PB200_API pb200_model * pb200_model_create(const pb200_hparams * hp, int device, int layer_begin, int layer_end, int with_embd, int with_head);
 PB200_API void          pb200_model_free(pb200_model * m);
 /* tensor names follow GGUF: "token_embd.weight", "output_norm.weight", "output.weight", "rope_freqs.weight",

@@ -197,9 +197,11 @@ int pb200_get_rows(int type, const void * table, int64_t k, const int32_t * ids,
 int pb200_attn_decode(const float * q, const void * k_cache_f16, const void * v_cache_f16, float * out, int n_head, int n_head_kv, int head_dim,
                       const int32_t * pos_dev, int n_ctx, float scale, void * stream) {
     if (!q || !k_cache_f16 || !v_cache_f16 || !out || !pos_dev || head_dim != 128 || n_head_kv <= 0 || n_head <= 0 || n_head % n_head_kv) return PB200_EINVAL;
-    g_launches++;
-    return launch_attn_decode(q, (const __half *) k_cache_f16, (const __half *) v_cache_f16, out, n_head, n_head_kv, head_dim, pos_dev, n_ctx, scale,
-                              (cudaStream_t) stream, false);
+    const int rc = launch_attn_decode(q, (const __half *) k_cache_f16, (const __half *) v_cache_f16, out, n_head, n_head_kv, head_dim, pos_dev, n_ctx,
+                                      scale, (cudaStream_t) stream, false);
+    if (rc == (int) cudaErrorNotSupported) return PB200_ENOTSUP;   // n_ctx above the score row k_attn_rows keeps in shared memory
+    if (rc == 0) g_launches++;
+    return rc;
 }
 
 int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * act_ws, int prologue, const float * in0, const float * in1, float eps,
@@ -255,9 +257,11 @@ int pb200_attn_prefill(const float * q, const void * k_cache_f16, const void * v
                        const int32_t * pos_dev, int n_tok, int n_kv_max, float scale, void * stream) {
     if (!q || !k_cache_f16 || !v_cache_f16 || !out || !pos_dev || head_dim != 128 || n_head_kv <= 0 || n_head % n_head_kv || n_tok <= 0 || n_kv_max <= 0)
         return PB200_EINVAL;
-    g_launches++;
-    return launch_attn_batch(q, (const __half *) k_cache_f16, (const __half *) v_cache_f16, out, n_head, n_head_kv, head_dim, pos_dev, n_tok, n_kv_max,
-                             scale, (cudaStream_t) stream);
+    const int rc = launch_attn_batch(q, (const __half *) k_cache_f16, (const __half *) v_cache_f16, out, n_head, n_head_kv, head_dim, pos_dev, n_tok,
+                                     n_kv_max, scale, (cudaStream_t) stream);
+    if (rc == (int) cudaErrorNotSupported) return PB200_ENOTSUP;
+    if (rc == 0) g_launches++;
+    return rc;
 }
 
 }  // extern "C"

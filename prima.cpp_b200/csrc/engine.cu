@@ -210,6 +210,7 @@ pb200_model * pb200_model_create(const pb200_hparams * hp, int device, int layer
     if (hp->n_head_kv <= 0 || hp->n_head <= 0 || hp->n_ff <= 0 || hp->n_vocab <= 0 || hp->n_ctx <= 0 || hp->n_embd <= 0) return nullptr;
     if (hp->head_dim != 128 || hp->n_head % hp->n_head_kv != 0 || hp->n_embd % 256 != 0) return nullptr;
     if (cudaSetDevice(device) != cudaSuccess) return nullptr;
+    if (hp->n_ctx > attn_rows_max_kv()) return nullptr;   // the attention fallback keeps a whole score row in shared memory
     pb200_model * m = new pb200_model();
     m->hp = *hp;
     m->device = device;

@@ -654,9 +654,24 @@ int sm_count() {
     if (!cache[dev]) cudaDeviceGetAttribute(&cache[dev], cudaDevAttrMultiProcessorCount, dev);
     return cache[dev];
 }
+size_t dyn_smem_limit(FuncAttrCache & c, const void * fn) {
+    const int dev = cur_device();
+    if (!c.limit[dev]) {
+        int optin = 0;
+        cudaFuncAttributes fa{};
+        if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess || cudaFuncGetAttributes(&fa, fn) != cudaSuccess) {
+            cudaGetLastError();
+            return 0;
+        }
+        c.limit[dev] = (size_t) optin > fa.sharedSizeBytes ? (size_t) optin - fa.sharedSizeBytes : 0;
+    }
+    return c.limit[dev];
+}
 cudaError_t ensure_dyn_smem(FuncAttrCache & c, const void * fn, size_t bytes, bool max_carveout) {
     const int dev = cur_device();
     if (bytes <= c.bytes[dev]) return cudaSuccess;
+    const size_t limit = dyn_smem_limit(c, fn);
+    if (limit && bytes > limit) return cudaErrorNotSupported;   // refused here: a failed cudaFuncSetAttribute would linger as the last error
     if (bytes > 48 * 1024 || max_carveout) {
         cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(bytes, 48 * 1024));
         if (e != cudaSuccess) return e;

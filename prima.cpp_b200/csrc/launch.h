@@ -73,10 +73,14 @@ struct LaunchCfg {
 
 // ---- per-device host state (gemv.cu): cudaFuncSetAttribute / SM count are per device, one process may drive several ----
 constexpr int PB_MAX_DEV = 64;
-struct FuncAttrCache { size_t bytes[PB_MAX_DEV] = {0}; };
+struct FuncAttrCache { size_t bytes[PB_MAX_DEV] = {0}; size_t limit[PB_MAX_DEV] = {0}; };
 int cur_device();
 int sm_count();                       // of the current device
-// raise a kernel's dynamic shared-memory limit on the current device if needed (max_carveout: also prefer the full 228 KB carve-out)
+// the most dynamic shared memory a launch of fn may request on the current device: the opt-in limit per block minus fn's static
+// shared memory (0 if the device cannot be queried)
+size_t dyn_smem_limit(FuncAttrCache & c, const void * fn);
+// raise a kernel's dynamic shared-memory limit on the current device if needed (max_carveout: also prefer the full 228 KB carve-out);
+// cudaErrorNotSupported, with nothing changed, when bytes exceed dyn_smem_limit
 cudaError_t ensure_dyn_smem(FuncAttrCache & c, const void * fn, size_t bytes, bool max_carveout);
 // wait watchdogs (common.cuh): host-mapped flag every kernel with a bounded wait gets a pointer to; check_clear_abort() returns 1
 // once per abort and re-arms — the C ABI reports PB200_EABORTED for the call that synchronised on the aborted launch
@@ -126,6 +130,9 @@ int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int
 //   out[h][:] = softmax(scale * K[0..n_kv) . q_h) . V   — GQA-aware, K/V read once per kv head.  n_kv = *pos_dev + 1.
 int launch_attn_decode(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,
                        const int32_t * pos_dev, int n_ctx, float scale, cudaStream_t stream, bool pdl);
+// k_attn_rows keeps a whole score row in shared memory: the longest row (a multiple of 32) it takes on the current device.  Longer
+// n_ctx / n_kv_max make launch_attn_decode, launch_attn_batch's per-row form and launch_attn_step's fallback return cudaErrorNotSupported.
+int attn_rows_max_kv();
 // batched form for prompt processing: token t (q row t, out row t) attends to cache rows [0, pos_dev[t]].  The tiled kernel when its
 // scores fit shared memory, else k_attn_rows per (head, token)
 int launch_attn_batch(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,

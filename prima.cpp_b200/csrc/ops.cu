@@ -10,6 +10,8 @@
 
 #include <math.h>
 
+#include <algorithm>
+
 namespace pb {
 
 // ------------------------------------------------------------------------------------------------
@@ -832,9 +834,10 @@ __global__ void __launch_bounds__(A2_THREADS, 1) k_attn2(const __grid_constant__
 }
 
 // ------------------------------------------------------------------------------------------------
-// soft_max_ext rows (plugin): y = softmax(x*scale + mask)
+// soft_max_ext rows (plugin): y = softmax(x*scale + mask).  The row is staged in shared memory when it fits (in_smem), otherwise the
+// softmax runs in place on the output row in global memory: same arithmetic in the same order, any row length.
 __global__ void __launch_bounds__(256) k_soft_max(const float * __restrict__ x, const float * __restrict__ mask, float * __restrict__ y, int ncols,
-                                                  int64_t rows_per_mask_cycle, float scale) {
+                                                  int64_t rows_per_mask_cycle, float scale, bool in_smem) {
     extern __shared__ float sm[];
     __shared__ float s_red[8];
     __shared__ double s_redd[8];
@@ -843,13 +846,14 @@ __global__ void __launch_bounds__(256) k_soft_max(const float * __restrict__ x, 
     const float * xr = x + row * ncols;
     const float * mr = mask ? mask + (row % rows_per_mask_cycle) * ncols : nullptr;
     float * yr = y + row * ncols;
+    float * S = in_smem ? sm : yr;
     for (int i = threadIdx.x; i < ncols; i += 256) {
         float v = __fmul_rn(xr[i], scale);
         if (mr) v = __fadd_rn(v, mr[i]);
-        sm[i] = v;
+        S[i] = v;
     }
-    const float inv = block_softmax<8, true>(sm, ncols, s_red, s_redd, &s_b);
-    for (int i = threadIdx.x; i < ncols; i += 256) yr[i] = __fmul_rn(sm[i], inv);
+    const float inv = block_softmax<8, true>(S, ncols, s_red, s_redd, &s_b);
+    for (int i = threadIdx.x; i < ncols; i += 256) yr[i] = __fmul_rn(S[i], inv);   // element i: written and read by the same thread
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1117,15 +1121,23 @@ int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int
     return (int) cudaGetLastError();
 }
 
-// k_attn_rows<FRESH> for n_head heads x n_tok tokens (q / out rows tok_stride floats apart), scores of up to n_kv_max cells
+// k_attn_rows<FRESH> for n_head heads x n_tok tokens (q / out rows tok_stride floats apart), scores of up to n_kv_max cells.
+// Dynamic shared memory: the score row padded to 32 plus red[8][128]; cudaErrorNotSupported when that exceeds the device's limit.
+static FuncAttrCache attn_rows_attr[2];
+static size_t attn_rows_smem(int n_kv_max) { return ((size_t) ((n_kv_max + 31) & ~31) + 8 * 128) * sizeof(float); }
+int attn_rows_max_kv() {
+    const size_t lim = std::min(dyn_smem_limit(attn_rows_attr[0], (const void *) k_attn_rows<false>),
+                                dyn_smem_limit(attn_rows_attr[1], (const void *) k_attn_rows<true>));
+    const int64_t n = (int64_t) (lim / sizeof(float)) - 8 * 128;   // largest padded row with attn_rows_smem(n) <= lim
+    return n > 0 ? (int) (n & ~31) : 0;
+}
 template <bool FRESH>
 static int launch_attn_rows(const float * q, const float * k, const float * v, __half * kc, __half * vc, float * out, int n_head, int n_head_kv,
                             const int32_t * pos_dev, const RopeParams & rp, const float * freq_factors, float scale, int n_tok, int64_t tok_stride,
                             int n_kv_max, cudaStream_t stream, bool pdl) {
-    const size_t smem = ((size_t) ((n_kv_max + 31) & ~31) + 8 * 128) * sizeof(float);
-    static FuncAttrCache attr_cache;
+    const size_t smem = attn_rows_smem(n_kv_max);
     {
-        cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_attn_rows<FRESH>, smem, false);
+        cudaError_t e = ensure_dyn_smem(attn_rows_attr[FRESH], (const void *) k_attn_rows<FRESH>, smem, false);
         if (e != cudaSuccess) return (int) e;
     }
     LaunchCfg lc(dim3(n_head, n_tok), dim3(256), smem, stream, pdl);
@@ -1231,13 +1243,14 @@ int launch_flash_attn_ext(const float * q, const void * k, const void * v, const
 
 int launch_soft_max(const float * x, const float * mask, float * y, int ncols, int64_t nrows, int64_t rows_per_mask_cycle, float scale,
                     cudaStream_t stream) {
-    const size_t smem = (size_t) ncols * sizeof(float);
+    size_t smem = (size_t) ncols * sizeof(float);
     static FuncAttrCache sm_attr;
     {
         cudaError_t e = ensure_dyn_smem(sm_attr, (const void *) k_soft_max, smem, false);
-        if (e != cudaSuccess) return (int) e;
+        if (e == cudaErrorNotSupported) smem = 0;   // the row does not fit: softmax in place in y
+        else if (e != cudaSuccess) return (int) e;
     }
-    k_soft_max<<<(unsigned) nrows, 256, smem, stream>>>(x, mask, y, ncols, rows_per_mask_cycle, scale);
+    k_soft_max<<<(unsigned) nrows, 256, smem, stream>>>(x, mask, y, ncols, rows_per_mask_cycle, scale, smem != 0);
     return (int) cudaGetLastError();
 }
 

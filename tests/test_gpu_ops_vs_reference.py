@@ -2,7 +2,7 @@
 with the reference's own CPU backend on the same seeded inputs.  The reference's results are recorded in golden/reference_golden.npz
 (golden/make_reference_golden.py builds each op with the reference's ggml and computes it on its CPU backend), so the comparison needs
 no reference tree.  Bars: the reference's own NMSE thresholds (tests/test-backend-ops.cpp: MUL_MAT 5e-4 :1660, SOFT_MAX 1e-6 :2077,
-others 1e-7 :320), and bit-exact results where the op only moves or converts values."""
+FLASH_ATTN_EXT 5e-4, others 1e-7 :320), and bit-exact results where the op only moves or converts values."""
 import ctypes as C
 from pathlib import Path
 
@@ -60,6 +60,37 @@ def test_op_matches_reference_cpu_backend(cuda, lib, refgold, op):
                 sync()
                 got = y.cpu().numpy().reshape(T, N)
             assert nmse(got, want) < 5e-4, (O.TYPE_NAME[t], nmse(got, want))
+        return
+    if op in ("FLASH_ATTN_EXT", "MUL_MAT_F16"):
+        # GQA over cache views, q permuted ([n_tok][n_head][D] in memory), f16 causal -inf mask with holes (RG.ATT)
+        H, HK, D, Tn, n_kv, n_ctx = (RG.ATT[k] for k in ("H", "HK", "D", "T", "n_kv", "n_ctx"))
+        i64 = lambda v: (C.c_int64 * len(v))(*v)  # noqa: E731
+        qd, kd = dev_f32(inp["q"]), torch.from_numpy(inp["kc"]).cuda()
+        if op == "FLASH_ATTN_EXT":
+            vd, md = torch.from_numpy(inp["vc"]).cuda(), torch.from_numpy(inp["mask"]).cuda()
+            y = torch.full((Tn * H * D,), float("nan"), device="cuda")
+            fn = lib.c.pb200_flash_attn_ext
+            fn.argtypes = [C.c_void_p] * 5 + [C.c_int] * 5 + [C.c_void_p] * 3 + [C.c_int64, C.c_float, C.c_float, C.c_float, C.c_void_p]
+            lib.check(fn(ptr(qd), ptr(kd), ptr(vd), ptr(md), ptr(y), D, Tn, H, HK, n_kv, i64([H * D * 4, D * 4]), i64([HK * D * 2, D * 2]),
+                         i64([HK * D * 2, D * 2]), n_kv * 2, inp["scale"], 0.0, 0.0, None), "flash_attn_ext")
+            sync()
+            got, want = y.cpu().numpy().reshape(Tn, H, D), refgold["op_FLASH_ATTN_EXT"]
+            assert nmse(got, want) < 5e-4, nmse(got, want)          # test-backend-ops.cpp: FLASH_ATTN_EXT max_nmse_err 5e-4
+            return
+        fn = lib.c.pb200_mul_mat_f16
+        fn.argtypes = [C.c_void_p] * 3 + [C.c_int64, C.c_void_p, C.c_int64, C.c_int64] + [C.c_void_p] * 4
+        vtd, pd = torch.from_numpy(inp["vt"]).cuda(), dev_f32(inp["p"])
+        kq = torch.full((H * Tn * n_kv,), float("nan"), device="cuda")
+        kqv = torch.full((H * Tn * D,), float("nan"), device="cuda")
+        # KQ: K-cache view [D, n_kv, HK] x permuted q [D, T, H];  KQV: transposed-V view [n_kv, D, HK] (rows n_ctx apart) x probs [n_kv, T, H]
+        lib.check(fn(ptr(kd), ptr(qd), ptr(kq), D, i64([n_kv, Tn, H, 1]), H // HK, 1, i64([2, HK * D * 2, D * 2, inp["kc"].nbytes]),
+                     i64([4, H * D * 4, D * 4, inp["q"].nbytes]), i64([4, n_kv * 4, n_kv * Tn * 4, kq.numel() * 4]), None), "mul_mat_f16 kq")
+        lib.check(fn(ptr(vtd), ptr(pd), ptr(kqv), n_kv, i64([D, Tn, H, 1]), H // HK, 1, i64([2, n_ctx * 2, D * n_ctx * 2, inp["vt"].nbytes]),
+                     i64([4, n_kv * 4, n_kv * Tn * 4, inp["p"].nbytes]), i64([4, D * 4, D * Tn * 4, kqv.numel() * 4]), None), "mul_mat_f16 kqv")
+        sync()
+        for name, y, shape in (("kq", kq, (H, Tn, n_kv)), ("kqv", kqv, (H, Tn, D))):
+            got, want = y.cpu().numpy().reshape(shape), refgold[f"op_MUL_MAT_F16_{name}"]
+            assert nmse(got, want) < 5e-4, (name, nmse(got, want))  # test-backend-ops.cpp: MUL_MAT max_nmse_err 5e-4
         return
     want = refgold[f"op_{op}"]
     if op == "RMS_NORM":
