@@ -49,7 +49,7 @@ size_t pb200_act_workspace_bytes(int64_t k) { return act_ws_bytes(k); }
 int pb200_quantize_act(int wtype, const float * x, int64_t k, void * act_ws, void * stream) {
     if (!type_ok(wtype) || !x || !act_ws || k <= 0 || k % block_elems(wtype) != 0) return PB200_EINVAL;
     g_launches++;
-    return launch_quantize_act(x, (int) k, act_mode_for(wtype), act_from_ws(act_ws, k), (cudaStream_t) stream, false);
+    return launch_quantize_act(x, nullptr, (int) k, act_mode_for(wtype), act_from_ws(act_ws, k), (cudaStream_t) stream, false);
 }
 
 int pb200_mul_mat_vec_q(int type, const void * W, int64_t n, int64_t k, const void * act_ws, float * y, const float * bias, const float * resid,

@@ -222,10 +222,4 @@ __device__ __forceinline__ void bulk_prefetch_l2(const void * gsrc, uint32_t byt
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// nearest_int of ggml-quants.c:1639-1644 (round-half-even via the 1.5*2^23 magic add), bit-exact
-__device__ __forceinline__ int nearest_int_magic(float f) {
-    float v = __fadd_rn(f, 12582912.f);
-    return (__float_as_int(v) & 0x007fffff) - 0x00400000;
-}
-
 }  // namespace pb

@@ -19,8 +19,6 @@ struct __align__(16) GemvSmemCtl {
 constexpr int GEMV_CTL_BYTES = 768;
 static_assert(sizeof(GemvSmemCtl) <= GEMV_CTL_BYTES, "ctl block");
 
-__device__ __forceinline__ float silu_f(float x) { return __fdiv_rn(x, 1.0f + expf(-x)); }   // ggml.c:2560
-
 // TRACE instantiation only: slot k (0..5) of this CTA's 8-entry row = %globaltimer (ns) at stamp k; slots 6 / 7 = clock64 at
 // the first / last stamp (the SM clock during the launch follows from the two)
 template <bool TRACE>
@@ -132,8 +130,7 @@ __device__ __forceinline__ void dist_prologue(const GemvParams & P, GemvSmemCtl 
         double t = 0.0;
 #pragma unroll
         for (int i = 0; i < GEMV_NW; i++) t += ctl->red[i];
-        const float mean = (float) (t / (double) P.K);
-        scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, P.eps)));
+        scale = rms_scale(t, P.K, P.eps);
     }
     for (int b = myblk; b < nblk; b += GEMV_NW * (int) gridDim.x) {
         if (b != myblk) { load8(P.in0 + b * 256 + lane * 8, bx); load8(P.in1 + b * 256 + lane * 8, bw); }   // tiny grids only
@@ -963,9 +960,9 @@ int launch_gemv(const GemvDesc * d, int nmat, int K, const ActQ & act, const Gem
     }
     int e = 0;
     if (nmode == 1) {
-        if (pro.kind == PRO_QUANTIZE) e = launch_quantize_act(pro.in0, K, modes[0], act, stream, pdl);
+        if (pro.kind == PRO_QUANTIZE) e = launch_quantize_act(pro.in0, nullptr, K, modes[0], act, stream, pdl);
         else if (pro.kind == PRO_RMSNORM) e = launch_rmsnorm_quant(pro.in0, pro.in1, K, pro.eps, modes[0], act, nullptr, stream, pdl);
-        else if (pro.kind == PRO_SILU_MUL) e = launch_silu_mul_quant(pro.in0, pro.in1, K, modes[0], act, nullptr, stream, pdl);
+        else if (pro.kind == PRO_SILU_MUL) e = launch_quantize_act(pro.in0, pro.in1, K, modes[0], act, stream, pdl);
         if (e) return e;
         if (pro.kind != PRO_NONE) { nlaunch++; pdl = true; }
         return gemv_kernels(d, nmat, K, act, stream, pdl, nlaunch, start);
@@ -986,7 +983,7 @@ int launch_gemv(const GemvDesc * d, int nmat, int K, const ActQ & act, const Gem
         int ns = 0;
         for (int i = 0; i < nmat; i++)
             if (act_mode_for(d[i].type) == modes[j]) sub[ns++] = d[i];
-        e = launch_quantize_act(x, K, modes[j], act, stream, pdl);
+        e = launch_quantize_act(x, nullptr, K, modes[j], act, stream, pdl);
         if (e) return e;
         nlaunch++;
         pdl = true;

@@ -36,6 +36,7 @@
 
 #include "common.cuh"
 #include "launch.h"
+#include "quantize.cuh"
 
 namespace pb {
 
@@ -489,32 +490,13 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
 // Fused producers of the activation (pre_kind): PRO_SILU_MUL = silu(x) * aux[t][k] (llm_build_ffn's SILU + MUL in front of ffn_down, the f32
 // product never goes to HBM), PRO_RMSNORM = rms_norm(x) * aux[k] (llm_build_norm in front of q|k|v and gate|up): the same arithmetic, rounding for rounding, as
 // k_silu_mul / k_rms_norm_rows followed by the plain pass.
-__device__ __forceinline__ float mmq_silu(float x) { return __fdiv_rn(x, 1.0f + expf(-x)); }   // ggml.c:2560
 __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, int64_t ldx, int T, int K, int BN, uint8_t * __restrict__ out,
                                                   int blk32, int pre_kind, const float * __restrict__ aux, int64_t ld_aux, float eps) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nblk = (K + 255) / 256;
     const int t = blockIdx.x;                       // 0 .. Tpad-1
     const int b_bytes = BN * 128;
-    float nscale = 1.f;
-    if (pre_kind == PRO_RMSNORM && t < T) {                   // k_rms_norm_rows' sum, in its order (ggml.c:11950-11996: double-precision sum of squares)
-        __shared__ double red[8];
-        __shared__ float s_scale;
-        const float * xr = x + (size_t) t * ldx;
-        double sum = 0.0;
-        for (int i = threadIdx.x; i < K; i += 256) sum += (double) __fmul_rn(xr[i], xr[i]);
-        sum = warp_sum_d(sum);
-        if (lane == 0) red[warp] = sum;
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            double tt = 0;
-            for (int i = 0; i < 8; i++) tt += red[i];
-            const float mean = (float) (tt / (double) K);
-            s_scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, eps)));
-        }
-        __syncthreads();
-        nscale = s_scale;
-    }
+    const float nscale = pre_kind == PRO_RMSNORM && t < T ? block_rms_scale(x + (size_t) t * ldx, K, eps) : 1.f;   // k_rms_norm_rows' scale
     for (int b = warp; b < nblk; b += 8) {
         float v[8];
         const bool live = b * 256 + lane * 8 < K;   // K % 32 == 0: a 4-lane group (one 32-block) is live or dead as a whole
@@ -527,47 +509,28 @@ __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, 
                 const float4 e = q[0], f = q[1];
                 const float w[8] = {e.x, e.y, e.z, e.w, f.x, f.y, f.z, f.w};
 #pragma unroll
-                for (int i = 0; i < 8; i++) v[i] = pre_kind == PRO_SILU_MUL ? __fmul_rn(mmq_silu(v[i]), w[i]) : __fmul_rn(__fmul_rn(v[i], nscale), w[i]);
+                for (int i = 0; i < 8; i++) v[i] = pre_kind == PRO_SILU_MUL ? __fmul_rn(silu_f(v[i]), w[i]) : __fmul_rn(__fmul_rn(v[i], nscale), w[i]);
             }
         } else {
 #pragma unroll
             for (int i = 0; i < 8; i++) v[i] = 0.f;
         }
-        float amax = 0.f, vmax = 0.f;
-        int idx = 0x7fffffff;
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-            const float ax = fabsf(v[i]);
-            if (ax > amax) { amax = ax; vmax = v[i]; idx = lane * 8 + i; }
-        }
-        warp_argmax(amax, idx, &vmax);
-        uint32_t h[4] = {0u, 0u, 0u, 0u};
+        int q[8];
+        float d;
         if (blk32) {
-            float am = 0.f;
-#pragma unroll
-            for (int i = 0; i < 8; i++) am = fmaxf(am, fabsf(v[i]));
-            am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, 1));
-            am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, 2));
-            const float d = __half2float(__float2half_rn(__fdiv_rn(am, 127.f)));
-            const float id = am != 0.f ? __fdiv_rn(127.f, am) : 0.f;
-            float f[8];
-#pragma unroll
-            for (int i = 0; i < 8; i++) f[i] = __fmul_rn(d, (float) __float2int_rn(__fmul_rn(v[i], id)));
-            h[0] = pack_h2(f[0], f[2]); h[1] = pack_h2(f[1], f[3]); h[2] = pack_h2(f[4], f[6]); h[3] = pack_h2(f[5], f[7]);
-        } else if (amax != 0.f) {
-            const float iscale = __fdiv_rn(-127.f, vmax);
-            const float d = __fdiv_rn(1.f, iscale);
-            float f[8];
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                int q = nearest_int_magic(__fmul_rn(iscale, v[i]));
-                q = q < 127 ? q : 127;
-                f[i] = __fmul_rn(d, (float) q);
-            }
-#pragma unroll
-            // within every 4 consecutive k the order is (0,2,1,3): the weight expansion produces its half2 pairs that way
-            h[0] = pack_h2(f[0], f[2]); h[1] = pack_h2(f[1], f[3]); h[2] = pack_h2(f[4], f[6]); h[3] = pack_h2(f[5], f[7]);
+            d = __half2float(__float2half_rn(q8_01_quant(v, q)));
+        } else {
+            float amax, vmax;
+            int idx;
+            q8K_lane_absmax(v, lane * 8, amax, vmax, idx);
+            warp_argmax(amax, idx, &vmax);
+            d = q8K_quant(v, amax, vmax, q);
         }
+        float f[8];
+#pragma unroll
+        for (int i = 0; i < 8; i++) f[i] = __fmul_rn(d, (float) q[i]);
+        // within every 4 consecutive k the order is (0,2,1,3): the weight expansion produces its half2 pairs that way
+        const uint32_t h[4] = {pack_h2(f[0], f[2]), pack_h2(f[1], f[3]), pack_h2(f[4], f[6]), pack_h2(f[5], f[7])};
         const int k = b * 256 + lane * 8;
         const int kc = k >> 6, j = (k & 63) >> 3;
         const int tt = t / BN, tl = t % BN;

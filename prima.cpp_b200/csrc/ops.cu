@@ -15,8 +15,8 @@
 namespace pb {
 
 // ------------------------------------------------------------------------------------------------
-// activation quantization: one warp per 256 values
-__global__ void __launch_bounds__(256) k_quantize_act(const float * __restrict__ x, int K, int mode, ActQ out) {
+// activation quantization of x (u == nullptr) or of silu(x) * u: one warp per 256 values
+__global__ void __launch_bounds__(256) k_quantize_act(const float * __restrict__ x, const float * __restrict__ u, int K, int mode, ActQ out) {
     pdl_trigger();   // dependents may launch now; they still wait for this grid's completion in their own pdl_wait()
     pdl_wait();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -24,41 +24,18 @@ __global__ void __launch_bounds__(256) k_quantize_act(const float * __restrict__
     const int64_t base = blk * 256 + lane * 8;
     if (blk * 256 >= K) return;
     float v[8];
-    if (base + 8 <= K) {
-        const float4 a = *reinterpret_cast<const float4 *>(x + base), b = *reinterpret_cast<const float4 *>(x + base + 4);
-        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+    if (base + 8 <= K && ((((uintptr_t) x) | ((uintptr_t) u)) & 15) == 0) {   // both operands in flight before either is used
+        const float4 x0 = __ldcg(reinterpret_cast<const float4 *>(x + base)), x1 = __ldcg(reinterpret_cast<const float4 *>(x + base + 4));
+        v[0] = x0.x; v[1] = x0.y; v[2] = x0.z; v[3] = x0.w; v[4] = x1.x; v[5] = x1.y; v[6] = x1.z; v[7] = x1.w;
+        if (u) {
+            const float4 u0 = __ldcg(reinterpret_cast<const float4 *>(u + base)), u1 = __ldcg(reinterpret_cast<const float4 *>(u + base + 4));
+            const float uv[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+#pragma unroll
+            for (int i = 0; i < 8; i++) v[i] = __fmul_rn(silu_f(v[i]), uv[i]);
+        }
     } else {
 #pragma unroll
-        for (int i = 0; i < 8; i++) v[i] = base + i < K ? x[base + i] : 0.f;
-    }
-    quantize_warp(mode, v, lane, blk, out);
-}
-
-__device__ __forceinline__ float silu_f32(float x) { return __fdiv_rn(x, 1.0f + expf(-x)); }   // ggml.c:2560
-
-__global__ void __launch_bounds__(256) k_silu_mul_quant(const float * __restrict__ g, const float * __restrict__ u, int K, int mode, ActQ out,
-                                                        float * __restrict__ f32_out) {
-    pdl_trigger();   // dependents may launch now; they still wait for this grid's completion in their own pdl_wait()
-    pdl_wait();
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t blk = (int64_t) blockIdx.x * 8 + warp;
-    const int64_t base = blk * 256 + lane * 8;
-    if (blk * 256 >= K) return;
-    float v[8];
-    if (base + 8 <= K && ((((uintptr_t) g) | ((uintptr_t) u)) & 15) == 0) {   // both operands in flight before either is used
-        const float4 g0 = __ldcg(reinterpret_cast<const float4 *>(g + base)), g1 = __ldcg(reinterpret_cast<const float4 *>(g + base + 4));
-        const float4 u0 = __ldcg(reinterpret_cast<const float4 *>(u + base)), u1 = __ldcg(reinterpret_cast<const float4 *>(u + base + 4));
-        const float gv[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w}, uv[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
-#pragma unroll
-        for (int i = 0; i < 8; i++) v[i] = __fmul_rn(silu_f32(gv[i]), uv[i]);
-    } else {
-#pragma unroll
-        for (int i = 0; i < 8; i++) v[i] = base + i < K ? __fmul_rn(silu_f32(g[base + i]), u[base + i]) : 0.f;
-    }
-    if (f32_out) {
-#pragma unroll
-        for (int i = 0; i < 8; i++)
-            if (base + i < K) f32_out[base + i] = v[i];
+        for (int i = 0; i < 8; i++) v[i] = base + i >= K ? 0.f : u ? __fmul_rn(silu_f(x[base + i]), u[base + i]) : x[base + i];
     }
     quantize_warp(mode, v, lane, blk, out);
 }
@@ -83,10 +60,7 @@ __global__ void __launch_bounds__(1024) k_rmsnorm_quant(const float * __restrict
     if (warp == 0) {
         double t = red[lane];
         t = warp_sum_d(t);
-        if (lane == 0) {
-            const float mean = (float) (t / (double) n);
-            s_scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, eps)));
-        }
+        if (lane == 0) s_scale = rms_scale(t, n, eps);
     }
     __syncthreads();
     const float scale = s_scale;
@@ -145,8 +119,7 @@ __global__ void __launch_bounds__(RQ_WARPS * 32) k_rmsnorm_q8K(const float * __r
     double t = 0.0;
 #pragma unroll
     for (int i = 0; i < RQ_WARPS; i++) t += red[i];
-    const float mean = (float) (t / (double) n);
-    const float scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, eps)));
+    const float scale = rms_scale(t, n, eps);
 #pragma unroll
     for (int j = 0; j < RQ_B; j++) {
         const int b = warp + j * RQ_WARPS;
@@ -161,24 +134,9 @@ __global__ void __launch_bounds__(RQ_WARPS * 32) k_rmsnorm_q8K(const float * __r
 // plain row-wise rms_norm for the plugin (no weight): one CTA per row
 __global__ void __launch_bounds__(256) k_rms_norm_rows(const float * __restrict__ x, float * __restrict__ y, int n, float eps,
                                                        const float * __restrict__ w) {
-    __shared__ double red[8];
-    __shared__ float s_scale;
     const float * xr = x + (int64_t) blockIdx.x * n;
     float * yr = y + (int64_t) blockIdx.x * n;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    double sum = 0.0;
-    for (int i = threadIdx.x; i < n; i += 256) sum += (double) __fmul_rn(xr[i], xr[i]);
-    sum = warp_sum_d(sum);
-    if (lane == 0) red[warp] = sum;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = 0;
-        for (int i = 0; i < 8; i++) t += red[i];
-        const float mean = (float) (t / (double) n);
-        s_scale = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(mean, eps)));
-    }
-    __syncthreads();
-    const float scale = s_scale;
+    const float scale = block_rms_scale(xr, n, eps);
     if (w) {   // the following MUL node by the norm weight (src/llama.cpp:9772-9802), same two roundings as the separate kernels
         for (int i = threadIdx.x; i < n; i += 256) yr[i] = __fmul_rn(__fmul_rn(xr[i], scale), w[i]);
     } else {
@@ -791,15 +749,12 @@ __global__ void __launch_bounds__(A2_THREADS, 1) k_attn2(const __grid_constant__
         __syncthreads();
         const uint32_t rank = h & 1u;
         float xv[4];
-        float amax = 0.f, vmax = 0.f;
-        int idx = 0x7fffffff;
+        float amax, vmax;
+        int idx;
         if (warp == 0) {
 #pragma unroll
-            for (int i = 0; i < 4; i++) {
-                xv[i] = sm->o_s[4 * lane + i];
-                const float ax = fabsf(xv[i]);
-                if (ax > amax) { amax = ax; vmax = xv[i]; idx = (int) rank * 128 + 4 * lane + i; }   // strict '>': first occurrence
-            }
+            for (int i = 0; i < 4; i++) xv[i] = sm->o_s[4 * lane + i];
+            q8K_lane_absmax(xv, (int) rank * 128 + 4 * lane, amax, vmax, idx);
             warp_argmax(amax, idx, &vmax);
             if (lane == 0) { sm->cand[0] = amax; sm->cand[1] = vmax; sm->cand[2] = __int_as_float(idx); }
         }
@@ -809,21 +764,12 @@ __global__ void __launch_bounds__(A2_THREADS, 1) k_attn2(const __grid_constant__
             const int oi = __float_as_int(ld_dsmem_f32(&sm->cand[2], rank ^ 1u));
             argmax_combine(amax, idx, oa, oi, &vmax, ov);
             const int64_t blk = h >> 1;
-            uint32_t packed = 0u;
-            int sum = 0;
-            float d = 0.f;
-            if (amax != 0.f) {
-                const float iscale = __fdiv_rn(-127.f, vmax);
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    int qv = nearest_int_magic(__fmul_rn(iscale, xv[i]));
-                    qv = qv < 127 ? qv : 127;
-                    sum += qv;
-                    packed |= (uint32_t) (qv & 0xff) << (8 * i);
-                }
-                d = __fdiv_rn(1.f, iscale);
-            }
-            *reinterpret_cast<uint32_t *>(outq.qs + blk * act_qs_stride(outq) + rank * 128 + 4 * lane) = packed;
+            int qv[4];
+            const float d = q8K_quant(xv, amax, vmax, qv);
+            uint32_t packed[1];
+            int sum;
+            pack_q8(qv, packed, sum);
+            *reinterpret_cast<uint32_t *>(outq.qs + blk * act_qs_stride(outq) + rank * 128 + 4 * lane) = packed[0];
             sum += __shfl_xor_sync(0xffffffffu, sum, 1);
             sum += __shfl_xor_sync(0xffffffffu, sum, 2);
             if ((lane & 3) == 0) outq.bsums[blk * act_bs_stride(outq) + rank * 8 + (lane >> 2)] = (int16_t) sum;
@@ -927,11 +873,11 @@ __global__ void k_binary(int op, const float * __restrict__ a, const float * __r
 }
 __global__ void k_silu(const float * __restrict__ x, float * __restrict__ y, int64_t n) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) y[i] = silu_f32(x[i]);
+    if (i < n) y[i] = silu_f(x[i]);
 }
 __global__ void k_silu_mul(const float * __restrict__ g, const float * __restrict__ u, float * __restrict__ y, int64_t n) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) y[i] = __fmul_rn(silu_f32(g[i]), u[i]);
+    if (i < n) y[i] = __fmul_rn(silu_f(g[i]), u[i]);
 }
 __global__ void k_cpy_f32_f16(const float * __restrict__ x, __half * __restrict__ y, int64_t n) {
     const int64_t i = (int64_t) blockIdx.x * blockDim.x + threadIdx.x;
@@ -1076,15 +1022,10 @@ int launch_mul_mat_f16(const void * A, const void * B, void * D, int64_t K, cons
     return (int) cudaGetLastError();
 }
 
-int launch_quantize_act(const float * x, int K, int mode, const ActQ & out, cudaStream_t stream, bool pdl) {
+int launch_quantize_act(const float * x, const float * up, int K, int mode, const ActQ & out, cudaStream_t stream, bool pdl) {
     const int ngroups = (K + 255) / 256;
     LaunchCfg lc(dim3((ngroups + 7) / 8), dim3(256), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_quantize_act, x, K, mode, out);
-}
-int launch_silu_mul_quant(const float * gate, const float * up, int K, int mode, const ActQ & out, float * f32_out, cudaStream_t stream, bool pdl) {
-    const int ngroups = (K + 255) / 256;
-    LaunchCfg lc(dim3((ngroups + 7) / 8), dim3(256), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_silu_mul_quant, gate, up, K, mode, out, f32_out);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_quantize_act, x, up, K, mode, out);
 }
 int launch_rmsnorm_quant(const float * x, const float * w, int n, float eps, int mode, const ActQ & out, float * f32_out, cudaStream_t stream, bool pdl) {
     if (mode == ACT_Q8_K && w && !f32_out && out.qs && n % 256 == 0 && n / 256 <= RQ_WARPS * 4 && ((uintptr_t) x & 15) == 0 && ((uintptr_t) w & 15) == 0) {

@@ -48,41 +48,43 @@ class GemvMat(C.Structure):
 def test_gemv_fused_prologue_rungs(cuda, lib, port, prologue):
     """pb200_gemv_fused on a q|k|v group of mixed k-quant types: with barrier words the prologue runs distributed inside the GEMV
     (one launch); without them a producer kernel runs in front (two launches).  Both leave the oracle's q8_K quantization of the
-    prologue's output in act_ws and match the oracle's mat-vec to fp32 summation order."""
-    K, eps = 2048, 1e-5
+    prologue's output in act_ws and match the oracle's mat-vec to fp32 summation order.  The sizes reach every rung: K = 2048 whole
+    rows and k_rmsnorm_q8K<2>; 12 288 split rows, the prologue's strided sum of squares and k_rmsnorm_q8K<4>; 28 672 k_rmsnorm_quant."""
+    eps = 1e-5
     types, Ns = [O.Q4_K, O.Q4_K, O.Q6_K], [512, 128, 128]
-    Ws = [O.synth_blocks(t, n, K, seed=17 + i) for i, (t, n) in enumerate(zip(types, Ns))]
-    rng = np.random.default_rng(prologue)
-    a = rng.standard_normal(K).astype(np.float32)
-    b = (1.0 + 0.1 * rng.standard_normal(K)).astype(np.float32) if prologue == 1 else rng.standard_normal(K).astype(np.float32)
-    ad, bd = dev_f32(a), dev_f32(b)
-    if prologue == 1:
-        x = port.rms_norm(a, eps) * b
-    else:
-        # silu's expf: the device's, from the plain silu * mul ops (same arithmetic as the fused prologues), next to the oracle's
-        xd = torch.zeros(K, device="cuda")
-        lib.check(lib.c.pb200_silu_mul(ptr(ad), ptr(bd), ptr(xd), K, None), "silu_mul")
-        sync()
-        x = xd.cpu().numpy()
-        assert np.max(np.abs(x - port.silu_mul(a, b))) <= rel_tol(x, 1e-6)
-    want_act = port.quantize_act(O.Q4_K, x)
-    wants = [port.mul_mat(t, w, n, K, x)[0] for t, n, w in zip(types, Ns, Ws)]
-    Wd = [dev_u8(w) for w in Ws]
     fn = lib.c.pb200_gemv_fused
     fn.argtypes = [C.c_int, C.POINTER(GemvMat), C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_void_p]
-    for barrier in (True, False):
-        ws = act_ws(lib, K)
-        sync_ws = torch.zeros(16, dtype=torch.uint8, device="cuda")
-        ys = [torch.full((n,), float("nan"), device="cuda") for n in Ns]
-        mats = (GemvMat * 3)(*[GemvMat(t, 0, w.data_ptr(), n, y.data_ptr(), None) for t, w, n, y in zip(types, Wd, Ns, ys)])
-        n0 = lib.c.pb200_kernel_launches()
-        lib.check(fn(3, mats, K, ws.data_ptr(), prologue, ad.data_ptr(), bd.data_ptr(), eps, sync_ws.data_ptr() if barrier else None, 1, None),
-                  "gemv_fused")
-        sync()
-        assert lib.c.pb200_kernel_launches() - n0 == (1 if barrier else 2)
-        assert np.array_equal(act_ws_fields(ws, K, "q8_K"), want_act), f"activation differs (barrier={barrier})"
-        for y, want in zip(ys, wants):
-            assert np.max(np.abs(y.cpu().numpy() - want)) <= rel_tol(want)
+    for K in (2048, 12288, 28672):
+        Ws = [O.synth_blocks(t, n, K, seed=17 + i) for i, (t, n) in enumerate(zip(types, Ns))]
+        rng = np.random.default_rng(prologue)
+        a = rng.standard_normal(K).astype(np.float32)
+        b = (1.0 + 0.1 * rng.standard_normal(K)).astype(np.float32) if prologue == 1 else rng.standard_normal(K).astype(np.float32)
+        ad, bd = dev_f32(a), dev_f32(b)
+        if prologue == 1:
+            x = port.rms_norm(a, eps) * b
+        else:
+            # silu's expf: the device's, from the plain silu * mul ops (same arithmetic as the fused prologues), next to the oracle's
+            xd = torch.zeros(K, device="cuda")
+            lib.check(lib.c.pb200_silu_mul(ptr(ad), ptr(bd), ptr(xd), K, None), "silu_mul")
+            sync()
+            x = xd.cpu().numpy()
+            assert np.max(np.abs(x - port.silu_mul(a, b))) <= rel_tol(x, 1e-6)
+        want_act = port.quantize_act(O.Q4_K, x)
+        wants = [port.mul_mat(t, w, n, K, x)[0] for t, n, w in zip(types, Ns, Ws)]
+        Wd = [dev_u8(w) for w in Ws]
+        for barrier in (True, False):
+            ws = act_ws(lib, K)
+            sync_ws = torch.zeros(16, dtype=torch.uint8, device="cuda")
+            ys = [torch.full((n,), float("nan"), device="cuda") for n in Ns]
+            mats = (GemvMat * 3)(*[GemvMat(t, 0, w.data_ptr(), n, y.data_ptr(), None) for t, w, n, y in zip(types, Wd, Ns, ys)])
+            n0 = lib.c.pb200_kernel_launches()
+            lib.check(fn(3, mats, K, ws.data_ptr(), prologue, ad.data_ptr(), bd.data_ptr(), eps, sync_ws.data_ptr() if barrier else None, 1, None),
+                      "gemv_fused")
+            sync()
+            assert lib.c.pb200_kernel_launches() - n0 == (1 if barrier else 2), (K, barrier)
+            assert np.array_equal(act_ws_fields(ws, K, "q8_K"), want_act), f"activation differs (K={K}, barrier={barrier})"
+            for y, want in zip(ys, wants):
+                assert np.max(np.abs(y.cpu().numpy() - want)) <= rel_tol(want), (K, barrier)
 
 
 @pytest.mark.parametrize("t", [O.Q8_0, O.Q5_1], ids=lambda t: O.TYPE_NAME[t])

@@ -27,14 +27,15 @@ def test_quantize_act_bit_exact(cuda, lib, port, t):
     cases += [np.zeros(K, np.float32), np.tile(np.array([1.0, -1.0, 0.5, -0.5], np.float32), K // 4),
               np.tile(np.array([-3.0, 3.0, 1.5, 0.0], np.float32), K // 4)]
     z = np.zeros(K, np.float32); z[300] = -2.5; cases.append(z)
-    for x in cases:
-        ws = act_ws(lib, K)
-        xd = dev_f32(x)
-        lib.check(lib.c.pb200_quantize_act(t, ptr(xd), K, ptr(ws), None), "quantize_act")
-        sync()
-        got = act_ws_fields(ws, K, MODE[t])
-        want = port.quantize_act(t, x)
-        assert np.array_equal(got, want), f"activation quantization differs for {O.TYPE_NAME[t]}"
+    for offset in (0, 1):   # 1: x one float past a 16-byte boundary, so the kernel must not use its 128-bit loads
+        for x in cases:
+            ws = act_ws(lib, K)
+            xd = dev_f32(np.concatenate([np.zeros(offset, np.float32), x]))
+            lib.check(lib.c.pb200_quantize_act(t, C.c_void_p(xd.data_ptr() + 4 * offset), K, ptr(ws), None), "quantize_act")
+            sync()
+            got = act_ws_fields(ws, K, MODE[t])
+            want = port.quantize_act(t, x)
+            assert np.array_equal(got, want), f"activation quantization differs for {O.TYPE_NAME[t]} (x offset {offset})"
 
 
 @pytest.mark.parametrize("t", KQ, ids=lambda t: O.TYPE_NAME[t])
