@@ -68,6 +68,10 @@ def load(with_plugin: bool = True, with_cudaref: bool = False):
     g.lgh_graph_builds.restype = C.c_uint64
     g.lgh_graph_builds.argtypes = [vp]
     g.lgh_graph_nodes.argtypes = [vp]
+    g.lgh_reserve.argtypes = [vp, C.c_int]
+    g.lgh_compute_buffer_base.restype = vp
+    g.lgh_compute_buffer_base.argtypes = [vp]
+    g.lgh_unsupported_nodes.argtypes = [vp]
     g.lgh_decode.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_int]
     g.lgh_get_hidden.argtypes = [vp, vp]
     g.lgh_phase_seconds.argtypes = [vp, C.POINTER(C.c_double)]
@@ -81,8 +85,11 @@ WEIGHT_ORDER = ("attn_q", "attn_k", "attn_v", "attn_output", "ffn_gate", "ffn_up
 class HostModel:
     """A model living in the buffers of one ggml backend ("CPU", "B200_0", ...), driven like llama_decode drives it."""
 
-    def __init__(self, hp: dict, types: dict, backend: str, n_threads: int = 8, has_bias: bool = False, has_freq_factors: bool = False):
-        """types: tensor name -> ggml_type for "token_embd.weight", "output.weight" and "blk.N.<WEIGHT_ORDER>.weight"."""
+    def __init__(self, hp: dict, types: dict, backend: str, n_threads: int = 8, has_bias: bool = False, has_freq_factors: bool = False,
+                 n_tokens_max: int = 1):
+        """types: tensor name -> ggml_type for "token_embd.weight", "output.weight" and "blk.N.<WEIGHT_ORDER>.weight".
+        n_tokens_max: the largest batch the compute buffer is reserved for (llama.cpp's n_ubatch); a larger batch still runs, but
+        grows (moves) the buffer."""
         self.g, self.plug = load(with_plugin=backend.startswith("B200"), with_cudaref=backend.startswith("CUDA"))
         self.hp = hp
         H = HParams(**{k: hp[k] for k in ("n_layer", "n_embd", "n_head", "n_head_kv", "head_dim", "n_ff", "n_vocab", "n_ctx", "rope_mode", "n_ctx_orig",
@@ -94,6 +101,10 @@ class HostModel:
         self.h = self.g.lgh_create(C.byref(H), arr, backend.encode(), n_threads)
         if not self.h:
             raise RuntimeError(f"lgh_create failed for backend {backend}")
+        rc = self.g.lgh_reserve(self.h, int(n_tokens_max))
+        if rc != 0:
+            self.close()
+            raise RuntimeError(f"lgh_reserve({n_tokens_max}) failed for backend {backend}: {rc}")
 
     def set_tensor(self, name: str, data) -> None:
         import numpy as np
@@ -148,6 +159,16 @@ class HostModel:
     @property
     def graph_nodes(self) -> int:
         return self.g.lgh_graph_nodes(self.h)
+
+    @property
+    def compute_buffer_base(self) -> int:
+        """Device / host address of the compute buffer (0 before the first decode); constant while every graph fits the reservation."""
+        return self.g.lgh_compute_buffer_base(self.h) or 0
+
+    @property
+    def unsupported_nodes(self) -> int:
+        """Non-view nodes of the current graph for which ggml_backend_supports_op is false (llama.cpp would run them on the CPU)."""
+        return self.g.lgh_unsupported_nodes(self.h)
 
     def close(self) -> None:
         if self.h:

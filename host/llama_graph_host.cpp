@@ -11,6 +11,11 @@
 //
 // This file is host-application code.  It links the host's ggml only (host/Makefile builds one from the reference tree,
 // unmodified) and knows nothing about libprima_b200.so.  FA off, KV cache f16, V cache transposed — the reference defaults.
+//
+// Compute buffer: like llama_new_context_with_model (src/llama.cpp:21361-21402), one ggml_gallocr per context reserves the
+// worst-case graph (n_tokens_max tokens, n_kv = n_ctx) once and keeps its buffer for the life of the context; each graph rebuild
+// frees only the graph's ggml_context.  Graphs that fit the reservation therefore land at the same addresses every time their
+// topology comes back, which is what lets a backend replay work it captured for that topology.
 #include "ggml.h"
 #include "ggml-alloc.h"
 #include "ggml-backend.h"
@@ -48,7 +53,8 @@ struct lgh_ctx {
     std::map<std::string, ggml_tensor *> by_name;
     // the graph of the current (n_tokens, n_kv) bucket, reused token after token (only the cache-view offsets and inputs change)
     ggml_context * gctx = nullptr;
-    ggml_gallocr_t galloc = nullptr;
+    ggml_gallocr_t galloc = nullptr;   // kept across graph rebuilds: its buffer is reserved for (n_tokens_max, n_ctx)
+    int n_tokens_max = 1;
     ggml_cgraph * gf = nullptr;
     int g_tokens = 0;
     int64_t g_nkv = 0;
@@ -118,8 +124,8 @@ void * lgh_create(const lgh_hparams * hp, const int32_t * types, const char * ba
 void lgh_free(void * p) {
     lgh_ctx * c = (lgh_ctx *) p;
     if (!c) return;
-    if (c->galloc) ggml_gallocr_free(c->galloc);
     if (c->gctx) ggml_free(c->gctx);
+    if (c->galloc) ggml_gallocr_free(c->galloc);
     if (c->wbuf) ggml_backend_buffer_free(c->wbuf);
     if (c->wctx) ggml_free(c->wctx);
     if (c->backend) ggml_backend_free(c->backend);
@@ -162,14 +168,30 @@ void lgh_kv_clear(void * p) {
 }
 uint64_t lgh_graph_builds(void * p) { return ((lgh_ctx *) p)->n_graph_builds; }
 int lgh_graph_nodes(void * p) { lgh_ctx * c = (lgh_ctx *) p; return c->gf ? ggml_graph_n_nodes(c->gf) : 0; }
+// base address of the compute buffer the current graph lives in (NULL before the first lgh_decode)
+void * lgh_compute_buffer_base(void * p) {
+    lgh_ctx * c = (lgh_ctx *) p;
+    return c->gf && c->logits && c->logits->buffer ? ggml_backend_buffer_get_base(c->logits->buffer) : nullptr;
+}
+// non-view nodes of the current graph the backend does not support; llama.cpp's scheduler would run those on the CPU
+int lgh_unsupported_nodes(void * p) {
+    lgh_ctx * c = (lgh_ctx *) p;
+    if (!c->gf) return -1;
+    int n = 0;
+    for (int i = 0; i < ggml_graph_n_nodes(c->gf); i++) {
+        ggml_tensor * t = ggml_graph_node(c->gf, i);
+        if (t->op == GGML_OP_NONE || t->op == GGML_OP_RESHAPE || t->op == GGML_OP_VIEW || t->op == GGML_OP_PERMUTE || t->op == GGML_OP_TRANSPOSE) continue;
+        if (!ggml_backend_supports_op(c->backend, t)) n++;
+    }
+    return n;
+}
 
 static void build_graph(lgh_ctx * g, int n_tokens, int64_t n_kv) {
     const lgh_hparams & hp = g->hp;
     const int64_t H = hp.n_head, HK = hp.n_head_kv, D = hp.head_dim;
     const int64_t EK = HK * D;
     const int64_t n_ctx = hp.n_ctx;
-    if (g->galloc) { ggml_gallocr_free(g->galloc); g->galloc = nullptr; }
-    if (g->gctx) { ggml_free(g->gctx); g->gctx = nullptr; }
+    if (g->gctx) { ggml_free(g->gctx); g->gctx = nullptr; g->gf = nullptr; }
     const size_t max_nodes = (size_t) 64 + 40 * (size_t) hp.n_layer;
     ggml_init_params ip = { ggml_tensor_overhead() * max_nodes * 2 + ggml_graph_overhead_custom(max_nodes * 2, false) + (1u << 20), nullptr, true };
     ggml_context * c = g->gctx = ggml_init(ip);
@@ -246,10 +268,25 @@ static void build_graph(lgh_ctx * g, int n_tokens, int64_t n_kv) {
     ggml_set_output(cur);
     g->logits = cur;
     ggml_build_forward_expand(gf, cur);
-    g->galloc = ggml_gallocr_new(ggml_backend_get_default_buffer_type(g->backend));
-    ggml_gallocr_alloc_graph(g->galloc, gf);
     g->g_tokens = n_tokens; g->g_nkv = n_kv;
-    g->n_graph_builds++;
+}
+
+// worst-case reservation (llama_new_context_with_model: ggml_backend_sched_reserve on a graph of n_ubatch tokens over the whole
+// cache).  ggml_gallocr_alloc_graph reuses the reserved buffer for every graph that fits it and grows it only for one that does not.
+static bool reserve_compute_buffer(lgh_ctx * g) {
+    if (!g->galloc) g->galloc = ggml_gallocr_new(ggml_backend_get_default_buffer_type(g->backend));
+    build_graph(g, g->n_tokens_max, g->hp.n_ctx);
+    const bool ok = ggml_gallocr_reserve(g->galloc, g->gf);
+    ggml_free(g->gctx); g->gctx = nullptr; g->gf = nullptr;   // the next lgh_decode builds its own graph
+    g->logits = g->l_out = nullptr;
+    return ok;
+}
+// size the compute buffer for prompts of up to n_tokens_max tokens (the context's n_ubatch; 1 unless called)
+int lgh_reserve(void * p, int n_tokens_max) {
+    lgh_ctx * g = (lgh_ctx *) p;
+    if (n_tokens_max < 1 || n_tokens_max > g->hp.n_ctx) return -1;
+    g->n_tokens_max = n_tokens_max;
+    return reserve_compute_buffer(g) ? 0 : -2;
 }
 
 // n_tokens tokens at positions pos0 .. pos0+n_tokens-1 (kv_head = pos0), HOST buffers in and out.
@@ -264,7 +301,12 @@ int lgh_decode(void * p, const int32_t * tokens, int n_tokens, int pos0, float *
     if (n_kv < 32) n_kv = 32;
     if (n_kv > hp.n_ctx) n_kv = hp.n_ctx;
     double t0 = now_s();
-    if (!g->gf || g->g_tokens != n_tokens || g->g_nkv != n_kv) build_graph(g, n_tokens, n_kv);
+    if (!g->gf || g->g_tokens != n_tokens || g->g_nkv != n_kv) {
+        if (!g->galloc && !reserve_compute_buffer(g)) return -3;
+        build_graph(g, n_tokens, n_kv);
+        if (!ggml_gallocr_alloc_graph(g->galloc, g->gf)) return -3;
+        g->n_graph_builds++;
+    }
     g->t_build += now_s() - t0; t0 = now_s();
     // re-point the cache store views at kv_head (what a rebuilt graph would carry in view_offs)
     for (size_t iv = 0; iv < g->k_views.size(); iv++) {

@@ -106,6 +106,10 @@ struct b200_backend_ctx {
     std::vector<b200_plan *> plans;
     void * mmq_ws = nullptr;       // fp16 activation tiles for the tensor-core path (grown on demand)
     size_t mmq_ws_bytes = 0;
+    // generation of the plugin-owned device buffers a captured launch can hold by value (act_ws, mmq_ws, fact_ws, scratch,
+    // attn_tmp, sync_ws, kvh_dev): bumped at every (re)allocation and folded into each plan's `bind`, so that a CUDA graph
+    // captured before a buffer moved is recaptured instead of replayed.  Buffers only grow, so it changes a bounded number of times.
+    uint64_t ws_gen = 0;
     std::string name;
 };
 struct b200_buffer_ctx {
@@ -319,20 +323,25 @@ static bool b200_compute_node(b200_backend_ctx * ctx, ggml_tensor * dst) {
             }
             const int64_t K = a->ne[0], N = a->ne[1];
             const size_t need = pb200_act_workspace_bytes(K);
+            // no allocation inside a capture (as grow_ws): enqueue nothing, the capture is discarded and the call runs directly
+            if (need > ctx->act_ws_bytes && ctx->capturing) { ctx->capture_failed = true; return true; }
             if (need > ctx->act_ws_bytes) {
                 if (ctx->act_ws) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->act_ws); }
                 CUDA_OK(cudaMalloc(&ctx->act_ws, need + 256));
                 ctx->act_ws_bytes = need;
+                ctx->ws_gen++;
             }
             const int64_t r2 = b->ne[2] / a->ne[2], r3 = b->ne[3] / a->ne[3];
             if (b->ne[1] >= MMQ_MIN_COLS && mmq_ok(a->type, K) && b->nb[1] % 16 == 0 && (uintptr_t) b->data % 16 == 0 && b->nb[2] % 16 == 0 && b->nb[3] % 16 == 0 &&
                 (uintptr_t) a->data % 16 == 0 && a->nb[2] % 16 == 0 && a->nb[3] % 16 == 0) {   // the prep kernel reads rows as float4
                 // batched / prefill: the reference switches to mul_mat_q above 8 columns as well (ggml-cuda/mmq.cu:137-139)
                 const size_t need_q = pb200_mul_mat_q_workspace_bytes(K, b->ne[1]);
+                if (need_q > ctx->mmq_ws_bytes && ctx->capturing) { ctx->capture_failed = true; return true; }
                 if (need_q > ctx->mmq_ws_bytes) {
                     if (ctx->mmq_ws) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->mmq_ws); }
                     CUDA_OK(cudaMalloc(&ctx->mmq_ws, need_q + 256));
                     ctx->mmq_ws_bytes = need_q;
+                    ctx->ws_gen++;
                 }
                 for (int64_t i3 = 0; i3 < b->ne[3]; i3++)
                     for (int64_t i2 = 0; i2 < b->ne[2]; i2++) {
@@ -490,6 +499,14 @@ static bool is_kq(enum ggml_type t) { return t == GGML_TYPE_Q4_K || t == GGML_TY
 static bool is_vec_f32(const ggml_tensor * t, int64_t n) {
     return t && t->type == GGML_TYPE_F32 && t->ne[0] == n && t->ne[1] == 1 && t->ne[2] == 1 && t->ne[3] == 1 && t->nb[0] == sizeof(float);
 }
+// a MUL_MAT the fused GEMV takes: k-quant weights, one contiguous f32 activation column, K % 256 == 0, K <= 28672
+static bool gemv_fusable(const ggml_tensor * t) {
+    if (t->op != GGML_OP_MUL_MAT) return false;
+    const ggml_tensor * W = t->src[0], * X = t->src[1];
+    if (!is_kq(W->type) || !ggml_is_contiguous(W) || W->ne[2] != 1 || W->ne[3] != 1) return false;
+    const int64_t K = W->ne[0];
+    return is_vec_f32(X, K) && K % 256 == 0 && K <= 28672 && t->type == GGML_TYPE_F32 && ggml_is_contiguous(t);
+}
 static const ggml_tensor * strip_views(const ggml_tensor * t) {   // RESHAPE / PERMUTE / TRANSPOSE / VIEW of a COMPUTED tensor
     while (t && (t->op == GGML_OP_RESHAPE || t->op == GGML_OP_PERMUTE || t->op == GGML_OP_TRANSPOSE || t->op == GGML_OP_VIEW) && t->src[0]) t = t->src[0];
     return t;
@@ -633,11 +650,9 @@ static b200_plan * build_plan(ggml_cgraph * g, uint64_t key) {
         // 2) mat-vec groups (anchor: the activation shared by k-quant MUL_MATs with one column)
         for (int i = 0; i < G.n; i++) {
             const ggml_tensor * t = ggml_graph_node(g, i);
-            if (t->op != GGML_OP_MUL_MAT || taken[i]) continue;
+            if (taken[i] || !gemv_fusable(t)) continue;
             const ggml_tensor * W = t->src[0], * X = t->src[1];
-            if (!is_kq(W->type) || !ggml_is_contiguous(W) || W->ne[2] != 1 || W->ne[3] != 1) continue;
             const int64_t K = W->ne[0];
-            if (!is_vec_f32(X, K) || K % 256 != 0 || K > 28672 || t->type != GGML_TYPE_F32 || !ggml_is_contiguous(t)) continue;
             b200_step st{};
             st.kind = 1; st.prologue = 0; st.p0 = st.p1 = -1; st.ws = 0;
             for (int j = 0; j < 3; j++) st.out_scratch[j] = -1;
@@ -719,10 +734,19 @@ static b200_plan * build_plan(ggml_cgraph * g, uint64_t key) {
                     }
                     if (slot < 0 && co.size() == 1) {
                         const ggml_tensor * c0 = ggml_graph_node(g, co[0]);
-                        if (c0->op == GGML_OP_UNARY && ggml_get_unary_op(c0) == GGML_UNARY_OP_SILU) slot = SCR_G;
-                        else if (c0->op == GGML_OP_MUL) {
+                        int mul_i = -1;
+                        if (c0->op == GGML_OP_UNARY && ggml_get_unary_op(c0) == GGML_UNARY_OP_SILU) {
+                            std::vector<int> cs; real_consumers(G, co[0], cs);
+                            if (cs.size() == 1) { slot = SCR_G; mul_i = cs[0]; }
+                        } else if (c0->op == GGML_OP_MUL) {
                             const ggml_tensor * other = c0->src[0] == ggml_graph_node(g, st.out[j]) ? c0->src[1] : c0->src[0];
-                            if (other && other->op == GGML_OP_UNARY && ggml_get_unary_op(other) == GGML_UNARY_OP_SILU) slot = SCR_U;
+                            if (other && other->op == GGML_OP_UNARY && ggml_get_unary_op(other) == GGML_UNARY_OP_SILU) { slot = SCR_U; mul_i = co[0]; }
+                        }
+                        // gate / up may only stay private if silu(gate) * up feeds a down projection the silu-prologue GEMV takes
+                        // (an ffn_down of Q5_1 / Q8_0, as for n_ff % 256 != 0, runs 1:1 and reads gate / up from the graph)
+                        if (slot >= 0) {
+                            std::vector<int> cm; real_consumers(G, mul_i, cm);
+                            if (cm.size() != 1 || !gemv_fusable(ggml_graph_node(g, cm[0]))) slot = -1;
                         }
                     }
                     st.out_scratch[j] = slot;
@@ -762,6 +786,23 @@ static b200_plan * build_plan(ggml_cgraph * g, uint64_t key) {
             std::vector<int> co; real_consumers(G, A.cont, co);
             A.out_private = (A.quant_out && co.size() == 1) ? 1 : 0;
         }
+        // and every gate / up kept private must be read by a silu-prologue step: nothing else sees the private buffers
+        for (int q = 0; q < G.n; q++) {
+            if (!has[q] || at[q].kind != 1) continue;
+            for (int j = 0; j < at[q].nmat; j++) {
+                const int slot = at[q].out_scratch[j];
+                if (slot != SCR_G && slot != SCR_U) continue;
+                const ggml_tensor * o = ggml_graph_node(g, at[q].out[j]);
+                bool read = false;
+                for (int r = 0; r < G.n && !read; r++) {
+                    if (!has[r] || at[r].kind != 1 || at[r].prologue != 2) continue;
+                    const ggml_tensor * un = ggml_graph_node(g, at[r].p0), * mul = ggml_graph_node(g, at[r].p1);
+                    const ggml_tensor * up = mul->src[0] == un ? mul->src[1] : mul->src[0];
+                    read = slot == SCR_G ? (un->src[0] == o && at[r].in_scratch[0] == SCR_G) : (up == o && at[r].in_scratch[1] == SCR_U);
+                }
+                if (!read) fused_ok = false;
+            }
+        }
     }
     b200_plan * plan = new b200_plan();
     plan->key = key; plan->n_nodes = G.n;
@@ -793,6 +834,7 @@ static float * grow_scratch(b200_backend_ctx * ctx, int slot, size_t floats) {
         if (ctx->scratch[slot]) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->scratch[slot]); }
         CUDA_OK(cudaMalloc((void **) &ctx->scratch[slot], floats * 4 + 256));
         ctx->scratch_floats[slot] = floats;
+        ctx->ws_gen++;
     }
     return ctx->scratch[slot];
 }
@@ -802,6 +844,7 @@ static void * grow_ws(b200_backend_ctx * ctx, int role, size_t need) {
         if (ctx->fact_ws[role]) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->fact_ws[role]); }
         CUDA_OK(cudaMalloc(&ctx->fact_ws[role], need + 256));
         ctx->fact_bytes[role] = need;
+        ctx->ws_gen++;
     }
     return ctx->fact_ws[role];
 }
@@ -823,7 +866,8 @@ static bool run_gemv_step(b200_backend_ctx * ctx, ggml_cgraph * g, const b200_st
         mats[j].add = st.add_vec[j] >= 0 ? (const float *) out->src[st.add_src[j]]->data : nullptr;
     }
     void * ws = grow_ws(ctx, st.ws, pb200_act_workspace_bytes(K));
-    if (!ctx->sync_ws) { CUDA_OK(cudaMalloc(&ctx->sync_ws, 256)); CUDA_OK(cudaMemsetAsync(ctx->sync_ws, 0, 256, ctx->stream)); }
+    if (!ctx->sync_ws && ctx->capturing) { ctx->capture_failed = true; return true; }
+    if (!ctx->sync_ws) { CUDA_OK(cudaMalloc(&ctx->sync_ws, 256)); CUDA_OK(cudaMemsetAsync(ctx->sync_ws, 0, 256, ctx->stream)); ctx->ws_gen++; }
     int rc;
     if (st.prologue == 1) {
         const ggml_tensor * nrm = ggml_graph_node(g, st.p0), * mul = ggml_graph_node(g, st.p1);
@@ -876,6 +920,7 @@ static bool run_attn_step(b200_backend_ctx * ctx, ggml_cgraph * g, const b200_st
             if (ctx->attn_tmp) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->attn_tmp); }
             CUDA_OK(cudaMalloc((void **) &ctx->attn_tmp, out_bytes + 256));
             ctx->attn_tmp_floats = (size_t) (H * D);
+            ctx->ws_gen++;
         }
         out = ctx->attn_tmp;
     }
@@ -956,19 +1001,21 @@ static enum ggml_status b200_backend_graph_compute(ggml_backend_t backend, ggml_
     const bool has_attn = plan->has_attn;
     ctx->skip.assign((size_t) plan->n_nodes, 0);
     for (int i : plan->store_nodes) ctx->skip[(size_t) i] = 1;
-    uint64_t bind = 0xcbf29ce484222325ull;
+    uint64_t addr_bind = 0xcbf29ce484222325ull;
     for (int i = 0; i < plan->n_nodes; i++) {
         if (ctx->skip[(size_t) i]) continue;
         const ggml_tensor * t = ggml_graph_node(cgraph, i);
         uint64_t w = (uint64_t) (uintptr_t) t->data;
         for (int k = 0; k < 3; k++) if (t->src[k]) w = w * 1315423911ull + (uint64_t) (uintptr_t) t->src[k]->data;   // leafs (weights, inputs) included
-        bind = fnv(bind, w);
+        addr_bind = fnv(addr_bind, w);
     }
+    const uint64_t bind = fnv(addr_bind, ctx->ws_gen);   // an exec captured before a workspace moved must not be replayed
     const int kvh = has_attn ? plan_kv_head(cgraph, plan) : -1;
     const bool graphable = use_graphs && kvh != -2 && plan->steps.size() >= 8;
     if (graphable && !ctx->kvh_dev) {
         CUDA_OK(cudaMalloc((void **) &ctx->kvh_dev, 256));
         CUDA_OK(cudaMallocHost((void **) &ctx->kvh_host, 64 * sizeof(int32_t)));
+        ctx->ws_gen++;
     }
     auto push_cell = [&]() {
         if (kvh >= 0) {   // a ring of pinned words: the host may run several calls ahead of the copies
@@ -1011,7 +1058,9 @@ static enum ggml_status b200_backend_graph_compute(ggml_backend_t backend, ggml_
         plan->seen = -1000000;          // this plan cannot be captured: direct launches from now on
     }
     run_plan(ctx, cgraph, plan);
-    if (plan->bind == bind) plan->seen++; else { plan->bind = bind; plan->seen = 1; }
+    // keyed with the generation this call leaves behind: a call that grew a workspace does not delay its own plan's capture
+    const uint64_t bind_end = fnv(addr_bind, ctx->ws_gen);
+    if (plan->bind == bind_end) plan->seen++; else { plan->bind = bind_end; plan->seen = 1; }
     return GGML_STATUS_SUCCESS;   // asynchronous: work is enqueued on the backend stream
 }
 
