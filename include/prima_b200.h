@@ -98,7 +98,9 @@ PB200_API int pb200_mul_mat_f16(const void * a_f16, const float * b_f32, float *
                                 const int64_t * a_strides, const int64_t * b_strides, const int64_t * d_strides, void * stream);
 /* batched (prefill) product: dst[t][n] = sum_k W[n][k] * x[t][k] (+ bias[n]) (+ resid[t][n]); W: n rows of k-quant blocks
  * (Q4_K/Q5_K/Q6_K with k % 256 == 0, or Q8_0/Q5_1 with k % 64 == 0), x: t rows of ldx floats, dst / resid: t rows of n floats, resid must not alias dst; W and x 16-byte aligned, ldx % 4 == 0.  Activations are quantized like the CPU backend does for that weight type (q8_K, or q8_0/q8_1 per 32 values),
- * then both operands run as fp16 on the tensor cores with fp32 accumulation.  ws: pb200_mul_mat_q_workspace_bytes(k, t). */
+ * then both operands run as fp16 on the tensor cores with fp32 accumulation.  ws: pb200_mul_mat_q_workspace_bytes(k, t) = tpad * (2 k + 4)
+ * bytes, tpad = t rounded up to the token tile: the fp16 activation image, then one f32 power-of-two scale per padded row that keeps
+ * every activation magnitude inside fp16's normal range. */
 PB200_API size_t pb200_mul_mat_q_workspace_bytes(int64_t k, int64_t t);
 PB200_API int pb200_mul_mat_q(int type, const void * W, int64_t n, int64_t k, const float * x, int64_t ldx, int64_t t, float * dst,
                               const float * bias, const float * resid, void * ws, void * stream);

@@ -7,6 +7,8 @@
 // formulas (ggml-quants.c:2040-2065, 2390-2420, 2690-2725) evaluated in fp16 (exact integer q, fp16 sub-block scale and
 // offset, one fused multiply-add); both operands are fp16 on the tensor pipe with fp32 accumulation.  The result differs
 // from the integer-dot CPU value by a few fp16 roundings per product (NMSE ~1e-6; tests/test_gpu_mmq.py states the bound).
+// Operand range: each activation row is scaled by a power of two into [2^14, 2^15) before its fp16 rounding (k_mmq_prep) and the
+// epilogue undoes it, so any finite f32 activation works; the weights' sub-block scales d*sc below 2^-14 remain fp16 subnormals.
 //
 //   dst[t][n] = sum_k W[n][k] * X[t][k]        W: N x K k-quant rows, X: T x K f32, dst: T x N f32 (ggml layout)
 // Also the 32-element block types Q8_0 / Q5_1 (K % 64 == 0; activations quantized per 32 values like their CPU dot): Qwen2.5-72B's
@@ -16,8 +18,9 @@
 // tile of BN <= 128 columns).  The units of a launch, ordered tile by tile, are cut into one contiguous range per CTA (at most one CTA
 // per SM), so every SM gets the same number of 64-element MMA steps whatever N, K and T are.  A CTA walks its range segment by segment
 // (segment = its part of one tile); a segment that covers the tile's whole K stores its result, a partial one adds it into the
-// pre-zeroed dst with fp32 atomics (two or three addends per element: the order of fp32 adds is the only non-determinism, below the
-// kernel's own fp16 rounding).  Inside a CTA the pipeline never drains between segments (raw-block ring, A and B stages and their
+// pre-zeroed dst with fp32 atomics (one addend per CTA sharing the tile, up to ceil(ngrp / upc) + 1: 15 for K = 29 568, T = 24 on 132 SMs;
+// the order of fp32 adds is the only non-determinism, below the kernel's own fp16 rounding).  Bias and residual ride on the K group 0
+// segment only.  Inside a CTA the pipeline never drains between segments (raw-block ring, A and B stages and their
 // barriers run on CTA-wide counters):
 //   warps 0..7  two consumer warpgroups: warpgroup w issues 4 x wgmma.mma_async (M=64, N=BN, K=16, f16 in, f32 accumulators in
 //               registers) per step for weight rows [64w, 64w + 64) of the tile, keeps one step in flight, and at the end of a segment
@@ -57,6 +60,7 @@ struct MmqParams {
     int * abort_flag;      // host-mapped, raised by the wait watchdog
     const uint8_t * W;
     const uint8_t * B;     // activations, fp16, tiled [T/BN][K/64][BN x 128 B swizzled]
+    const float * rscale;  // [Tpad]: 2^-e_t, undoes the power-of-two row scale of the activation image (k_mmq_prep)
     float * dst;           // [T][N]
     const float * bias;    // [N] or null
     const float * resid;   // [T][N] or null: residual added in the epilogue
@@ -352,6 +356,15 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
             const int t0 = (tile / P.rtiles) * BN + 2 * (lane & 3);
             const int nrow = (tile % P.rtiles) * MMQ_BM + wg * 64 + (warp & 3) * 16 + (lane >> 2);
             const bool first = sbb == 0, whole = first && sbe == P.ngrp;   // bias / residual ride on the K group 0 segment
+            // undo the activation row scale (exact, a power of two) before bias and residual: t0 + 8 j + e < Tpad, rscale covers the padding
+#pragma unroll
+            for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+                for (int e = 0; e < 2; e++) {
+                    const float s = __ldg(P.rscale + t0 + 8 * j + e);
+                    acc[4 * j + e] = __fmul_rn(acc[4 * j + e], s);
+                    acc[4 * j + 2 + e] = __fmul_rn(acc[4 * j + 2 + e], s);
+                }
 #pragma unroll
             for (int i = 0; i < 2; i++) {
                 const int n = nrow + 8 * i;
@@ -379,7 +392,7 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
                             if (t < P.T) {
                                 const float y = __fadd_rn(__fadd_rn(acc[4 * (j0 + j) + 2 * i + e], bias), rv[2 * j + e]);
                                 if (whole) P.dst[(size_t) t * P.N + n] = y;
-                                else atomicAdd(&P.dst[(size_t) t * P.N + n], y);   // <= 3 addends onto 0
+                                else atomicAdd(&P.dst[(size_t) t * P.N + n], y);   // one addend per CTA sharing the tile, onto 0
                             }
                         }
                 }
@@ -490,13 +503,26 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
 // Fused producers of the activation (pre_kind): PRO_SILU_MUL = silu(x) * aux[t][k] (llm_build_ffn's SILU + MUL in front of ffn_down, the f32
 // product never goes to HBM), PRO_RMSNORM = rms_norm(x) * aux[k] (llm_build_norm in front of q|k|v and gate|up): the same arithmetic, rounding for rounding, as
 // k_silu_mul / k_rms_norm_rows followed by the plain pass.
+// Operand range: the values d*q of row t are written as fp16 of d*q*2^e_t, e_t chosen so that the row's largest |d*q| lands in
+// [2^14, 2^15) (e_t <= 126: rows whose largest value is below 2^-112 stay below that), and rscale[t] = 2^-e_t, which the consumers'
+// epilogue applies to the fp32 accumulators.  So no activation overflows fp16 (|x| >= 65 520 was inf) or falls into its subnormals
+// (rows with amax below ~1e-3 lost bits, below ~1e-7 were zero); where d*q was a normal fp16 already the scaled value is the old one
+// times 2^e_t and the result is bit-identical.  The row's q and d wait in shared memory (mmq_prep_smem) while the CTA reduces the max.
+static size_t mmq_prep_smem(int64_t K) { return (size_t) ((K + 255) / 256) * (256 + 8 * sizeof(float)); }   // int8 q[256] | f32 d[8] per 256 values
+
 __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, int64_t ldx, int T, int K, int BN, uint8_t * __restrict__ out,
-                                                  int blk32, int pre_kind, const float * __restrict__ aux, int64_t ld_aux, float eps) {
+                                                  float * __restrict__ rscale, int blk32, int pre_kind, const float * __restrict__ aux,
+                                                  int64_t ld_aux, float eps) {
+    extern __shared__ uint8_t prep_smem[];
+    __shared__ float s_max[8];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nblk = (K + 255) / 256;
+    int8_t * sq = reinterpret_cast<int8_t *>(prep_smem);                    // [nblk][256]
+    float * sd = reinterpret_cast<float *>(prep_smem + (size_t) nblk * 256);  // [nblk][8]: d of each 32 values
     const int t = blockIdx.x;                       // 0 .. Tpad-1
     const int b_bytes = BN * 128;
     const float nscale = pre_kind == PRO_RMSNORM && t < T ? block_rms_scale(x + (size_t) t * ldx, K, eps) : 1.f;   // k_rms_norm_rows' scale
+    float rmax = 0.f;                               // largest |d * q| this thread quantized
     for (int b = warp; b < nblk; b += 8) {
         float v[8];
         const bool live = b * 256 + lane * 8 < K;   // K % 32 == 0: a 4-lane group (one 32-block) is live or dead as a whole
@@ -526,9 +552,34 @@ __global__ void __launch_bounds__(256) k_mmq_prep(const float * __restrict__ x, 
             warp_argmax(amax, idx, &vmax);
             d = q8K_quant(v, amax, vmax, q);
         }
+        uint32_t packed[2];
+        int qsum;
+        pack_q8(q, packed, qsum);
+        *reinterpret_cast<uint2 *>(sq + (size_t) b * 256 + lane * 8) = make_uint2(packed[0], packed[1]);
+        if ((lane & 3) == 0) sd[b * 8 + (lane >> 2)] = d;
+#pragma unroll
+        for (int i = 0; i < 8; i++) rmax = fmaxf(rmax, fabsf(__fmul_rn(d, (float) q[i])));
+    }
+    rmax = warp_max(rmax);
+    if (lane == 0) s_max[warp] = rmax;
+    __syncthreads();
+    rmax = s_max[0];
+#pragma unroll
+    for (int i = 1; i < 8; i++) rmax = fmaxf(rmax, s_max[i]);
+    // e = 14 - floor(log2(rmax)) from the exponent field (a zero row keeps e = 0)
+    const int e = rmax > 0.f ? min(14 - (((__float_as_int(rmax) >> 23) & 0xff) - 127), 126) : 0;
+    const float up = __int_as_float((127 + e) << 23);
+    if (threadIdx.x == 0) rscale[t] = __int_as_float((127 - e) << 23);
+    for (int b = warp; b < nblk; b += 8) {
+        const bool live = b * 256 + lane * 8 < K;
+        const uint2 pq = *reinterpret_cast<const uint2 *>(sq + (size_t) b * 256 + lane * 8);
+        const float d = sd[b * 8 + (lane >> 2)];
         float f[8];
 #pragma unroll
-        for (int i = 0; i < 8; i++) f[i] = __fmul_rn(d, (float) q[i]);
+        for (int i = 0; i < 8; i++) {
+            const int qi = (int) (int8_t) (((i < 4 ? pq.x : pq.y) >> (8 * (i & 3))) & 0xff);
+            f[i] = __fmul_rn(__fmul_rn(d, (float) qi), up);
+        }
         // within every 4 consecutive k the order is (0,2,1,3): the weight expansion produces its half2 pairs that way
         const uint32_t h[4] = {pack_h2(f[0], f[2]), pack_h2(f[1], f[3]), pack_h2(f[4], f[6]), pack_h2(f[5], f[7])};
         const int k = b * 256 + lane * 8;
@@ -545,10 +596,10 @@ static int mmq_pick_bn(int T) {   // a power of two: one kernel instance per wid
     while (bn < T && bn < MMQ_BN_MAX) bn <<= 1;
     return bn;
 }
-size_t mmq_workspace_bytes(int64_t K, int64_t T) {
+size_t mmq_workspace_bytes(int64_t K, int64_t T) {   // the fp16 activation image [Tpad][K], then rscale [Tpad] f32
     const int BN = mmq_pick_bn((int) T);
     const int64_t tpad = (T + BN - 1) / BN * BN;
-    return (size_t) (tpad * K * 2);
+    return (size_t) (tpad * K * 2 + tpad * 4);
 }
 bool mmq_supported(int type, int64_t K) {
     if (is_kquant(type)) return K % 256 == 0 && K >= 256;
@@ -584,6 +635,8 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
     P.abort_flag = abort_flag();
     P.W = (const uint8_t *) W;
     P.B = (const uint8_t *) ws;
+    float * rscale = reinterpret_cast<float *>((uint8_t *) ws + (size_t) tpad * (size_t) K * 2);   // behind the image (mmq_workspace_bytes)
+    P.rscale = rscale;
     P.dst = dst;
     P.bias = bias;
     P.resid = resid;
@@ -610,9 +663,13 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
     const int grid_x = (int) ((total + upc - 1) / upc);
     const bool split = upc % P.ngrp != 0;      // some tile is shared by two CTAs: partial results meet in dst by atomic add
     if (!reuse_prep) {
-        k_mmq_prep<<<tpad, 256, 0, st>>>(x, ldx, (int) T, (int) K, BN, (uint8_t *) ws, is_kquant(type) ? 0 : 1, pre ? pre->kind : PRO_NONE,
-                                         pre ? pre->aux : nullptr, pre ? pre->ld_aux : 0, pre ? pre->eps : 0.f);
-        cudaError_t e0 = cudaGetLastError();
+        static FuncAttrCache prep_attr;
+        const size_t prep_smem = mmq_prep_smem(K);
+        cudaError_t e0 = ensure_dyn_smem(prep_attr, (const void *) k_mmq_prep, prep_smem, false);
+        if (e0 != cudaSuccess) return e0;
+        k_mmq_prep<<<tpad, 256, prep_smem, st>>>(x, ldx, (int) T, (int) K, BN, (uint8_t *) ws, rscale, is_kquant(type) ? 0 : 1, pre ? pre->kind : PRO_NONE,
+                                                 pre ? pre->aux : nullptr, pre ? pre->ld_aux : 0, pre ? pre->eps : 0.f);
+        e0 = cudaGetLastError();
         if (e0 != cudaSuccess) return e0;
     }
     if (split) {

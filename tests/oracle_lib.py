@@ -298,5 +298,34 @@ def synth_blocks(t: int, N: int, K: int, seed: int, scale: float = 1.0) -> np.nd
     return out.reshape(-1)
 
 
+# byte ranges of the quants and of the block scale d inside one block
+_QBYTES = {Q4_K: slice(16, 144), Q5_K: slice(16, 176), Q6_K: slice(0, 192), Q8_0: slice(2, 34), Q5_1: slice(4, 24)}
+_DBYTES = {Q4_K: slice(0, 2), Q5_K: slice(0, 2), Q6_K: slice(208, 210), Q8_0: slice(0, 2), Q5_1: slice(0, 2)}
+
+
+def edge_blocks(t: int, N: int, K: int, seed: int) -> np.ndarray:
+    """synth_blocks with the bit patterns random blocks (almost) never hold, by row r % 6: 0 random; 1 every quant byte 0x00; 2 every
+    quant byte 0xFF; 3 the type's extreme: Q8_0 q = -128, Q6_K sub-block scales -128 with q = -32, Q4_K / Q5_K 6-bit scales and mins all
+    63, Q5_1 offset m = 0 with q = 31; 4 d = 0 in every block; 5 d = 0 in every other block."""
+    be, bb = BLOCK[t]
+    b = synth_blocks(t, N, K, seed).reshape(N, K // be, bb)
+    q, dd = _QBYTES[t], _DBYTES[t]
+    b[1::6, :, q] = 0x00
+    b[2::6, :, q] = 0xFF
+    if t == Q8_0:
+        b[3::6, :, q] = 0x80
+    elif t == Q6_K:
+        b[3::6, :, q] = 0x00
+        b[3::6, :, 192:208] = 0x80
+    elif t in (Q4_K, Q5_K):
+        b[3::6, :, 4:16] = 0xFF
+    else:
+        b[3::6, :, 2:4] = 0x00
+        b[3::6, :, q] = 0xFF
+    b[4::6, :, dd] = 0x00
+    b[5::6, ::2, dd] = 0x00
+    return b.reshape(-1)
+
+
 def f32_to_f16_bits(a: np.ndarray) -> np.ndarray:
     return np.asarray(a, dtype=np.float32).astype(np.float16).view(np.uint16)

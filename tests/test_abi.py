@@ -46,9 +46,9 @@ def test_argument_validation_no_gpu(lib, pkg):
     assert not c.pb200_model_create(C.byref(hp), 0, 0, 2, 1, 1)   # n_embd % 256 != 0 -> NULL, no abort
     assert c.pb200_decode(None, 0, 0, None) == -4
     assert c.pb200_prefill(None, None, 1, 0, None) == -4
-    # batched tensor-core product: workspace = padded rows x K fp16; argument errors before any CUDA call
-    assert c.pb200_mul_mat_q_workspace_bytes(8192, 512) == 512 * 8192 * 2
-    assert c.pb200_mul_mat_q_workspace_bytes(8192, 20) == 32 * 8192 * 2      # 20 rows -> one 32-column tile
+    # batched tensor-core product: workspace = padded rows x (K fp16 + one f32 row scale); argument errors before any CUDA call
+    assert c.pb200_mul_mat_q_workspace_bytes(8192, 512) == 512 * (8192 * 2 + 4)
+    assert c.pb200_mul_mat_q_workspace_bytes(8192, 20) == 32 * (8192 * 2 + 4)      # 20 rows -> one 32-column tile
     assert c.pb200_mul_mat_q(12, None, 128, 256, None, 256, 8, None, None, None, None, None) == -1
     assert c.pb200_attn_prefill(None, None, None, None, 8, 2, 128, None, 4, 4, 0.1, None) == -1
 

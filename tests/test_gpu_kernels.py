@@ -67,6 +67,23 @@ def test_gemv_small_block_types_vs_oracle(cuda, lib, port, t, N, K):
     assert np.max(np.abs(got - want)) <= rel_tol(want)
 
 
+@pytest.mark.parametrize("t", O.QUANT_TYPES, ids=lambda t: O.TYPE_NAME[t])
+def test_gemv_weight_bit_patterns_vs_oracle(cuda, lib, port, t):
+    """The weight blocks of oracle_lib.edge_blocks (quant bytes all 0x00 / 0xFF, Q8_0 q = -128, Q6_K scale -128 with q = -32, scales and
+    mins of 63, d = 0) through the GEMV families above: k-quant ring; Q8_0 / Q5_1 on the ring (K % 128 == 0) and the per-warp kernels."""
+    for K in ([2048] if t in KQ else [2048, 1984]):
+        N = 96
+        W = O.edge_blocks(t, N, K, seed=K + t)
+        x = np.random.default_rng(K + t).standard_normal(K).astype(np.float32)
+        want = port.mul_mat(t, W, N, K, x)[0]
+        Wd, xd, ws = dev_u8(W), dev_f32(x), act_ws(lib, K)
+        y = torch.full((N,), float("nan"), device="cuda")
+        lib.check(lib.c.pb200_mul_mat_vec(t, ptr(Wd), N, K, ptr(xd), ptr(y), ptr(ws), None), "mul_mat_vec")
+        sync()
+        got = y.cpu().numpy()
+        assert np.max(np.abs(got - want)) <= rel_tol(want), (K, np.max(np.abs(got - want)), rel_tol(want))
+
+
 def test_gemv_golden_reference_quantized_weights(cuda, lib):
     """Weights quantized by the reference's own ggml_quantize_chunk (committed fixture), outputs of its CPU mul_mat."""
     from pathlib import Path
