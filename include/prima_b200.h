@@ -132,7 +132,7 @@ typedef struct pb200_gemv_mat {
     float * y;             /* [n]  y = W . act (+ add[row]) */
     const float * add;     /* optional [n]: bias or residual added in the epilogue (ggml ADD node folded in) */
 } pb200_gemv_mat;
-/* Up to 3 matrices sharing one activation of length k (k % 256 == 0, k <= 28672), ONE launch.  prologue:
+/* Up to 3 matrices sharing one activation of length k (k % 256 == 0, k <= 29696), ONE launch.  prologue:
  *   0  act_ws already holds the q8_K activation (pb200_quantize_act, or pb200_attn_ggml with act_ws_out)
  *   1  act = q8_K( rms_norm(in0, eps) * in1 )     ggml RMS_NORM + MUL by the norm weight   (llm_build_norm, src/llama.cpp:9772-9802)
  *   2  act = q8_K( silu(in0) * in1 )              ggml UNARY(SILU) + MUL                    (llm_build_ffn, src/llama.cpp:9858-9907)

@@ -113,6 +113,94 @@ def test_engine_llama3_70b_layer_shapes_vs_compiled_reference(cuda, pkg):
     eng.close()
 
 
+def nmse(a, b):
+    return float(np.sum((a - b) ** 2) / np.sum(b ** 2))
+
+
+def check_tie_split_parity(got, want):
+    """The multi-token bar without the first-token exactness, for runs that split on an activation-quantization tie at token 0: every
+    token within 0.05 max-abs (the reference's AVX2 / AVX-512 self-divergence, DESIGN.md), NMSE below 2e-3, >= 90 % equal greedy tokens."""
+    e = np.max(np.abs(got - want), axis=1)
+    assert np.max(e) < 0.05, e
+    assert nmse(got, want) < 2e-3, nmse(got, want)
+    assert np.mean(got.argmax(1) == want.argmax(1)) >= 0.9
+
+
+def test_engine_qwen25_72b_layer_shapes_vs_port(cuda, pkg, port):
+    """2 full-size Qwen2.5-72B layers (n_embd 8192, 64/8 heads, n_ff 29 568, q5_K_M: biased q|k|v at K 8192, ffn_down on Q5_1 then Q8_0
+    behind the silu * mul -> q8_0 / q8_1 producer with the residual, v Q5_K then Q6_K) decoded token by token against the oracle port.
+    Token 0 of this model holds near-tie q8_K codes (see the next test): on an H100 the engine's hidden[0] is 1.2e-2 from the port's and
+    1.2e-2 from the reference's, while the port is 8e-3 from the reference, so the bar is check_tie_split_parity, plus hidden[0] NMSE."""
+    tm, toks = RG.engine_q72b_model()
+    toks = toks[:8]
+    want, hid = tm.port_decode(port, toks)
+    eng = tm.load_engine(pkg)
+    got = np.zeros_like(want)
+    for i, t in enumerate(toks):
+        eng.decode(int(t), i, got[i])
+        if i == 0:
+            assert nmse(eng.hidden(), hid[0]) < 2e-3
+    eng.close()
+    check_tie_split_parity(got, want)
+
+
+def test_engine_qwen25_72b_layer_shapes_vs_compiled_reference(cuda, pkg):
+    """The same model against the reference CPU backend's recorded logits (its AVX2 build).  At token 0 one q8_K code of layer 1's
+    attention input sits on a rounding tie (x * 127 / amax = -28.49999): the reference rounds it to -29, the port to -28 from an input
+    one fp32 ulp away, and that one code moves hidden[0] by 8e-3 and the logits by 2.3e-2.  The reference's own AVX2 and AVX-512
+    builds flip codes the same way on this model from token 2 on (up to 3.3e-2 on the logits), so the first-token exactness of
+    check_decode_parity cannot hold here; the bars are what the reference meets against itself: every token within 0.05 max-abs
+    (DESIGN.md, the 1e-3 logits bar), NMSE over the run below 2e-3, the same greedy tokens on >= 90 % of the steps."""
+    tm, toks = RG.engine_q72b_model()
+    z = np.load(G / "reference_golden.npz")
+    want, hid0 = z["engine_q72b_logits"], z["engine_q72b_hidden0"]
+    eng = tm.load_engine(pkg)
+    got = np.zeros_like(want)
+    for i, t in enumerate(toks[: len(want)]):
+        eng.decode(int(t), i, got[i])
+        if i == 0:
+            assert nmse(eng.hidden(), hid0) < 2e-3
+    eng.close()
+    check_tie_split_parity(got, want)
+
+
+def test_prefill_qwen25_72b_layer_shapes_vs_compiled_reference(cuda, pkg):
+    """The same model's 24-token prompt through pb200_prefill (tensor-core mat-muls at K 29 568 on Q5_1 / Q8_0 with the residual, the bias
+    epilogue on q|k|v), then 4 decode steps: against the reference's batched prompt + decode and the engine's own sequential decode, with
+    test_prefill_matches_sequential_decode_and_oracle's bars."""
+    tm, toks = RG.engine_q72b_model()
+    want = np.load(G / "reference_golden.npz")["engine_q72b_prefill_logits"]
+    T, nv = 24, tm.hp["n_vocab"]
+    eng = tm.load_engine(pkg)
+    seq = np.zeros((T, nv), np.float32)
+    for i, t in enumerate(toks[:T]):
+        eng.decode(int(t), i, seq[i])
+    eng.kv_clear()
+    got = np.zeros((len(toks), nv), np.float32)
+    eng.prefill(toks[:T], 0, got[T - 1])
+    for i in range(T, len(toks)):
+        eng.decode(int(toks[i]), i, got[i])
+    eng.close()
+    assert nmse(got[T - 1], want[T - 1]) < 2e-3, nmse(got[T - 1], want[T - 1])
+    assert nmse(got[T - 1], seq[T - 1]) < 1e-3, nmse(got[T - 1], seq[T - 1])
+    assert nmse(got[T:], want[T:]) < 2e-3, nmse(got[T:], want[T:])
+
+
+def test_engine_llama3_8b_layer_shapes_vs_port(cuda, pkg, port):
+    """2 Llama-3-8B-shape layers (n_embd 4096, 32/8 heads, n_ff 14 336: rpw 2 short rows with owner-only stages in q|k|v, wo, gate|up;
+    v on Q5_K then Q6_K, the wpr 2 ffn_down on Q4_K then Q6_K) decoded against the oracle port."""
+    tm = TinyModel(n_layer=2, n_embd=4096, n_head=32, n_head_kv=8, n_ff=14336, n_vocab=512, n_ctx=32, arch="llama", ftype="q4_K_M", seed=27,
+                   branch_scale=0.1)
+    toks = [(i * 7919 + 13) % 512 for i in range(8)]
+    want, _ = tm.port_decode(port, toks)
+    eng = tm.load_engine(pkg)
+    got = np.zeros_like(want)
+    for i, t in enumerate(toks):
+        eng.decode(int(t), i, got[i])
+    eng.close()
+    check_decode_parity(got, want)
+
+
 def test_engine_chaotic_model_statistics(cuda, pkg, port):
     """Unit-gain random net (chaotic): quantization flips are amplified layer by layer.  Bound the noise statistically:
     every token's logits stay within 0.2 max-abs (|logits| ~ 3), the median token within 1e-3... and tokens with no flip

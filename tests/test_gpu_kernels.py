@@ -39,7 +39,8 @@ def test_quantize_act_bit_exact(cuda, lib, port, t):
 
 
 @pytest.mark.parametrize("t", KQ, ids=lambda t: O.TYPE_NAME[t])
-@pytest.mark.parametrize("N,K", [(64, 256), (37, 512), (8, 2048), (129, 4096), (24, 8192), (19, 14336), (10, 28672)])
+@pytest.mark.parametrize("N,K", [(64, 256), (37, 512), (8, 2048), (129, 4096), (24, 8192), (19, 14336), (10, 28672),
+                                 (21, 29952), (9, 53248)])   # beyond the ring's 29 696: k_gemv_generic (aligned k-quant dots, scalar Q6_K)
 def test_gemv_kquant_vs_oracle(cuda, lib, port, t, N, K):
     W = O.synth_blocks(t, N, K, seed=N * 31 + K)
     rng = np.random.default_rng(K + N)
