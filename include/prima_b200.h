@@ -123,6 +123,31 @@ PB200_API int pb200_flash_attn_ext(const float * q, const void * k_f16, const vo
                                    int n_head, int n_head_kv, int n_kv, const int64_t * q_nb, const int64_t * k_nb, const int64_t * v_nb, int64_t mask_nb1,
                                    float scale, float max_bias, float logit_softcap, void * stream);
 
+/* ---- seeded sampling on the device: the chain gpt_sampler_init builds for temp > 0 without mirostat (common/sampling.cpp:140-224):
+ *   top-k -> top-p -> min-p -> temperature -> softmax -> dist (src/llama-sampling.cpp:91-165, 557-588, 624-684, 913-918, 66-89, 18-46)
+ * top_k <= 0: the whole vocabulary; top_p 1: off; min_p 0: off; min_keep as in the reference; temp <= 0: greedy (first index of
+ * the maximum, the same kernel as pb200_argmax_seq).  The draw is std::mt19937(seed) through std::discrete_distribution (two 32-bit
+ * outputs per draw; nothing is drawn when one token survives), so a sequence of draws follows the reference's generator.  Equal
+ * logits are ordered by ascending token id.  Penalties, logit bias, tail-free, typical, dynamic temperature, mirostat and grammars
+ * are not part of this chain.  Invalid parameters (NaN / inf, top_p outside (0, 1], min_p outside [0, 1), min_keep < 0) return
+ * PB200_EINVAL.  Where every softmax weight vanishes (a temperature so small that logit / temp overflows, a row of -inf) the token
+ * is the top one.  Top-p is cut where the exact running mass reaches p; the reference's float running sum over a whole vocabulary
+ * (top_k <= 0) can stop a little earlier (up to about 5e-4 of mass measured, a few dozen tokens of 130 000). */
+typedef struct pb200_sampling {
+    int32_t top_k;
+    float   top_p, min_p, temp;
+    int32_t min_keep;
+    uint32_t seed;             /* explicit: choosing a random seed (LLAMA_DEFAULT_SEED) is the host's business */
+} pb200_sampling;
+/* device memory one generator state takes (624 words + index, padded) */
+PB200_API size_t pb200_sampler_state_bytes(void);
+/* state_dev = std::mt19937(seed), enqueued on stream */
+PB200_API int pb200_sampler_seed(void * state_dev, uint32_t seed, void * stream);
+/* one token from logits[n_vocab] (device) -> *token_dev; advances state_dev.  One launch, no host synchronisation or allocation:
+ * capturable in a CUDA graph.  p->seed is not used here (pb200_sampler_seed seeds).  PB200_ENOTSUP when n_vocab / 16 logits exceed
+ * the device's shared memory per block (n_vocab above about 880 000 on an H100). */
+PB200_API int pb200_sample(const float * logits, int n_vocab, const pb200_sampling * p, void * state_dev, int32_t * token_dev, void * stream);
+
 /* ---- fused decode launches (what the engine is made of), for graph-level fusion in a host such as the ggml-backend plugin ---- */
 typedef struct pb200_gemv_mat {
     int32_t type;          /* k-quant type of W (Q4_K / Q5_K / Q6_K) */
@@ -228,8 +253,13 @@ PB200_API int pb200_set_tokpos_seq(pb200_model * m, int seq, int32_t token, int3
 /* greedy sampling on the device (ggml-cuda/argmax.cu:7): argmax of the slot's logits -> pb200_sample_device(m, seq); feed_back != 0 on a
  * shard that also holds the embedding writes it into the slot's token as well (single-GPU generation without a host round trip) */
 PB200_API int pb200_argmax_seq(pb200_model * m, int seq, int feed_back);
+/* seeded sampling per slot (the chain of pb200_sample): pb200_sampling_set_seq stores the parameters and seeds the slot's own generator
+ * with p->seed (on the model stream; call it outside any capture); pb200_sample_seq then works like pb200_argmax_seq with those
+ * parameters -> pb200_sample_device(m, seq), and with feed_back the slot's token.  PB200_ESTATE for a slot without parameters. */
+PB200_API int pb200_sampling_set_seq(pb200_model * m, int seq, const pb200_sampling * p);
+PB200_API int pb200_sample_seq(pb200_model * m, int seq, int feed_back);
 PB200_API int32_t * pb200_token_device(pb200_model * m, int seq);    /* int32[2]: {token, position} of the slot */
-PB200_API int32_t * pb200_sample_device(pb200_model * m, int seq);   /* int32: greedy token of the slot's last step */
+PB200_API int32_t * pb200_sample_device(pb200_model * m, int seq);   /* int32: the slot's last sample (pb200_argmax_seq or pb200_sample_seq) */
 PB200_API float * pb200_logits_device(pb200_model * m);      /* [n_vocab] f32 */
 PB200_API float * pb200_hidden_in_device(pb200_model * m);   /* [n_embd] f32: input of layer_begin (written by the previous stage) */
 PB200_API float * pb200_hidden_out_device(pb200_model * m);  /* [n_embd] f32: output of layer_end-1 */

@@ -264,4 +264,17 @@ int pb200_attn_prefill(const float * q, const void * k_cache_f16, const void * v
     return rc;
 }
 
+size_t pb200_sampler_state_bytes(void) { return sampler_state_bytes(); }
+int pb200_sampler_seed(void * state_dev, uint32_t seed, void * stream) {
+    if (!state_dev) return PB200_EINVAL;
+    return launch_sampler_seed(state_dev, seed, (cudaStream_t) stream);
+}
+int pb200_sample(const float * logits, int n_vocab, const pb200_sampling * p, void * state_dev, int32_t * token_dev, void * stream) {
+    if (!logits || n_vocab <= 0 || !state_dev || !token_dev || !sampling_params_ok(p)) return PB200_EINVAL;
+    const int rc = launch_sample(logits, n_vocab, *p, state_dev, token_dev, nullptr, (cudaStream_t) stream, false);
+    if (rc == (int) cudaErrorNotSupported) return PB200_ENOTSUP;
+    if (rc == 0) g_launches++;
+    return rc;
+}
+
 }  // extern "C"

@@ -84,7 +84,10 @@ struct pb200_model {
     RopeParams rp{};
     int n_seq = 1;                      // independent sequences with their own KV cache / token / position (the pipeline keeps one per stage in flight)
     std::vector<cudaGraphExec_t> graph_exec;   // one captured step per sequence slot
-    int32_t * sample_dev = nullptr;     // [n_seq] greedy token of the last step (pb200_argmax_seq)
+    int32_t * sample_dev = nullptr;     // [n_seq] token of the slot's last sample (pb200_argmax_seq / pb200_sample_seq)
+    uint8_t * sampler_state = nullptr;  // [n_seq] mt19937 states of pb200_sample_seq, sampler_state_bytes() apart
+    std::vector<pb200_sampling> sampling;   // per slot, valid where sampling_set
+    std::vector<char> sampling_set;
     uint64_t launches_per_step = 0;
     int64_t weight_bytes = 0;
     std::vector<void *> allocs;
@@ -486,6 +489,9 @@ int pb200_model_finalize(pb200_model * m) {
     CK(cudaMemset(m->tokpos_dev, 0, 16 * (size_t) m->n_seq));
     CK(m->alloc((void **) &m->sample_dev, 4 * (size_t) m->n_seq));
     CK(cudaMemset(m->sample_dev, 0, 4 * (size_t) m->n_seq));
+    if (m->with_head) CK(m->alloc((void **) &m->sampler_state, sampler_state_bytes() * (size_t) m->n_seq));
+    m->sampling.assign((size_t) m->n_seq, pb200_sampling{});
+    m->sampling_set.assign((size_t) m->n_seq, 0);
     CK(cudaMallocHost((void **) &m->tokpos_host, 16));
     if (m->with_head) CK(cudaMallocHost((void **) &m->logits_host, (size_t) hp.n_vocab * 4));
     rope_params_init(m->rp, hp.head_dim, hp.rope_mode, hp.n_ctx_orig, hp.rope_freq_base, hp.rope_freq_scale, 0.0f, 1.0f, 32.0f, 1.0f);
@@ -741,6 +747,10 @@ __global__ void __launch_bounds__(1024) k_argmax(const float * __restrict__ x, i
         if (lane == 0) { *out = bi; if (out2) *out2 = bi; }
     }
 }
+extern "C++" int pb::launch_argmax(const float * x, int n, int32_t * out, int32_t * out2, cudaStream_t stream, bool pdl) {
+    LaunchCfg lc(dim3(1), dim3(1024), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_argmax, x, n, out, out2);
+}
 __global__ void k_advance_pos(int32_t * tp) { pdl_trigger(); pdl_wait(); tp[1] += 1; }
 
 int pb200_decode_async(pb200_model * m, int32_t token, int32_t pos) {
@@ -816,6 +826,26 @@ int pb200_argmax_seq(pb200_model * m, int seq, int feed_back) {
     g_launches++;
     return (int) cudaLaunchKernelEx(&lc.cfg, k_argmax, (const float *) m->logits, (int) m->hp.n_vocab, m->sample_dev + seq,
                                     (int32_t *) (feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr));
+}
+// seeded sampling of the slot (sample.cu): parameters checked and the slot's generator seeded here, on the model stream
+int pb200_sampling_set_seq(pb200_model * m, int seq, const pb200_sampling * p) {
+    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
+    if (seq < 0 || seq >= m->n_seq || !sampling_params_ok(p)) return PB200_EINVAL;
+    cudaSetDevice(m->device);
+    CK(launch_sampler_seed(m->sampler_state + sampler_state_bytes() * (size_t) seq, p->seed, m->stream));
+    m->sampling[seq] = *p;
+    m->sampling_set[seq] = 1;
+    return 0;
+}
+// like pb200_argmax_seq with the slot's sampling parameters: -> sample_dev[seq] (and with feed_back the slot's token)
+int pb200_sample_seq(pb200_model * m, int seq, int feed_back) {
+    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
+    if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
+    if (!m->sampling_set[seq]) return PB200_ESTATE;
+    cudaSetDevice(m->device);
+    g_launches++;
+    return launch_sample((const float *) m->logits, (int) m->hp.n_vocab, m->sampling[seq], m->sampler_state + sampler_state_bytes() * (size_t) seq,
+                         m->sample_dev + seq, feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr, m->stream, true);
 }
 int32_t * pb200_token_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->tokpos_dev + 4 * seq : nullptr; }
 int32_t * pb200_sample_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->sample_dev + seq : nullptr; }

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "../../include/prima_b200.h"
 #include "common.cuh"
 
 namespace pb {
@@ -174,6 +175,16 @@ cudaError_t launch_mmq(int type, const void * W, int64_t N, int64_t K, const flo
 // resid: [T][N] added in the epilogue (must not alias dst).  reuse_prep: ws already holds this x (same K, T) from the previous launch_mmq
 // on the stream (q|k|v and gate|up share one activation: the q8_K -> fp16 tiling pass runs once)
 int launch_get_rows(const void * table, int type, int K, const int32_t * ids, int n_ids, float * y, cudaStream_t stream, bool pdl);
+
+// greedy token: first index of the maximum of x[n] -> *out (and *out2 if set); the engine's k_argmax
+int launch_argmax(const float * x, int n, int32_t * out, int32_t * out2, cudaStream_t stream, bool pdl);
+// seeded sampling (sample.cu): the reference's top-k / top-p / min-p / temperature / dist chain over x[n] -> *out (and *out2 if set),
+// one clustered launch; temp <= 0 launches launch_argmax.  state: sampler_state_bytes() of device memory seeded by launch_sampler_seed.
+// cudaErrorNotSupported when a slice of n / 16 logits exceeds the device's shared memory.
+size_t sampler_state_bytes();
+bool sampling_params_ok(const pb200_sampling * p);   // finite, top_p in (0, 1], min_p in [0, 1), min_keep >= 0
+int launch_sampler_seed(void * state, uint32_t seed, cudaStream_t stream);
+int launch_sample(const float * x, int n, const pb200_sampling & p, void * state, int32_t * out, int32_t * out2, cudaStream_t stream, bool pdl);
 
 // element-wise helpers for the plugin
 int launch_binary(int op /*0 add, 1 mul*/, const float * a, const float * b, float * y, int64_t n, int64_t nb /*b broadcast period*/, cudaStream_t stream);

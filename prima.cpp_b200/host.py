@@ -31,6 +31,20 @@ class HParams(C.Structure):
                [(n, C.c_float) for n in ("rope_freq_base", "rope_freq_scale", "rms_eps")]
 
 
+class Sampling(C.Structure):
+    """pb200_sampling: the reference's sampler chain (top-k -> top-p -> min-p -> temperature -> dist); temp <= 0 is greedy."""
+    _fields_ = [("top_k", C.c_int32), ("top_p", C.c_float), ("min_p", C.c_float), ("temp", C.c_float), ("min_keep", C.c_int32),
+                ("seed", C.c_uint32)]
+
+
+def sampling(top_k: int = 40, top_p: float = 0.95, min_p: float = 0.05, temp: float = 0.8, min_keep: int = 0, seed: int | None = None) -> Sampling:
+    """Defaults of llama-cli (common/common.h:103-137); seed None draws a random one, like LLAMA_DEFAULT_SEED."""
+    if seed is None:
+        import secrets
+        seed = secrets.randbits(32)
+    return Sampling(int(top_k), float(top_p), float(min_p), float(temp), int(min_keep), int(seed) & 0xFFFFFFFF)
+
+
 class Pb200Error(RuntimeError):
     pass
 
@@ -107,6 +121,11 @@ class Lib:
         for n in ("pb200_token_device", "pb200_sample_device"):
             getattr(c, n).restype = vp
             getattr(c, n).argtypes = [vp, C.c_int]
+        c.pb200_sampler_state_bytes.restype = C.c_size_t
+        c.pb200_sampler_seed.argtypes = [vp, C.c_uint32, vp]
+        c.pb200_sample.argtypes = [vp, C.c_int, C.POINTER(Sampling), vp, vp, vp]
+        c.pb200_sampling_set_seq.argtypes = [vp, C.c_int, C.POINTER(Sampling)]
+        c.pb200_sample_seq.argtypes = [vp, C.c_int, C.c_int]
 
     @classmethod
     def get(cls) -> "Lib":
@@ -117,6 +136,18 @@ class Lib:
     def check(self, rc: int, what: str = "") -> None:
         if rc != 0:
             raise Pb200Error(f"{what}: {self.c.pb200_error_string(rc).decode()} ({rc})")
+
+    def sampler_state_bytes(self) -> int:
+        return self.c.pb200_sampler_state_bytes()
+
+    def sampler_seed(self, state_ptr: int, seed: int, stream: int = 0) -> None:
+        """state = std::mt19937(seed) in device memory of sampler_state_bytes()."""
+        self.check(self.c.pb200_sampler_seed(C.c_void_p(state_ptr), seed & 0xFFFFFFFF, C.c_void_p(stream)), "sampler_seed")
+
+    def sample(self, logits_ptr: int, n_vocab: int, p: Sampling, state_ptr: int, token_ptr: int, stream: int = 0) -> None:
+        """pb200_sample: one token from n_vocab device logits into the int32 at token_ptr (enqueued on stream)."""
+        self.check(self.c.pb200_sample(C.c_void_p(logits_ptr), n_vocab, C.byref(p), C.c_void_p(state_ptr), C.c_void_p(token_ptr), C.c_void_p(stream)),
+                   "sample")
 
 
 class Model:
@@ -242,6 +273,16 @@ class Model:
 
     def argmax_seq(self, seq: int, feed_back: bool = False) -> None:
         self.lib.check(self.lib.c.pb200_argmax_seq(self.h, seq, int(feed_back)), "argmax_seq")
+
+    def set_sampling(self, seq: int, top_k: int = 40, top_p: float = 0.95, min_p: float = 0.05, temp: float = 0.8, min_keep: int = 0,
+                     seed: int | None = None) -> None:
+        """Sampling parameters of slot seq (llama-cli's defaults); seeds the slot's generator (None: a random seed)."""
+        p = sampling(top_k, top_p, min_p, temp, min_keep, seed)
+        self.lib.check(self.lib.c.pb200_sampling_set_seq(self.h, seq, C.byref(p)), "sampling_set_seq")
+
+    def sample_seq(self, seq: int, feed_back: bool = False) -> None:
+        """argmax_seq with the slot's sampling parameters: the token goes to sample_ptr(seq) (and with feed_back to the slot)."""
+        self.lib.check(self.lib.c.pb200_sample_seq(self.h, seq, int(feed_back)), "sample_seq")
 
     def token_ptr(self, seq: int) -> int:
         return self.lib.c.pb200_token_device(self.h, seq)
