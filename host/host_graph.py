@@ -75,6 +75,13 @@ def load(with_plugin: bool = True, with_cudaref: bool = False):
     g.lgh_decode.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_int]
     g.lgh_get_hidden.argtypes = [vp, vp]
     g.lgh_phase_seconds.argtypes = [vp, C.POINTER(C.c_double)]
+    g.lgh_kv_seq_rm.argtypes = [vp, C.c_int32, C.c_int32]
+    g.lgh_kv_seq_add.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32]
+    g.lgh_kv_cells.argtypes = [vp, vp]
+    g.lgh_kshift_unsupported_nodes.argtypes = [vp]
+    g.lgh_kshift_nodes.argtypes = [vp]
+    g.lgh_k_shifts.restype = C.c_uint64
+    g.lgh_k_shifts.argtypes = [vp]
     _libs = (g, plug)
     return _libs
 
@@ -145,6 +152,36 @@ class HostModel:
 
     def kv_clear(self) -> None:
         self.g.lgh_kv_clear(self.h)
+
+    def kv_seq_rm(self, p0: int, p1: int) -> None:
+        """llama_kv_cache_seq_rm of the one sequence: cells holding positions [p0, p1) become empty (holes)."""
+        self.g.lgh_kv_seq_rm(self.h, int(p0), int(p1))
+
+    def kv_seq_add(self, p0: int, p1: int, delta: int) -> None:
+        """llama_kv_cache_seq_add: cells holding positions [p0, p1) now hold position + delta; the next decode first runs the
+        K-shift graph (one in-place f16 ROPE per layer) on the backend."""
+        self.g.lgh_kv_seq_add(self.h, int(p0), int(p1), int(delta))
+
+    def kv_cells(self):
+        """Position held by each cell (-1 = empty)."""
+        import numpy as np
+        out = np.empty(self.hp["n_ctx"], dtype=np.int32)
+        self.g.lgh_kv_cells(self.h, out.ctypes.data_as(C.c_void_p))
+        return out
+
+    @property
+    def kshift_unsupported_nodes(self) -> int:
+        """Non-view nodes of the K-shift graph the backend does not support (the scheduler aborts on such a node of a cache it owns)."""
+        return self.g.lgh_kshift_unsupported_nodes(self.h)
+
+    @property
+    def kshift_nodes(self) -> int:
+        return self.g.lgh_kshift_nodes(self.h)
+
+    @property
+    def k_shifts(self) -> int:
+        """K-shift graphs computed so far."""
+        return self.g.lgh_k_shifts(self.h)
 
     def phase_seconds(self) -> dict:
         """Host seconds since the last call in: graph (re)build + allocation, input upload, graph_compute (enqueue), wait + logits read."""

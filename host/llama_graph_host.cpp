@@ -61,6 +61,20 @@ struct lgh_ctx {
     ggml_tensor *inp_tokens = nullptr, *inp_pos = nullptr, *kq_mask = nullptr, *logits = nullptr, *l_out = nullptr;
     std::vector<ggml_tensor *> k_views, v_views;
     std::vector<float> mask_host;
+    // the KV cells of the one sequence (llama_kv_cell / llama_kv_cache, src/llama.cpp:2860-2960): a cell keeps its slot and carries
+    // the position stored in it (-1 = empty) and the RoPE delta accumulated since the last K-shift.  Until the first seq_rm / seq_add
+    // after a clear the cells are not consulted (`managed` false): a token at position p goes to cell p, as it always did here.
+    struct cell { int32_t pos = -1, delta = 0; };
+    std::vector<cell> cells;
+    uint32_t head = 0, used = 0;
+    bool managed = false, has_shift = false;
+    // the K-shift graph of build_k_shift (src/llama.cpp:10665-10719): its own context, built once; inp_K_shift lives in a buffer of
+    // the backend (its own allocator, like the scheduler's for this graph), every other node is an in-place view of a K cache
+    ggml_context * kctx = nullptr;
+    ggml_gallocr_t kgalloc = nullptr;
+    ggml_cgraph * kgf = nullptr;
+    ggml_tensor * inp_k_shift = nullptr;
+    uint64_t n_k_shifts = 0;
     uint64_t n_graph_builds = 0;
     double t_build = 0, t_set = 0, t_enqueue = 0, t_get = 0;   // host seconds spent per phase (diagnostics for bench.py)
 };
@@ -118,12 +132,15 @@ void * lgh_create(const lgh_hparams * hp, const int32_t * types, const char * ba
     c->wbuf = ggml_backend_alloc_ctx_tensors(c->wctx, c->backend);
     if (!c->wbuf) { fprintf(stderr, "lgh: weight buffer allocation failed\n"); ggml_free(c->wctx); ggml_backend_free(c->backend); delete c; return nullptr; }
     ggml_backend_buffer_clear(c->wbuf, 0);
+    c->cells.resize((size_t) hp->n_ctx);
     return c;
 }
 
 void lgh_free(void * p) {
     lgh_ctx * c = (lgh_ctx *) p;
     if (!c) return;
+    if (c->kgalloc) ggml_gallocr_free(c->kgalloc);
+    if (c->kctx) ggml_free(c->kctx);
     if (c->gctx) ggml_free(c->gctx);
     if (c->galloc) ggml_gallocr_free(c->galloc);
     if (c->wbuf) ggml_backend_buffer_free(c->wbuf);
@@ -165,6 +182,128 @@ void lgh_kv_clear(void * p) {
         ggml_backend_tensor_set(l.k, z.data(), 0, z.size());
         ggml_backend_tensor_set(l.v, z.data(), 0, z.size());
     }
+    for (auto & cl : c->cells) cl = lgh_ctx::cell();   // llama_kv_cache_clear (src/llama.cpp:4230-4243)
+    c->head = c->used = 0;
+    c->managed = c->has_shift = false;
+}
+
+// llama_kv_cache_seq_rm of the one sequence (src/llama.cpp:4245-4316, transformer branch): cells with pos in [p0, p1) become empty
+int lgh_kv_seq_rm(void * p, int32_t p0, int32_t p1) {
+    lgh_ctx * c = (lgh_ctx *) p;
+    c->managed = true;   // from here until the next clear, lgh_decode places tokens like llama_decode does
+    const uint32_t size = (uint32_t) c->cells.size();
+    uint32_t new_head = size;
+    if (p0 < 0) p0 = 0;
+    if (p1 < 0) p1 = INT32_MAX;
+    for (uint32_t i = 0; i < size; i++) {
+        lgh_ctx::cell & cl = c->cells[i];
+        if (cl.pos >= p0 && cl.pos < p1) {
+            cl.pos = -1;
+            c->used--;
+            if (new_head == size) new_head = i;
+        }
+    }
+    if (new_head != size && new_head < c->head) c->head = new_head;
+    return 0;
+}
+// llama_kv_cache_seq_add (src/llama.cpp:4378-4427): cells with pos in [p0, p1) move by delta in position (not in slot); the K rows
+// are re-rotated by the accumulated delta at the next lgh_decode
+int lgh_kv_seq_add(void * p, int32_t p0, int32_t p1, int32_t delta) {
+    lgh_ctx * c = (lgh_ctx *) p;
+    c->managed = true;   // from here until the next clear, lgh_decode places tokens like llama_decode does
+    const uint32_t size = (uint32_t) c->cells.size();
+    uint32_t new_head = size;
+    if (p0 < 0) p0 = 0;
+    if (p1 < 0) p1 = INT32_MAX;
+    if (p0 == p1) return 0;
+    for (uint32_t i = 0; i < size; i++) {
+        lgh_ctx::cell & cl = c->cells[i];
+        if (cl.pos >= p0 && cl.pos < p1) {
+            c->has_shift = true;
+            cl.pos += delta;
+            cl.delta += delta;
+            if (cl.pos < 0) {
+                cl.pos = -1;
+                c->used--;
+                if (new_head == size) new_head = i;
+            }
+        }
+    }
+    c->head = new_head != size ? new_head : 0;
+    return 0;
+}
+// position stored in each cell (-1 = empty), n_ctx entries
+void lgh_kv_cells(void * p, int32_t * pos_out) {
+    lgh_ctx * c = (lgh_ctx *) p;
+    for (size_t i = 0; i < c->cells.size(); i++) pos_out[i] = c->cells[i].pos;
+}
+
+// build_k_shift: one in-place ROPE per layer on the whole f16 K cache viewed as [head_dim, n_head_kv, n_ctx], positions = the cells'
+// deltas (inp_K_shift)
+static bool build_k_shift(lgh_ctx * c) {
+    if (c->kgf) return true;
+    const lgh_hparams & hp = c->hp;
+    const int64_t D = hp.head_dim, HK = hp.n_head_kv, n_ctx = hp.n_ctx;
+    const size_t max_nodes = (size_t) 16 + 4 * (size_t) hp.n_layer;
+    ggml_init_params ip = { ggml_tensor_overhead() * max_nodes + ggml_graph_overhead_custom(max_nodes, false) + (1u << 16), nullptr, true };
+    c->kctx = ggml_init(ip);
+    c->kgf = ggml_new_graph_custom(c->kctx, max_nodes, false);
+    c->inp_k_shift = ggml_new_tensor_1d(c->kctx, GGML_TYPE_I32, n_ctx);
+    ggml_set_input(c->inp_k_shift);
+    for (lgh_layer & L : c->L) {
+        ggml_tensor * k = ggml_view_3d(c->kctx, L.k, D, HK, n_ctx, ggml_row_size(L.k->type, D), ggml_row_size(L.k->type, D * HK), 0);
+        ggml_tensor * t = ggml_rope_ext_inplace(c->kctx, k, c->inp_k_shift, c->rope_ff, (int) D, hp.rope_mode, hp.n_ctx_orig, hp.rope_freq_base,
+                                                hp.rope_freq_scale, 0.0f, 1.0f, 32.0f, 1.0f);
+        ggml_build_forward_expand(c->kgf, t);
+    }
+    // only inp_K_shift needs memory: every other node is a view of a K cache
+    c->kgalloc = ggml_gallocr_new(ggml_backend_get_default_buffer_type(c->backend));
+    return ggml_gallocr_alloc_graph(c->kgalloc, c->kgf);
+}
+// llama_kv_cache_update_internal (src/llama.cpp:19102-19134): run the K-shift graph on the context's backend, then clear the deltas
+static bool apply_k_shift(lgh_ctx * c) {
+    if (!c->has_shift) return true;
+    if (!build_k_shift(c)) return false;
+    std::vector<int32_t> d(c->cells.size());
+    for (size_t i = 0; i < d.size(); i++) d[i] = c->cells[i].delta;   // llama_set_k_shift (:17262-17273)
+    ggml_backend_tensor_set(c->inp_k_shift, d.data(), 0, d.size() * sizeof(int32_t));
+    if (ggml_backend_graph_compute(c->backend, c->kgf) != GGML_STATUS_SUCCESS) return false;
+    c->has_shift = false;
+    for (auto & cl : c->cells) cl.delta = 0;
+    c->n_k_shifts++;
+    return true;
+}
+// non-view nodes of the K-shift graph the backend does not support (what ggml_backend_sched checks for a node whose source is a
+// pre-allocated tensor in this backend's buffer); -1 if it could not be built
+int lgh_kshift_unsupported_nodes(void * p) {
+    lgh_ctx * c = (lgh_ctx *) p;
+    if (!build_k_shift(c)) return -1;
+    int n = 0;
+    for (int i = 0; i < ggml_graph_n_nodes(c->kgf); i++) {
+        ggml_tensor * t = ggml_graph_node(c->kgf, i);
+        if (t->op == GGML_OP_NONE || t->op == GGML_OP_RESHAPE || t->op == GGML_OP_VIEW || t->op == GGML_OP_PERMUTE || t->op == GGML_OP_TRANSPOSE) continue;
+        if (!ggml_backend_supports_op(c->backend, t)) n++;
+    }
+    return n;
+}
+int lgh_kshift_nodes(void * p) { lgh_ctx * c = (lgh_ctx *) p; return build_k_shift(c) ? ggml_graph_n_nodes(c->kgf) : -1; }
+uint64_t lgh_k_shifts(void * p) { return ((lgh_ctx *) p)->n_k_shifts; }
+
+// llama_kv_cache_find_slot, transformer branch (src/llama.cpp:3998-4215): the first run of n_tokens empty cells from head
+static int find_slot(lgh_ctx * c, int n_tokens) {
+    const uint32_t size = (uint32_t) c->cells.size();
+    if ((uint32_t) n_tokens > size) return -1;
+    uint32_t n_tested = 0;
+    while (true) {
+        if (c->head + n_tokens > size) { n_tested += size - c->head; c->head = 0; continue; }
+        bool found = true;
+        for (int i = 0; i < n_tokens; i++) {
+            if (c->cells[c->head + i].pos >= 0) { found = false; c->head += i + 1; n_tested += i + 1; break; }
+        }
+        if (found) break;
+        if (n_tested >= size) return -1;
+    }
+    return (int) c->head;
 }
 uint64_t lgh_graph_builds(void * p) { return ((lgh_ctx *) p)->n_graph_builds; }
 int lgh_graph_nodes(void * p) { lgh_ctx * c = (lgh_ctx *) p; return c->gf ? ggml_graph_n_nodes(c->gf) : 0; }
@@ -289,15 +428,36 @@ int lgh_reserve(void * p, int n_tokens_max) {
     return reserve_compute_buffer(g) ? 0 : -2;
 }
 
-// n_tokens tokens at positions pos0 .. pos0+n_tokens-1 (kv_head = pos0), HOST buffers in and out.
+// n_tokens tokens at positions pos0 .. pos0+n_tokens-1, HOST buffers in and out.  The tokens are stored from kv_head = pos0, or, once
+// lgh_kv_seq_rm / lgh_kv_seq_add have been called since the last clear, in the first run of empty cells from the search head (a pending
+// K-shift runs first).
 // logits: [n_tokens][n_vocab] if all_logits, else [n_vocab] of the last token.  Returns 0 on success.
 int lgh_decode(void * p, const int32_t * tokens, int n_tokens, int pos0, float * logits, int all_logits) {
     lgh_ctx * g = (lgh_ctx *) p;
     const lgh_hparams & hp = g->hp;
     if (n_tokens <= 0 || pos0 < 0 || pos0 + n_tokens > hp.n_ctx) return -1;
     const int64_t EK = (int64_t) hp.n_head_kv * hp.head_dim;
+    if (!apply_k_shift(g)) return -2;   // llama_kv_cache_update before the slot search (src/llama.cpp:18433)
+    // the destination cell of the first token: its position until the cells are managed, else the reference's slot search
+    int cell0 = pos0;
+    if (g->managed) {
+        if (g->head > g->used + 2 * (uint32_t) n_tokens) g->head = 0;   // src/llama.cpp:18437-18440
+        cell0 = find_slot(g, n_tokens);
+        if (cell0 < 0) return -4;
+    }
+    for (int i = 0; i < n_tokens; i++) {
+        lgh_ctx::cell & cl = g->cells[(size_t) (cell0 + i)];
+        if (cl.pos < 0) g->used++;
+        cl.pos = pos0 + i;
+    }
+    g->head = (uint32_t) (cell0 + n_tokens) >= g->cells.size() ? 0 : (uint32_t) (cell0 + n_tokens);   // :18578-18586
     // kv_self.n = min(size, max(pad, GGML_PAD(cell_max, pad))), pad = 32 when FA off (src/llama.cpp:4485, 18442-18451)
-    int64_t n_kv = ((pos0 + n_tokens + 31) / 32) * 32;
+    int64_t cell_max = pos0 + n_tokens;
+    if (g->managed) {
+        cell_max = 0;
+        for (int64_t i = (int64_t) g->cells.size(); i > 0; i--) if (g->cells[(size_t) (i - 1)].pos >= 0) { cell_max = i; break; }
+    }
+    int64_t n_kv = ((cell_max + 31) / 32) * 32;
     if (n_kv < 32) n_kv = 32;
     if (n_kv > hp.n_ctx) n_kv = hp.n_ctx;
     double t0 = now_s();
@@ -311,17 +471,20 @@ int lgh_decode(void * p, const int32_t * tokens, int n_tokens, int pos0, float *
     // re-point the cache store views at kv_head (what a rebuilt graph would carry in view_offs)
     for (size_t iv = 0; iv < g->k_views.size(); iv++) {
         ggml_tensor * kv = g->k_views[iv], * vv = g->v_views[iv];
-        kv->view_offs = ggml_row_size(kv->type, EK) * (size_t) pos0;
+        kv->view_offs = ggml_row_size(kv->type, EK) * (size_t) cell0;
         kv->data = (char *) kv->view_src->data + kv->view_offs;
-        vv->view_offs = (size_t) pos0 * ggml_element_size(vv);
+        vv->view_offs = (size_t) cell0 * ggml_element_size(vv);
         vv->data = (char *) vv->view_src->data + vv->view_offs;
     }
     std::vector<int32_t> posv(n_tokens);
     for (int i = 0; i < n_tokens; i++) posv[i] = pos0 + i;
     const int64_t n_tok_pad = GGML_PAD(n_tokens, GGML_KQ_MASK_PAD);
     g->mask_host.resize((size_t) (n_kv * n_tok_pad));
-    for (int64_t j = 0; j < n_tok_pad; j++)      // llama_set_inputs causal mask (src/llama.cpp:17330-17380)
-        for (int64_t i = 0; i < n_kv; i++) g->mask_host[(size_t) (j * n_kv + i)] = (j < n_tokens && i <= pos0 + j) ? 0.0f : -INFINITY;
+    for (int64_t j = 0; j < n_tok_pad; j++)      // llama_set_inputs causal mask (src/llama.cpp:17330-17380): empty cells and later positions hidden
+        for (int64_t i = 0; i < n_kv; i++) {
+            const int32_t cp = g->managed ? g->cells[(size_t) i].pos : (int32_t) i;
+            g->mask_host[(size_t) (j * n_kv + i)] = (j < n_tokens && cp >= 0 && cp <= pos0 + j) ? 0.0f : -INFINITY;
+        }
     ggml_backend_tensor_set(g->inp_tokens, tokens, 0, sizeof(int32_t) * (size_t) n_tokens);
     ggml_backend_tensor_set(g->inp_pos, posv.data(), 0, sizeof(int32_t) * (size_t) n_tokens);
     ggml_backend_tensor_set(g->kq_mask, g->mask_host.data(), 0, sizeof(float) * g->mask_host.size());

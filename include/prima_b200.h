@@ -13,6 +13,9 @@
  *   pb200_quantize_act      quantize_q8_1 quantize.cu:4-38; CPU: quantize_row_q8_K_ref ggml-quants.c:3785-3822
  *   pb200_rms_norm          ggml_cuda_op_rms_norm norm.cu:206-224; CPU ggml.c:11950-11996
  *   pb200_rope              ggml_cuda_op_rope rope.cu:188-271; CPU ggml.c:14143-14266
+ *   pb200_rope_f16          the same on f16 rows (rope.cu:200-262); CPU ggml.c:14269-14380
+ *   pb200_kv_seq_shift      llama_kv_cache_seq_rm + seq_add (src/llama.cpp:4378-4427) and the K-shift graph of build_k_shift
+ *                           (:10665-10719) that llama_kv_cache_update_internal runs at the next decode (:19102-19134)
  *   pb200_soft_max          ggml_cuda_op_soft_max softmax.cu:170-206; CPU ggml.c:13783-13880
  *   pb200_attn_decode       FA-off attention chain: ggml_cuda_mul_mat_batched_cublas x2 + soft_max + cont,
  *                           ggml-cuda.cu:1737-1881; graph src/llama.cpp:10032-10165
@@ -85,6 +88,12 @@ PB200_API int pb200_rms_norm(const float * x, float * y, int64_t n, int64_t nrow
 PB200_API int pb200_rope(const float * x, float * y, int64_t n_tokens, int n_head, int head_dim, int n_dims, int mode, const int32_t * pos,
                          float freq_base, float freq_scale, float ext_factor, float attn_factor, float beta_fast, float beta_slow,
                          int n_ctx_orig, const float * freq_factors, void * stream);
+/* GGML_OP_ROPE on f16 rows (ggml_compute_forward_rope_f16, ggml.c:14269-14380): x, y contiguous f16 [n_rows][n_head][head_dim], row t
+ * rotated by pos[t] (device int32), f16 -> f32, rotate, round to f16; y may equal x (the in-place K-shift of a KV cache).  Modes 0 (NORM)
+ * and 2 (NEOX), n_dims <= head_dim (the tail is copied), YaRN and freq factors; other parameters as in pb200_rope. */
+PB200_API int pb200_rope_f16(const void * x, void * y, int64_t n_rows, int n_head, int head_dim, int n_dims, int mode, const int32_t * pos,
+                             float freq_base, float freq_scale, float ext_factor, float attn_factor, float beta_fast, float beta_slow,
+                             int n_ctx_orig, const float * freq_factors, void * stream);
 PB200_API int pb200_soft_max(const float * x, const float * mask, float * y, int64_t ncols, int64_t nrows, int64_t mask_rows, float scale, void * stream);
 PB200_API int pb200_silu_mul(const float * gate, const float * up, float * y, int64_t n, void * stream);
 /* element-wise glue of the graph (binbcast.cu / unary.cu / cpy.cu): y = a (+|*) b[i % nb]  (op 0 add, 1 mul); y = silu(x);
@@ -235,6 +244,26 @@ PB200_API int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host, 
                                   float * logits_host, int32_t synchronize);
 PB200_API float * pb200_prefill_hidden_device(pb200_model * m);
 PB200_API int pb200_kv_clear(pb200_model * m);
+/* prima's context shift on this shard's cache for slot seq (what llama-cli does when the context fills, examples/main/main.cpp:578-608):
+ *   llama_kv_cache_seq_rm(seq, p0 + delta, p0) + llama_kv_cache_seq_add(seq, p0, p1, delta)
+ * (src/llama.cpp:4378-4427; K rotated like build_k_shift, :10665-10719).  The engine keeps cell == position, so the cells are
+ * compacted: cell c in [p0, p1) moves to c + delta, for every layer of this shard (any pipeline shard, with or without embedding / head).
+ *   - Arguments: delta < 0, p0 + delta >= 0, p0 < p1 <= n_ctx, 0 <= seq < n_seq, else PB200_EINVAL; NULL / unfinalized model: PB200_ESTATE
+ *     (the three conditions on delta, p0 and p1 alone are checked first, before the model).
+ *   - The moved K row is f16(rope(f32(K), pos = delta)), V rows are copied bit for bit.  That is what the reference's K-shift computes; it
+ *     is NOT K computed directly at the new position (the row was rounded to f16 at its old position and is rounded again here).
+ *     Equality with the reference holds for one shift between two decodes, which is what llama-cli does.  The reference adds up the deltas of several
+ *     seq_add calls and rotates once at the next decode; this call rotates and rounds every time, so two shifts with no decode in
+ *     between are rounded twice where the reference rounds once.
+ *   - Cells below p0 + delta and all other slots stay bit-identical; cells [p1 + delta, p1) are unspecified afterwards.
+ *   - The slot's device position (pb200_token_device(m, seq)[1]) moves by delta when it is >= p0; its token is kept.  A device-resident
+ *     loop (pb200_step_seq_dev + pb200_argmax_seq / pb200_sample_seq with feed_back) continues without a host round trip, and the captured
+ *     per-slot CUDA graphs stay valid (they read the position from device memory).
+ *   - One launch enqueued on the model stream, no host synchronisation; call it outside any stream capture, like pb200_sampling_set_seq. */
+PB200_API int pb200_kv_seq_shift(pb200_model * m, int seq, int32_t p0, int32_t p1, int32_t delta);
+/* device address of the f16 K (v == 0) or V (v != 0) cache of this shard: [n_seq][layer_end - layer_begin][n_ctx][n_head_kv * head_dim]
+ * (white-box tests and hosts that inspect the cache; NULL before finalize or on a shard without layers) */
+PB200_API void * pb200_kv_device(pb200_model * m, int v);
 
 /* one decode step, HOST in/out (the llama_decode-equivalent call): token id + position in, n_vocab logits out.
  * On a pipeline stage without the embedding / head the hidden state is exchanged through pb200_hidden_* instead. */

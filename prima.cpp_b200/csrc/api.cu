@@ -138,6 +138,16 @@ int pb200_rope(const float * x, float * y, int64_t n_tokens, int n_head, int hea
     return launch_rope(x, y, n_tokens, n_head, head_dim, (int64_t) n_head * head_dim, head_dim, pos, rp, freq_factors, (cudaStream_t) stream);
 }
 
+int pb200_rope_f16(const void * x, void * y, int64_t n_rows, int n_head, int head_dim, int n_dims, int mode, const int32_t * pos, float freq_base,
+                   float freq_scale, float ext_factor, float attn_factor, float beta_fast, float beta_slow, int n_ctx_orig, const float * freq_factors,
+                   void * stream) {
+    if (!x || !y || !pos || n_rows <= 0 || n_head <= 0 || n_dims <= 0 || n_dims > head_dim || (n_dims & 1) || n_rows * n_head > INT32_MAX) return PB200_EINVAL;
+    RopeParams rp;
+    rope_params_init(rp, n_dims, mode, n_ctx_orig, freq_base, freq_scale, ext_factor, attn_factor, beta_fast, beta_slow);
+    g_launches++;
+    return launch_rope_f16((const __half *) x, (__half *) y, n_rows, n_head, head_dim, pos, rp, freq_factors, (cudaStream_t) stream);
+}
+
 int pb200_soft_max(const float * x, const float * mask, float * y, int64_t ncols, int64_t nrows, int64_t mask_rows, float scale, void * stream) {
     if (!x || !y || ncols <= 0 || nrows <= 0) return PB200_EINVAL;
     g_launches++;

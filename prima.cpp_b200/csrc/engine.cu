@@ -714,6 +714,22 @@ int pb200_kv_clear(pb200_model * m) {
     return (int) cudaStreamSynchronize(m->stream);
 }
 
+// prima's context shift on slot seq (llama-cli, examples/main/main.cpp:578-608): one launch on the model stream moves cells [p0, p1) of
+// every layer of this shard to c + delta, re-rotating K by delta, and moves the slot's device position with them.  The captured
+// per-slot graphs read the position from device memory, so they stay valid.
+int pb200_kv_seq_shift(pb200_model * m, int seq, int32_t p0, int32_t p1, int32_t delta) {
+    if (delta >= 0 || (int64_t) p0 + delta < 0 || p0 >= p1) return PB200_EINVAL;   // checked before the model: no CUDA call needed
+    if (!m || !m->finalized) return PB200_ESTATE;
+    if (seq < 0 || seq >= m->n_seq || p1 > m->hp.n_ctx) return PB200_EINVAL;
+    cudaSetDevice(m->device);
+    const pb200_hparams & hp = m->hp;
+    const size_t nl = m->layers.size(), slot = (size_t) seq * nl * (size_t) hp.n_ctx * hp.n_head_kv * hp.head_dim;
+    g_launches++;
+    return launch_kv_shift(m->kcache ? m->kcache + slot : nullptr, m->vcache ? m->vcache + slot : nullptr, (int) nl, hp.n_head_kv, hp.n_ctx, p0, p1,
+                           delta, m->rp, m->rope_ff, m->tokpos_dev + 4 * seq, m->stream);
+}
+void * pb200_kv_device(pb200_model * m, int v) { return (m && m->finalized) ? (void *) (v ? m->vcache : m->kcache) : nullptr; }
+
 static int step(pb200_model * m, int seq = 0) {
     if (m->use_graph && (size_t) seq < m->graph_exec.size() && m->graph_exec[seq]) {
         g_launches += m->launches_per_step;

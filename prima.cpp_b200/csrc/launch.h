@@ -125,6 +125,13 @@ void rope_params_init(RopeParams & rp, int n_dims, int mode, int n_ctx_orig, flo
 // generic rope for the plugin: x [ntok][n_head][D] -> y, positions pos[ntok]
 int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int64_t tok_stride, int64_t head_stride, const int32_t * pos,
                 const RopeParams & rp, const float * freq_factors, cudaStream_t stream);
+// GGML_OP_ROPE on contiguous f16 rows x [ntok][n_head][D] -> y (y may equal x), positions pos[ntok]
+int launch_rope_f16(const __half * x, __half * y, int64_t ntok, int n_head, int D, const int32_t * pos, const RopeParams & rp, const float * freq_factors,
+                    cudaStream_t stream);
+// context shift of one slot's caches kc / vc ([n_layer][n_ctx][n_head_kv*128] f16 each): cells [p0, p1) -> c + delta (delta < 0), K rows
+// re-rotated by delta like launch_rope_f16 (rp.n_dims == 128), V rows copied; tokpos[1] += delta when it is >= p0.  One launch.
+int launch_kv_shift(__half * kc, __half * vc, int n_layer, int n_head_kv, int n_ctx, int p0, int p1, int delta, const RopeParams & rp,
+                    const float * freq_factors, int32_t * tokpos, cudaStream_t stream);
 
 // decode attention (k_attn_rows), FA-off numerics of the CPU backend (f16-rounded q and probabilities, f32 accumulation):
 //   out[h][:] = softmax(scale * K[0..n_kv) . q_h) . V   — GQA-aware, K/V read once per kv head.  n_kv = *pos_dev + 1.

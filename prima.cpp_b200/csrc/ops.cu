@@ -164,6 +164,93 @@ __global__ void k_rope(const float * __restrict__ x, float * __restrict__ y, int
     for (int i = rp.n_dims + threadIdx.x; i < D; i += blockDim.x) yd[i] = xs[i];
 }
 
+// GGML_OP_ROPE on f16 rows (ggml_compute_forward_rope_f16, ggml.c:14269-14380): f16 -> f32, rotate, round to f16.  One CTA per
+// (token, head); each element is read and written by the same thread, so y may equal x (the in-place K-shift of a KV cache).
+__global__ void k_rope_f16(const __half * x, __half * y, int n_head, int D, const int32_t * __restrict__ pos, RopeParams rp,
+                           const float * __restrict__ freq_factors) {
+    const int tok = blockIdx.x / n_head;
+    const __half * xs = x + (int64_t) blockIdx.x * D;
+    __half * yd = y + (int64_t) blockIdx.x * D;
+    const int half_dims = rp.n_dims / 2;
+    const bool neox = rp.mode & 2;
+    for (int pair = threadIdx.x; pair < half_dims; pair += blockDim.x) {
+        float c, s;
+        rope_cos_sin(rp, pos[tok], pair, freq_factors, c, s);
+        const int i0 = neox ? pair : 2 * pair, i1 = neox ? pair + half_dims : 2 * pair + 1;
+        float y0, y1;
+        rope_rotate(__half2float(xs[i0]), __half2float(xs[i1]), c, s, y0, y1);
+        yd[i0] = __float2half_rn(y0); yd[i1] = __float2half_rn(y1);
+    }
+    for (int i = rp.n_dims + threadIdx.x; i < D; i += blockDim.x) yd[i] = xs[i];
+}
+
+// Context shift of one sequence slot of the engine's cache (llama_kv_cache_seq_rm + llama_kv_cache_seq_add, src/llama.cpp:4378-4427,
+// then the K-shift graph of build_k_shift, :10665-10719): every cell c in [p0, p1) moves to c + delta (delta < 0); its K row becomes
+// f16(rope(f32(K), pos = delta)) with the rotation of k_rope_f16, its V row is copied bit for bit.  Per layer the caches are
+// [cell][n_head_kv * 128] f16.  One warp owns one (layer, K|V, kv head) column and walks its cells upwards, so the destination of a
+// move lies in cells the warp has already read: a launch never writes a cell another warp has yet to read.  Lanes 0-15 hold the
+// sixteen 16-byte pieces of an even cell's row, lanes 16-31 those of the following cell; KS_U cell pairs are loaded before any is
+// stored.  NORM pairs are lane-local, NEOX pairs (d, d + 64) sit 8 lanes apart and are exchanged with a shuffle.  head_dim == n_dims
+// == 128.  Thread 0 also moves the slot's device position by delta when it is >= p0.
+constexpr int KS_U = 8;
+constexpr int KS_WARPS = 4;
+__global__ void __launch_bounds__(KS_WARPS * 32) k_kv_shift(__half * kc, __half * vc, int n_cols, int n_head_kv, int64_t layer_stride, int p0,
+                                                            int p1, int delta, RopeParams rp, const float * __restrict__ freq_factors,
+                                                            int32_t * tokpos) {
+    if (blockIdx.x == 0 && threadIdx.x == 0 && tokpos[1] >= p0) tokpos[1] += delta;
+    const int col = blockIdx.x * KS_WARPS + (threadIdx.x >> 5);
+    if (col >= n_cols) return;
+    const int lane = threadIdx.x & 31, piece = lane & 15, odd = lane >> 4;
+    const int layer = col / (2 * n_head_kv), rem = col % (2 * n_head_kv);
+    const bool is_k = rem < n_head_kv;
+    const int64_t EK = (int64_t) n_head_kv * 128;
+    __half * base = (is_k ? kc : vc) + layer * layer_stride + (int64_t) (rem % n_head_kv) * 128 + piece * 8;
+    const bool neox = rp.mode & 2;
+    // this lane's dims 8 piece .. 8 piece + 7: NORM pairs 4 piece + j (j < 4), NEOX pairs 8 (piece % 8) + j (j < 8)
+    float cs[8], sn[8];
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        cs[j] = 1.f; sn[j] = 0.f;
+        if (is_k && (neox || j < 4)) rope_cos_sin(rp, delta, neox ? 8 * (piece & 7) + j : 4 * piece + j, freq_factors, cs[j], sn[j]);
+    }
+    for (int c0 = p0; c0 < p1; c0 += 2 * KS_U) {
+        uint4 r[KS_U];
+#pragma unroll
+        for (int u = 0; u < KS_U; u++) {
+            const int cell = c0 + 2 * u + odd;
+            r[u] = cell < p1 ? __ldcs(reinterpret_cast<const uint4 *>(base + cell * EK)) : make_uint4(0, 0, 0, 0);
+        }
+        __syncwarp();   // every load of this batch is done before any lane stores into a cell of it
+#pragma unroll
+        for (int u = 0; u < KS_U; u++) {
+            const int cell = c0 + 2 * u + odd;
+            if (is_k) {   // warp-uniform
+                __half2 * h = reinterpret_cast<__half2 *>(&r[u]);
+                float x[8];
+#pragma unroll
+                for (int j = 0; j < 4; j++) { const float2 f = __half22float2(h[j]); x[2 * j] = f.x; x[2 * j + 1] = f.y; }
+                float y[8];
+                if (neox) {
+                    const bool lo = piece < 8;
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        const float o = __shfl_xor_sync(0xffffffffu, x[j], 8);
+                        float y0, y1;
+                        rope_rotate(lo ? x[j] : o, lo ? o : x[j], cs[j], sn[j], y0, y1);
+                        y[j] = lo ? y0 : y1;
+                    }
+                } else {
+#pragma unroll
+                    for (int j = 0; j < 4; j++) rope_rotate(x[2 * j], x[2 * j + 1], cs[j], sn[j], y[2 * j], y[2 * j + 1]);
+                }
+#pragma unroll
+                for (int j = 0; j < 4; j++) h[j] = __halves2half2(__float2half_rn(y[2 * j]), __float2half_rn(y[2 * j + 1]));
+            }
+            if (cell < p1) __stcs(reinterpret_cast<uint4 *>(base + (cell + delta) * EK), r[u]);
+        }
+    }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Softmax of one row S[0..n) in shared memory by a CTA of WARPS warps, in the order of the FA-off chain's CPU soft_max
 // (ggml.c:13783): per-thread strided fmaxf, warp max, thread 0 folds the warps in order; e = expf(s - max) written back in place
@@ -1059,6 +1146,20 @@ void rope_params_init(RopeParams & rp, int n_dims, int mode, int n_ctx_orig, flo
 int launch_rope(const float * x, float * y, int64_t ntok, int n_head, int D, int64_t tok_stride, int64_t head_stride, const int32_t * pos,
                 const RopeParams & rp, const float * freq_factors, cudaStream_t stream) {
     k_rope<<<(unsigned) (ntok * n_head), 64, 0, stream>>>(x, y, n_head, D, tok_stride, head_stride, pos, rp, freq_factors);
+    return (int) cudaGetLastError();
+}
+
+int launch_rope_f16(const __half * x, __half * y, int64_t ntok, int n_head, int D, const int32_t * pos, const RopeParams & rp, const float * freq_factors,
+                    cudaStream_t stream) {
+    k_rope_f16<<<(unsigned) (ntok * n_head), 64, 0, stream>>>(x, y, n_head, D, pos, rp, freq_factors);
+    return (int) cudaGetLastError();
+}
+
+int launch_kv_shift(__half * kc, __half * vc, int n_layer, int n_head_kv, int n_ctx, int p0, int p1, int delta, const RopeParams & rp,
+                    const float * freq_factors, int32_t * tokpos, cudaStream_t stream) {
+    const int n_cols = n_layer * 2 * n_head_kv;
+    const int grid = std::max(1, (n_cols + KS_WARPS - 1) / KS_WARPS);   // at least one CTA: the slot position moves on shards without layers too
+    k_kv_shift<<<grid, KS_WARPS * 32, 0, stream>>>(kc, vc, n_cols, n_head_kv, (int64_t) n_ctx * n_head_kv * 128, p0, p1, delta, rp, freq_factors, tokpos);
     return (int) cudaGetLastError();
 }
 

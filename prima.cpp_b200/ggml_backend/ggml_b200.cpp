@@ -254,8 +254,10 @@ static bool b200_supports_op(ggml_backend_dev_t, const ggml_tensor * op) {
             return b->ne[1] * b->ne[2] * b->ne[3] <= 64;
         }
         case GGML_OP_ROPE: {
+            // f32 (q / k of the forward graph) or f16 -> f16 (the in-place K-shift of the f16 K cache, build_k_shift src/llama.cpp:10665-10719)
             const int mode = ((const int32_t *) op->op_params)[2];
-            return a->type == GGML_TYPE_F32 && op->type == GGML_TYPE_F32 && ggml_is_contiguous(a) && ggml_is_contiguous(op) && (mode == 0 || mode == 2) &&
+            const bool f32 = a->type == GGML_TYPE_F32 && op->type == GGML_TYPE_F32, f16 = a->type == GGML_TYPE_F16 && op->type == GGML_TYPE_F16;
+            return (f32 || f16) && ggml_is_contiguous(a) && ggml_is_contiguous(op) && (mode == 0 || mode == 2) &&
                    a->ne[3] == 1 && (op->src[2] == nullptr || op->src[2]->type == GGML_TYPE_F32);
         }
         case GGML_OP_SOFT_MAX: {
@@ -366,6 +368,11 @@ static bool b200_compute_node(b200_backend_ctx * ctx, ggml_tensor * dst) {
             const int32_t * p = (const int32_t *) dst->op_params;
             float fb, fs, ef, af, bf, bsl;
             memcpy(&fb, p + 5, 4); memcpy(&fs, p + 6, 4); memcpy(&ef, p + 7, 4); memcpy(&af, p + 8, 4); memcpy(&bf, p + 9, 4); memcpy(&bsl, p + 10, 4);
+            if (a->type == GGML_TYPE_F16) {
+                PB_OK(pb200_rope_f16(a->data, dst->data, a->ne[2], (int) a->ne[1], (int) a->ne[0], p[1], p[2], (const int32_t *) b->data, fb, fs, ef, af, bf,
+                                     bsl, p[4], dst->src[2] ? (const float *) dst->src[2]->data : nullptr, st));
+                return true;
+            }
             PB_OK(pb200_rope((const float *) a->data, (float *) dst->data, a->ne[2], (int) a->ne[1], (int) a->ne[0], p[1], p[2], (const int32_t *) b->data, fb, fs,
                              ef, af, bf, bsl, p[4], dst->src[2] ? (const float *) dst->src[2]->data : nullptr, st));
             return true;

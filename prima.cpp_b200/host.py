@@ -93,6 +93,10 @@ class Lib:
         c.pb200_model_weight_bytes.restype = i64
         c.pb200_model_weight_bytes.argtypes = [vp]
         c.pb200_kv_clear.argtypes = [vp]
+        c.pb200_kv_seq_shift.argtypes = [vp, C.c_int, i32, i32, i32]
+        c.pb200_kv_device.restype = vp
+        c.pb200_kv_device.argtypes = [vp, C.c_int]
+        c.pb200_rope_f16.argtypes = [vp, vp, i64, C.c_int, C.c_int, C.c_int, C.c_int, vp, f32, f32, f32, f32, f32, f32, C.c_int, vp, vp]
         c.pb200_decode.argtypes = [vp, i32, i32, vp]
         c.pb200_prefill.argtypes = [vp, vp, i32, i32, vp]
         c.pb200_prefill_stage.argtypes = [vp, vp, vp, i32, i32, vp, i32]
@@ -198,6 +202,16 @@ class Model:
 
     def kv_clear(self) -> None:
         self.lib.check(self.lib.c.pb200_kv_clear(self.h), "kv_clear")
+
+    def kv_shift(self, seq: int, p0: int, p1: int, delta: int) -> None:
+        """prima's context shift of slot seq (pb200_kv_seq_shift): cells [p0, p1) move to c + delta (delta < 0), K re-rotated by delta,
+        and the slot's device position moves with them.  Enqueued on the model stream.  llama-cli's rule when the context fills:
+        n_discard = (n_past - n_keep) // 2, kv_shift(seq, n_keep + n_discard, n_past, -n_discard)."""
+        self.lib.check(self.lib.c.pb200_kv_seq_shift(self.h, seq, int(p0), int(p1), int(delta)), "kv_seq_shift")
+
+    def kv_ptr(self, v: bool = False) -> int:
+        """Device address of the f16 K (or V) cache: [n_seq][layers of this shard][n_ctx][n_head_kv * 128]."""
+        return self.lib.c.pb200_kv_device(self.h, int(v)) or 0
 
     def decode(self, token: int, pos: int, logits_out=None):
         ptr = None if logits_out is None else logits_out.ctypes.data_as(C.c_void_p)

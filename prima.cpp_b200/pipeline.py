@@ -34,6 +34,9 @@ def layer_windows(n_layer: int, world: int) -> list[int]:
 
 
 class PipelineRunner:
+    """One token at a time through the stages.  The ranks are in lockstep per token, so a context shift needs nothing from the
+    runner: every rank calls its stage's kv_shift (Model.kv_shift) with the same arguments between the same two step() calls."""
+
     def __init__(self, stage, rank: int, world: int, dist=None, token_tensor=None, stream=None):
         self.stage, self.rank, self.world, self.dist = stage, rank, world, dist
         self.stream = stream      # the engine's stream as a torch stream: entered around every step (see the module docstring)
@@ -92,7 +95,8 @@ class RingRunner:
     The stage object provides: hidden_in / hidden_out (tensors aliasing the engine's buffers), token_in(seq) / token_out(seq)
     (int32[1] tensors: where a returned token lands on stage 0 / where the last stage leaves its sample), begin(seq, token, pos)
     (stage 0: first token of a sequence; other stages: position only) and run(seq) (one step of the slot, sampling included on the
-    last stage).  The same class drives CPU tensors over gloo in tests/test_pipeline_gloo.py."""
+    last stage), and kv_shift(seq, p0, p1, delta) where shift() is used.  The same class drives CPU tensors over gloo in
+    tests/test_pipeline_gloo.py."""
 
     def __init__(self, stage, rank: int, world: int, dist, stream=None):
         if world < 2 or dist is None:
@@ -100,6 +104,18 @@ class RingRunner:
         self.stage, self.rank, self.world, self.dist = stage, rank, world, dist
         self.stream = stream
         self.t = 0
+        self.runs: dict[int, int] = {}                          # runs of each sequence on this rank so far
+        self.shifts: dict[int, list[tuple[int, int, int, int]]] = {}
+
+    def shift(self, seq: int, at_step: int, p0: int, p1: int, delta: int) -> None:
+        """Context shift of sequence seq (prima forwards llama_kv_cache_seq_rm / seq_add down the ring, src/llama.cpp:17946, 18345):
+        every rank applies stage.kv_shift(seq, p0, p1, delta) immediately before its own run number at_step (0-based) of seq, so
+        the shift lands between the same two tokens of the sequence on every rank.  Stage r runs a given token of a sequence r time
+        slots after stage 0, which is why the point is counted in runs of the sequence, not in time slots.  Call it with the same
+        arguments on every rank, before that run."""
+        if at_step < self.runs.get(seq, 0):
+            raise ValueError(f"sequence {seq} has already run {self.runs.get(seq, 0)} steps on rank {self.rank}")
+        self.shifts.setdefault(seq, []).append((at_step, p0, p1, delta))
 
     def slots(self, n: int, first_tokens=None) -> None:
         """Runs time slots self.t .. self.t + n - 1 (the same n on every rank).  first_tokens[s] = (token, pos) seeds sequence s."""
@@ -130,7 +146,12 @@ class RingRunner:
                 sq = a % N
                 if a < N and first_tokens is not None:
                     st.begin(sq, *first_tokens[sq])
+                done = self.runs.get(sq, 0)
+                for sh in [s for s in self.shifts.get(sq, ()) if s[0] == done]:
+                    st.kv_shift(sq, *sh[1:])
+                    self.shifts[sq].remove(sh)
                 st.run(sq)
+                self.runs[sq] = done + 1
             self.t += 1
 
 
