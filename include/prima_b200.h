@@ -111,6 +111,8 @@ PB200_API int pb200_mul_mat_f16(const void * a_f16, const float * b_f32, float *
  * bytes, tpad = t rounded up to the token tile: the fp16 activation image, then one f32 power-of-two scale per padded row that keeps
  * every activation magnitude inside fp16's normal range. */
 PB200_API size_t pb200_mul_mat_q_workspace_bytes(int64_t k, int64_t t);
+/* 1 when pb200_mul_mat_q takes weights of this type with k columns (the type and k rule above), else 0 */
+PB200_API int pb200_mul_mat_q_supported(int type, int64_t k);
 PB200_API int pb200_mul_mat_q(int type, const void * W, int64_t n, int64_t k, const float * x, int64_t ldx, int64_t t, float * dst,
                               const float * bias, const float * resid, void * ws, void * stream);
 PB200_API int pb200_get_rows(int type, const void * table, int64_t k, const int32_t * ids, int64_t n_ids, float * y, void * stream);
@@ -173,19 +175,25 @@ typedef struct pb200_gemv_mat {
  * computed once, distributed over the launch's CTAs (one in-kernel grid barrier), left in act_ws.  sync_ws: 16 bytes of zero-initialised
  * device memory owned by the caller (barrier state, self-resetting; one per stream).  pdl != 0: the launch may start while the
  * previous kernel of the stream drains (programmatic dependent launch); its inputs are read only after that kernel has completed.
- * Returns PB200_ENOTSUP for types / shapes outside the fast kernel (callers fall back to the single ops). */
+ * Returns PB200_ENOTSUP for types / shapes outside the fast kernel: pb200_gemv_fused_supported tells them apart before the call. */
 PB200_API int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * act_ws, int prologue, const float * in0, const float * in1,
                                float eps, void * sync_ws, int pdl, void * stream);
+/* 1 when pb200_gemv_fused takes a matrix of this type with k columns (a k-quant type, k % 256 == 0, k <= 29696), else 0.  W's
+ * 16-byte alignment is a precondition on top of it. */
+PB200_API int pb200_gemv_fused_supported(int type, int64_t k);
 /* One token of the reference graph's FA-off attention chain as ONE launch (llm_build_kv_store + llm_build_kqv, src/llama.cpp:9673-9718,
  * 10032-10165): rope(q), rope(k) -> f16 K row into cell kv_head of k_cache [cell][n_head_kv*128]; v -> f16 into column kv_head of the
  * TRANSPOSED v cache [n_head_kv*128][vt_stride]; out[h] = softmax(scale * K q_h + mask) . V over n_cells cells (multiple of 32, mask f32
  * [n_cells], -inf = not visible).  head_dim 128, n_head even.  act_ws_out (optional): also leaves q8_K(out) there for the following
  * mat-vec.  kv_head_dev (optional): the cell is read from this device word instead of kv_head, so a CUDA graph that captured the launch can
- * be replayed for the next token.  rope op parameters as in pb200_rope.  Returns PB200_ENOTSUP for shapes it does not handle. */
+ * be replayed for the next token.  rope op parameters as in pb200_rope.  Returns PB200_ENOTSUP for shapes it does not handle, among
+ * them n_cells above pb200_attn_ggml_max_cells(). */
 PB200_API int pb200_attn_ggml(const float * q, const float * k, const float * v, void * k_cache_f16, void * v_cache_t_f16, int64_t vt_stride, float * out,
                               void * act_ws_out, int n_head, int n_head_kv, int head_dim, const int32_t * pos_dev, int n_cells, int kv_head,
                               const int32_t * kv_head_dev, const float * mask, int n_dims, int mode, float freq_base, float freq_scale, float ext_factor, float attn_factor,
                               float beta_fast, float beta_slow, int n_ctx_orig, const float * freq_factors, float scale, int pdl, void * stream);
+/* the largest n_cells pb200_attn_ggml takes on the current device (a multiple of 32): the score row lives in shared memory */
+PB200_API int pb200_attn_ggml_max_cells(void);
 
 /* ---- decode engine (one model shard per process / GPU) ---- */
 typedef struct pb200_hparams {

@@ -14,10 +14,6 @@ using namespace pb;
 
 extern std::atomic<uint64_t> g_launches;
 
-namespace {
-bool type_ok(int t) { return t == T_Q4_K || t == T_Q5_K || t == T_Q6_K || t == T_Q8_0 || t == T_Q5_1; }
-}  // namespace
-
 extern "C" {
 
 const char * pb200_version(void) { return "prima.cpp_b200 0.1 (sm_90a)"; }
@@ -47,14 +43,14 @@ void pb200_kernel_launches_add(uint64_t n) { g_launches += n; }
 size_t pb200_act_workspace_bytes(int64_t k) { return act_ws_bytes(k); }
 
 int pb200_quantize_act(int wtype, const float * x, int64_t k, void * act_ws, void * stream) {
-    if (!type_ok(wtype) || !x || !act_ws || k <= 0 || k % block_elems(wtype) != 0) return PB200_EINVAL;
+    if (!is_quant_type(wtype) || !x || !act_ws || k <= 0 || k % block_elems(wtype) != 0) return PB200_EINVAL;
     g_launches++;
     return launch_quantize_act(x, nullptr, (int) k, act_mode_for(wtype), act_from_ws(act_ws, k), (cudaStream_t) stream, false);
 }
 
 int pb200_mul_mat_vec_q(int type, const void * W, int64_t n, int64_t k, const void * act_ws, float * y, const float * bias, const float * resid,
                         void * stream) {
-    if (!type_ok(type) || !W || !act_ws || !y || n <= 0 || k <= 0 || k % block_elems(type) != 0) return PB200_EINVAL;
+    if (!is_quant_type(type) || !W || !act_ws || !y || n <= 0 || k <= 0 || k % block_elems(type) != 0) return PB200_EINVAL;
     GemvDesc d = {W, y, bias, resid, type, (int) n};
     uint64_t nl = 0;
     const int rc = launch_gemv(&d, 1, (int) k, act_from_ws(const_cast<void *>(act_ws), k), GemvPrologue{}, (cudaStream_t) stream, false, nl);
@@ -73,7 +69,7 @@ int pb200_mul_mat_vec_fused(int nmat, const int * types, const void * const * W,
     if (nmat < 1 || nmat > 3 || !types || !W || !n || !y || !act_ws) return PB200_EINVAL;
     GemvDesc d[3];
     for (int i = 0; i < nmat; i++) {
-        if (!type_ok(types[i]) || k % block_elems(types[i]) != 0) return PB200_EINVAL;
+        if (!is_quant_type(types[i]) || k % block_elems(types[i]) != 0) return PB200_EINVAL;
         if (act_mode_for(types[i]) != act_mode_for(types[0])) return PB200_EINVAL;   // one activation: one quantization format
         d[i] = GemvDesc{W[i], y[i], nullptr, nullptr, types[i], (int) n[i]};
     }
@@ -84,7 +80,7 @@ int pb200_mul_mat_vec_fused(int nmat, const int * types, const void * const * W,
 }
 
 int pb200_mul_mat_vec_host(int type, const void * W_dev, int64_t n, int64_t k, const float * x_host, float * y_host) {
-    if (!type_ok(type) || !W_dev || !x_host || !y_host) return PB200_EINVAL;
+    if (!is_quant_type(type) || !W_dev || !x_host || !y_host) return PB200_EINVAL;
     // per-thread cached staging buffers (pinned host + device), grown on demand
     struct Stage { float * hx = nullptr, * hy = nullptr, * dx = nullptr, * dy = nullptr; void * ws = nullptr; int64_t n = 0, k = 0; cudaStream_t st = nullptr; };
     static thread_local Stage S;
@@ -187,6 +183,7 @@ int pb200_mul_mat_f16(const void * a_f16, const float * b_f32, float * d, int64_
 }
 
 size_t pb200_mul_mat_q_workspace_bytes(int64_t k, int64_t t) { return (k > 0 && t > 0) ? mmq_workspace_bytes(k, t) : 0; }
+int pb200_mul_mat_q_supported(int type, int64_t k) { return mmq_supported(type, k); }
 int pb200_mul_mat_q(int type, const void * W, int64_t n, int64_t k, const float * x, int64_t ldx, int64_t t, float * dst, const float * bias,
                     const float * resid, void * ws, void * stream) {
     if (!W || !x || !dst || !ws || n <= 0 || t <= 0 || ldx < k || resid == dst) return PB200_EINVAL;
@@ -199,7 +196,7 @@ int pb200_aborted(void) { return check_clear_abort(); }
 
 int pb200_get_rows(int type, const void * table, int64_t k, const int32_t * ids, int64_t n_ids, float * y, void * stream) {
     if (!table || !ids || !y || k <= 0 || n_ids <= 0) return PB200_EINVAL;
-    if (!(type_ok(type) || type == T_F32 || type == T_F16)) return PB200_ENOTSUP;
+    if (!(is_quant_type(type) || type == T_F32 || type == T_F16)) return PB200_ENOTSUP;
     g_launches++;
     return launch_get_rows(table, type, (int) k, ids, (int) n_ids, y, (cudaStream_t) stream, false);
 }
@@ -214,6 +211,7 @@ int pb200_attn_decode(const float * q, const void * k_cache_f16, const void * v_
     return rc;
 }
 
+int pb200_gemv_fused_supported(int type, int64_t k) { return is_kquant(type) && k <= INT32_MAX && gemv_fused_prologue_ok((int) k); }
 int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * act_ws, int prologue, const float * in0, const float * in1, float eps,
                      void * sync_ws, int pdl, void * stream) {
     if (nmat < 1 || nmat > 3 || !mats || !act_ws || k <= 0 || prologue < 0 || prologue > 2) return PB200_EINVAL;
@@ -222,7 +220,7 @@ int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * ac
     GemvDesc d[3];
     for (int i = 0; i < nmat; i++) {
         if (!mats[i].W || !mats[i].y || mats[i].n <= 0) return PB200_EINVAL;
-        if (!is_kquant(mats[i].type) || ((uintptr_t) mats[i].W & 15)) return PB200_ENOTSUP;
+        if (!pb200_gemv_fused_supported(mats[i].type, k) || ((uintptr_t) mats[i].W & 15)) return PB200_ENOTSUP;
         d[i] = GemvDesc{mats[i].W, mats[i].y, nullptr, mats[i].add, mats[i].type, (int) mats[i].n};
     }
     static const int kind[3] = {PRO_NONE, PRO_RMSNORM, PRO_SILU_MUL};   // the ABI's prologue codes
@@ -233,6 +231,7 @@ int pb200_gemv_fused(int nmat, const pb200_gemv_mat * mats, int64_t k, void * ac
     return rc;
 }
 
+int pb200_attn_ggml_max_cells(void) { return attn2_max_cells(); }
 int pb200_attn_ggml(const float * q, const float * k, const float * v, void * k_cache_f16, void * v_cache_t_f16, int64_t vt_stride, float * out,
                     void * act_ws_out, int n_head, int n_head_kv, int head_dim, const int32_t * pos_dev, int n_cells, int kv_head,
                     const int32_t * kv_head_dev, const float * mask, int n_dims, int mode, float freq_base, float freq_scale, float ext_factor, float attn_factor, float beta_fast, float beta_slow,

@@ -31,6 +31,7 @@ __host__ __device__ inline int64_t row_bytes(int type, int64_t k) {
     return -1;
 }
 __host__ __device__ inline bool is_kquant(int t) { return t == T_Q4_K || t == T_Q5_K || t == T_Q6_K; }
+__host__ __device__ inline bool is_quant_type(int t) { return is_kquant(t) || t == T_Q8_0 || t == T_Q5_1; }   // the quantized weight types
 __host__ __device__ inline int block_elems(int t) { return is_kquant(t) ? 256 : ((t == T_Q8_0 || t == T_Q5_1) ? 32 : 1); }
 
 // ---------------------------------------------------------------------------------------------

@@ -204,8 +204,6 @@ static Tensor * find_tensor(pb200_model * m, const std::string & name, bool & is
     return nullptr;
 }
 
-static bool type_supported(int t) { return t == T_Q4_K || t == T_Q5_K || t == T_Q6_K || t == T_Q8_0 || t == T_Q5_1; }
-
 extern "C" {
 
 pb200_model * pb200_model_create(const pb200_hparams * hp, int device, int layer_begin, int layer_end, int with_embd, int with_head) {
@@ -262,7 +260,7 @@ int pb200_model_tensor_alloc(pb200_model * m, const char * name, int type, size_
         if (s == "token_embd.weight" || s == "output.weight" || s.rfind("blk.", 0) == 0) return 0;   // other stage
         return PB200_EINVAL;
     }
-    if (!type_supported(type)) return PB200_ENOTSUP;
+    if (!is_quant_type(type)) return PB200_ENOTSUP;
     if (t->K % block_elems(type) != 0) return PB200_EINVAL;
     const size_t need = (size_t) (row_bytes(type, t->K) * t->N);
     if (nbytes != need) return PB200_EINVAL;

@@ -140,6 +140,9 @@ int launch_attn_decode(const float * q, const __half * kcache, const __half * vc
 // k_attn_rows keeps a whole score row in shared memory: the longest row (a multiple of 32) it takes on the current device.  Longer
 // n_ctx / n_kv_max make launch_attn_decode, launch_attn_batch's per-row form and launch_attn_step's fallback return cudaErrorNotSupported.
 int attn_rows_max_kv();
+// k_attn2 keeps a score row of n cells (padded to 32) in shared memory behind its fixed part, at most 200 KB: the largest n (a multiple of
+// 32) it takes on the current device.  launch_attn_step / launch_attn_ggml refuse more (pb200_attn_ggml_max_cells).
+int attn2_max_cells();
 // batched form for prompt processing: token t (q row t, out row t) attends to cache rows [0, pos_dev[t]].  The tiled kernel when its
 // scores fit shared memory, else k_attn_rows per (head, token)
 int launch_attn_batch(const float * q, const __half * kcache, const __half * vcache, float * out, int n_head, int n_head_kv, int D,

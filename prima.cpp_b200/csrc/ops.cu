@@ -1220,14 +1220,19 @@ int launch_attn_batch(const float * q, const __half * kcache, const __half * vca
                                    RopeParams{}, nullptr, scale, n_tok, (int64_t) n_head * D, n_kv_max, stream, false);
 }
 
-// k_attn2: cudaErrorNotSupported for shapes the clustered kernel does not take (odd n_head, scores beyond its shared memory)
+static FuncAttrCache attn2_attr[2];   // k_attn2<false>, k_attn2<true>
+int attn2_max_cells() {
+    const size_t lim = std::min({(size_t) 200 * 1024, dyn_smem_limit(attn2_attr[0], (const void *) k_attn2<false>),
+                                 dyn_smem_limit(attn2_attr[1], (const void *) k_attn2<true>)});
+    return lim > sizeof(Attn2Smem) ? (int) (((lim - sizeof(Attn2Smem)) / sizeof(float)) & ~(size_t) 31) : 0;
+}
+// k_attn2: cudaErrorNotSupported for shapes the clustered kernel does not take (odd n_head, scores beyond attn2_max_cells())
 template <bool GGML>
 static int launch_attn2(Attn2Params & P, int n_score_slots, cudaStream_t stream, bool pdl) {
+    if ((P.n_head & 1) || P.n_head_kv <= 0 || P.n_head % P.n_head_kv || n_score_slots > attn2_max_cells()) return (int) cudaErrorNotSupported;
     const size_t smem = sizeof(Attn2Smem) + (size_t) ((n_score_slots + 31) & ~31) * sizeof(float);
-    if ((P.n_head & 1) || P.n_head_kv <= 0 || P.n_head % P.n_head_kv || smem > 200 * 1024) return (int) cudaErrorNotSupported;
-    static FuncAttrCache attr_cache;
     {
-        cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_attn2<GGML>, smem, false);
+        cudaError_t e = ensure_dyn_smem(attn2_attr[GGML], (const void *) k_attn2<GGML>, smem, false);
         if (e != cudaSuccess) return (int) e;
     }
     P.abort_flag = abort_flag();

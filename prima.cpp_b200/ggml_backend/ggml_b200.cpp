@@ -45,21 +45,28 @@ struct b200_device_ctx {
     std::string name, description;
 };
 // ---- execution plan of the fused decode path (see graph_compute) ----
+enum class step_kind { node, gemv, attn };
+// how a fused GEMV gets its q8_K activation: a quantize launch of its own, the rms-norm or silu·mul prologue of pb200_gemv_fused
+// (its prologue codes 1 and 2), or left in the workspace by the fused attention before it
+enum class gemv_prologue { quantize, rms_norm, silu_mul, from_attn };
+struct gemv_step {
+    int nmat;
+    int mm[3], out[3];        // MUL_MAT node, node whose buffer receives y (the MUL_MAT, or the ADD folded into the epilogue)
+    int add_src[3];           // out[j] is an ADD: which of its srcs is the added vector (-1: nothing added)
+    int out_slot[3];          // >= 0: the result never leaves the fused steps (q, k, v, gate, up): it goes to this private buffer
+    gemv_prologue prologue;
+    int p0, p1;               // rms_norm: RMS_NORM node, MUL node; silu_mul: UNARY node, MUL node (gate / up: private SCR_G, SCR_U)
+};
+struct attn_step {            // q / k / v come from the private SCR_Q, SCR_K, SCR_V
+    int rope_q, rope_k, cpy_k, cpy_v, kq, soft, kqv, cont;
+    bool quant_out;           // wo's step takes the activation this launch leaves quantized
+    bool out_private;         // the f32 attention output is read by nobody (wo takes the quantized copy): keep it private
+};
 struct b200_step {
-    int kind;                 // 0 = single node, 1 = fused GEMV group, 2 = fused attention
-    int node;                 // kind 0: node index
-    // kind 1
-    int nmat, mm[3], out[3], add_vec[3];   // MUL_MAT node, node whose buffer receives y, node/leaf supplying the added vector (-1 none; see add_src)
-    int add_src[3];                        // which src of the ADD node is the vector
-    int prologue;                          // 0 quantize src1 with a separate kernel, 1 rms-norm, 2 silu, 3 activation left quantized by the attention step
-    int p0, p1;                            // prologue 1: RMS_NORM node, MUL node; prologue 2: UNARY node, MUL node
-    int ws;                                // workspace role
-    int out_scratch[3];                    // >= 0: the result never leaves the fused steps (q, k, v, gate, up): it goes to this private buffer
-    int in_scratch[2];                     // prologue 2: gate / up come from these private buffers
-    // kind 2
-    int rope_q, rope_k, cpy_k, cpy_v, kq, soft, kqv, cont, quant_out;
-    int q_scratch, k_scratch, v_scratch;   // private buffers holding this token's q / k / v (see out_scratch)
-    int out_private;                       // the f32 attention output is read by nobody (wo takes the quantized copy): keep it private
+    step_kind kind;
+    int node;                 // where the step runs (kind node: the node itself)
+    gemv_step gemv;
+    attn_step attn;
 };
 struct b200_plan {
     uint64_t key;
@@ -82,33 +89,38 @@ struct b200_plan {
 // fused steps therefore never touch the graph's buffers; results that escape (ffn_inp, l_out, logits) are written at their own
 // node's position like the unfused path would.
 enum { SCR_Q = 0, SCR_K = 1, SCR_V = 2, SCR_G = 3, SCR_U = 4, SCR_ATT = 5, SCR_COUNT = 6 };
+// activation workspace of a fused GEMV, one per role so that a producer never overwrites what the previous launch may still be
+// reading under programmatic dependent launch: 0 quantize / rms-norm (K = n_embd), 1 attention output, 2 silu·mul (K = n_ff)
+static int act_role(gemv_prologue p) { return p == gemv_prologue::from_attn ? 1 : p == gemv_prologue::silu_mul ? 2 : 0; }
 
+// A device buffer of the backend that only grows (see grow_buf), freed with the backend.
+struct dev_buf {
+    void * p = nullptr;
+    size_t bytes = 0;
+    dev_buf() = default;
+    dev_buf(const dev_buf &) = delete;
+    dev_buf & operator=(const dev_buf &) = delete;
+    ~dev_buf() { if (p) cudaFree(p); }
+};
 struct b200_backend_ctx {
     int device;
     cudaStream_t stream = nullptr;
-    void * act_ws = nullptr;       // quantized-activation workspace (grown on demand)
-    size_t act_ws_bytes = 0;
-    // fused decode path (graph_compute): one activation workspace per role so that a producer never overwrites what the
-    // previous launch may still be reading under programmatic dependent launch; barrier state of pb200_gemv_fused; plan cache
-    void * fact_ws[3] = {nullptr, nullptr, nullptr};   // 0: norm prologue (K = n_embd), 1: attention output, 2: silu prologue (K = n_ff)
-    size_t fact_bytes[3] = {0, 0, 0};
-    void * sync_ws = nullptr;
-    float * attn_tmp = nullptr;
-    size_t attn_tmp_floats = 0;
-    float * scratch[SCR_COUNT] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    size_t scratch_floats[SCR_COUNT] = {0, 0, 0, 0, 0, 0};
+    dev_buf act_ws;           // quantized activation of the node-by-node mat-vec
+    dev_buf mmq_ws;           // fp16 activation tiles of the tensor-core path
+    dev_buf fact_ws[3];       // fused GEMV activations, by act_role
+    dev_buf sync_ws;          // barrier state of pb200_gemv_fused
+    dev_buf attn_tmp;
+    dev_buf scratch[SCR_COUNT];
+    dev_buf kvh_dev;          // destination cell of the current token (device word read by the captured attention launches)
     cudaEvent_t copy_event = nullptr;
-    int32_t * kvh_dev = nullptr;       // destination cell of the current token (device word read by the captured attention launches)
     int32_t * kvh_host = nullptr;      // pinned staging words for it
     unsigned kvh_idx = 0;
     bool capturing = false, capture_failed = false;
     std::vector<char> skip;
     std::vector<b200_plan *> plans;
-    void * mmq_ws = nullptr;       // fp16 activation tiles for the tensor-core path (grown on demand)
-    size_t mmq_ws_bytes = 0;
-    // generation of the plugin-owned device buffers a captured launch can hold by value (act_ws, mmq_ws, fact_ws, scratch,
-    // attn_tmp, sync_ws, kvh_dev): bumped at every (re)allocation and folded into each plan's `bind`, so that a CUDA graph
-    // captured before a buffer moved is recaptured instead of replayed.  Buffers only grow, so it changes a bounded number of times.
+    // generation of the dev_bufs above, which a captured launch holds by value: bumped at every (re)allocation and folded into each
+    // plan's `bind`, so that a CUDA graph captured before a buffer moved is recaptured instead of replayed.  Buffers only grow, so it
+    // changes a bounded number of times.
     uint64_t ws_gen = 0;
     std::string name;
 };
@@ -117,11 +129,21 @@ struct b200_buffer_ctx {
     void * base;
 };
 
-static const int64_t MMQ_MIN_COLS = 8;
-static bool mmq_ok(enum ggml_type t, int64_t k) {   // mirrors mmq_supported() of the library
-    if (t == GGML_TYPE_Q4_K || t == GGML_TYPE_Q5_K || t == GGML_TYPE_Q6_K) return k % 256 == 0;
-    return (t == GGML_TYPE_Q8_0 || t == GGML_TYPE_Q5_1) && k % 64 == 0 && k >= 256;
+// Makes b hold at least `need` bytes.  A captured CUDA graph holds b.p by value, so no allocation may happen inside a capture: there a
+// growth abandons the capture (capture_failed, the call then runs directly) and returns false, and the caller enqueues nothing.
+// Otherwise the old buffer is freed once the stream is idle, the new one is zeroed and ws_gen moves on.
+static bool grow_buf(b200_backend_ctx * ctx, dev_buf & b, size_t need) {
+    if (need <= b.bytes) return true;
+    if (ctx->capturing) { ctx->capture_failed = true; return false; }
+    if (b.p) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(b.p); }
+    CUDA_OK(cudaMalloc(&b.p, need + 256));
+    CUDA_OK(cudaMemsetAsync(b.p, 0, need + 256, ctx->stream));
+    b.bytes = need;
+    ctx->ws_gen++;
+    return true;
 }
+
+static const int64_t MMQ_MIN_COLS = 8;
 static bool type_is_quant(enum ggml_type t) {
     return t == GGML_TYPE_Q4_K || t == GGML_TYPE_Q5_K || t == GGML_TYPE_Q6_K || t == GGML_TYPE_Q8_0 || t == GGML_TYPE_Q5_1;
 }
@@ -250,7 +272,7 @@ static bool b200_supports_op(ggml_backend_dev_t, const ggml_tensor * op) {
             // quantized weights: rows of src1 must be dense.  The decode GEMV handles one activation column per launch; k-quant
             // weights with K % 256 == 0 take the tensor-core path (pb200_mul_mat_q) for any number of columns.
             if (!(ggml_is_contiguous(a) && b->nb[0] == sizeof(float) && ggml_is_contiguous(op) && a->ne[0] % ggml_blck_size(a->type) == 0)) return false;
-            if (mmq_ok(a->type, a->ne[0]) && b->nb[1] % 16 == 0) return true;
+            if (pb200_mul_mat_q_supported(a->type, a->ne[0]) && b->nb[1] % 16 == 0) return true;
             return b->ne[1] * b->ne[2] * b->ne[3] <= 64;
         }
         case GGML_OP_ROPE: {
@@ -324,33 +346,18 @@ static bool b200_compute_node(b200_backend_ctx * ctx, ggml_tensor * dst) {
                 return true;
             }
             const int64_t K = a->ne[0], N = a->ne[1];
-            const size_t need = pb200_act_workspace_bytes(K);
-            // no allocation inside a capture (as grow_ws): enqueue nothing, the capture is discarded and the call runs directly
-            if (need > ctx->act_ws_bytes && ctx->capturing) { ctx->capture_failed = true; return true; }
-            if (need > ctx->act_ws_bytes) {
-                if (ctx->act_ws) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->act_ws); }
-                CUDA_OK(cudaMalloc(&ctx->act_ws, need + 256));
-                ctx->act_ws_bytes = need;
-                ctx->ws_gen++;
-            }
+            if (!grow_buf(ctx, ctx->act_ws, pb200_act_workspace_bytes(K))) return true;
             const int64_t r2 = b->ne[2] / a->ne[2], r3 = b->ne[3] / a->ne[3];
-            if (b->ne[1] >= MMQ_MIN_COLS && mmq_ok(a->type, K) && b->nb[1] % 16 == 0 && (uintptr_t) b->data % 16 == 0 && b->nb[2] % 16 == 0 && b->nb[3] % 16 == 0 &&
+            if (b->ne[1] >= MMQ_MIN_COLS && pb200_mul_mat_q_supported(a->type, K) && b->nb[1] % 16 == 0 && (uintptr_t) b->data % 16 == 0 && b->nb[2] % 16 == 0 && b->nb[3] % 16 == 0 &&
                 (uintptr_t) a->data % 16 == 0 && a->nb[2] % 16 == 0 && a->nb[3] % 16 == 0) {   // the prep kernel reads rows as float4
                 // batched / prefill: the reference switches to mul_mat_q above 8 columns as well (ggml-cuda/mmq.cu:137-139)
-                const size_t need_q = pb200_mul_mat_q_workspace_bytes(K, b->ne[1]);
-                if (need_q > ctx->mmq_ws_bytes && ctx->capturing) { ctx->capture_failed = true; return true; }
-                if (need_q > ctx->mmq_ws_bytes) {
-                    if (ctx->mmq_ws) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->mmq_ws); }
-                    CUDA_OK(cudaMalloc(&ctx->mmq_ws, need_q + 256));
-                    ctx->mmq_ws_bytes = need_q;
-                    ctx->ws_gen++;
-                }
+                if (!grow_buf(ctx, ctx->mmq_ws, pb200_mul_mat_q_workspace_bytes(K, b->ne[1]))) return true;
                 for (int64_t i3 = 0; i3 < b->ne[3]; i3++)
                     for (int64_t i2 = 0; i2 < b->ne[2]; i2++) {
                         const char * w = (const char *) a->data + (i2 / r2) * a->nb[2] + (i3 / r3) * a->nb[3];
                         const float * x = (const float *) ((const char *) b->data + i2 * b->nb[2] + i3 * b->nb[3]);
                         float * y = (float *) ((char *) dst->data + i2 * dst->nb[2] + i3 * dst->nb[3]);
-                        PB_OK(pb200_mul_mat_q((int) a->type, w, N, K, x, (int64_t) (b->nb[1] / sizeof(float)), b->ne[1], y, nullptr, nullptr, ctx->mmq_ws, st));
+                        PB_OK(pb200_mul_mat_q((int) a->type, w, N, K, x, (int64_t) (b->nb[1] / sizeof(float)), b->ne[1], y, nullptr, nullptr, ctx->mmq_ws.p, st));
                     }
                 return true;
             }
@@ -360,7 +367,7 @@ static bool b200_compute_node(b200_backend_ctx * ctx, ggml_tensor * dst) {
                         const char * w = (const char *) a->data + (i2 / r2) * a->nb[2] + (i3 / r3) * a->nb[3];
                         const float * x = (const float *) ((const char *) b->data + i1 * b->nb[1] + i2 * b->nb[2] + i3 * b->nb[3]);
                         float * y = (float *) ((char *) dst->data + i1 * dst->nb[1] + i2 * dst->nb[2] + i3 * dst->nb[3]);
-                        PB_OK(pb200_mul_mat_vec((int) a->type, w, N, K, x, y, ctx->act_ws, st));
+                        PB_OK(pb200_mul_mat_vec((int) a->type, w, N, K, x, y, ctx->act_ws.p, st));
                     }
             return true;
         }
@@ -432,18 +439,11 @@ static void b200_backend_free(ggml_backend_t backend) {
     b200_backend_ctx * ctx = (b200_backend_ctx *) backend->context;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
-    if (ctx->act_ws) cudaFree(ctx->act_ws);
-    if (ctx->mmq_ws) cudaFree(ctx->mmq_ws);
-    for (void * p : ctx->fact_ws) if (p) cudaFree(p);
-    if (ctx->sync_ws) cudaFree(ctx->sync_ws);
-    if (ctx->attn_tmp) cudaFree(ctx->attn_tmp);
-    for (float * p : ctx->scratch) if (p) cudaFree(p);
     if (ctx->copy_event) cudaEventDestroy(ctx->copy_event);
-    if (ctx->kvh_dev) cudaFree(ctx->kvh_dev);
     if (ctx->kvh_host) cudaFreeHost(ctx->kvh_host);
     for (b200_plan * p : ctx->plans) delete p;
     cudaStreamDestroy(ctx->stream);
-    delete ctx;
+    delete ctx;   // frees the dev_bufs
     delete backend;
 }
 static ggml_backend_buffer_type_t b200_backend_get_default_buft(ggml_backend_t backend) {
@@ -502,22 +502,24 @@ static uint64_t graph_key(ggml_cgraph * g) {
     }
     return h;
 }
-static bool is_kq(enum ggml_type t) { return t == GGML_TYPE_Q4_K || t == GGML_TYPE_Q5_K || t == GGML_TYPE_Q6_K; }
 static bool is_vec_f32(const ggml_tensor * t, int64_t n) {
     return t && t->type == GGML_TYPE_F32 && t->ne[0] == n && t->ne[1] == 1 && t->ne[2] == 1 && t->ne[3] == 1 && t->nb[0] == sizeof(float);
 }
-// a MUL_MAT the fused GEMV takes: k-quant weights, one contiguous f32 activation column, K % 256 == 0, K <= 28672
+// a MUL_MAT the fused GEMV takes: weights pb200_gemv_fused accepts, one contiguous f32 activation column
 static bool gemv_fusable(const ggml_tensor * t) {
     if (t->op != GGML_OP_MUL_MAT) return false;
     const ggml_tensor * W = t->src[0], * X = t->src[1];
-    if (!is_kq(W->type) || !ggml_is_contiguous(W) || W->ne[2] != 1 || W->ne[3] != 1) return false;
-    const int64_t K = W->ne[0];
-    return is_vec_f32(X, K) && K % 256 == 0 && K <= 28672 && t->type == GGML_TYPE_F32 && ggml_is_contiguous(t);
+    if (!pb200_gemv_fused_supported(W->type, W->ne[0]) || !ggml_is_contiguous(W) || W->ne[2] != 1 || W->ne[3] != 1) return false;
+    return is_vec_f32(X, W->ne[0]) && t->type == GGML_TYPE_F32 && ggml_is_contiguous(t);
 }
 static const ggml_tensor * strip_views(const ggml_tensor * t) {   // RESHAPE / PERMUTE / TRANSPOSE / VIEW of a COMPUTED tensor
     while (t && (t->op == GGML_OP_RESHAPE || t->op == GGML_OP_PERMUTE || t->op == GGML_OP_TRANSPOSE || t->op == GGML_OP_VIEW) && t->src[0]) t = t->src[0];
     return t;
 }
+
+// How far apart the nodes of one motif lie: one layer's attention chain and the q|k|v group that feeds it sit within ATTN_WINDOW
+// nodes before its SOFT_MAX (its cache stores within ATTN_AHEAD after it), gate and up within FFN_WINDOW nodes before ffn_down.
+static const int ATTN_WINDOW = 96, ATTN_AHEAD = 16, FFN_WINDOW = 64;
 
 struct graph_info {
     ggml_cgraph * g;
@@ -526,6 +528,22 @@ struct graph_info {
     std::unordered_map<const ggml_tensor *, int> index;
     int idx(const ggml_tensor * t) const { auto it = index.find(t); return it == index.end() ? -1 : it->second; }
 };
+static graph_info index_graph(ggml_cgraph * g) {
+    graph_info G;
+    G.g = g; G.n = ggml_graph_n_nodes(g);
+    G.cons.assign(G.n, {});
+    G.index.reserve((size_t) G.n * 2);
+    for (int i = 0; i < G.n; i++) G.index[ggml_graph_node(g, i)] = i;
+    for (int i = 0; i < G.n; i++) {
+        const ggml_tensor * t = ggml_graph_node(g, i);
+        for (int k = 0; k < GGML_MAX_SRC; k++) {
+            if (!t->src[k]) continue;
+            const int j = G.idx(t->src[k]);
+            if (j >= 0 && j < i) G.cons[j].push_back(i);
+        }
+    }
+    return G;
+}
 // consumers of a node "through" no-op views: the real ops that eventually read it
 static void real_consumers(const graph_info & G, int i, std::vector<int> & out) {
     for (int c : G.cons[i]) {
@@ -533,6 +551,17 @@ static void real_consumers(const graph_info & G, int i, std::vector<int> & out) 
         if (is_noop(t->op)) real_consumers(G, c, out); else out.push_back(c);
     }
 }
+
+// the fused steps chosen so far
+struct fusion {
+    std::vector<char> taken;         // node computed by a fused step
+    std::vector<char> has;           // a fused step runs at node i: at[i]
+    std::vector<b200_step> at;
+    std::vector<int> attn_at;        // where the fused attention steps run
+    explicit fusion(int n) : taken(n, 0), has(n, 0), at(n) {}
+    void place(const b200_step & st) { at[st.node] = st; has[st.node] = 1; }
+    const gemv_step * gemv_at(int i) const { return has[i] && at[i].kind == step_kind::gemv ? &at[i].gemv : nullptr; }
+};
 
 static bool plan_attention(const graph_info & G, int soft, std::vector<char> & taken, b200_step & st) {
     ggml_cgraph * g = G.g;
@@ -547,7 +576,7 @@ static bool plan_attention(const graph_info & G, int soft, std::vector<char> & t
     const ggml_tensor * ropeq = strip_views(qp);
     if (!ropeq || ropeq->op != GGML_OP_ROPE || qp->ne[0] != 128 || qp->ne[1] != 1 || qp->ne[3] != 1) return false;   // [D, n_tokens = 1, H]
     const int64_t D = 128, H = qp->ne[2], n_kv = kview->ne[1], HK = kview->ne[2];
-    if (kview->ne[0] != D || HK <= 0 || H % HK || (H & 1) || (n_kv & 31)) return false;
+    if (kview->ne[0] != D || HK <= 0 || H % HK || (H & 1) || (n_kv & 31) || n_kv > pb200_attn_ggml_max_cells()) return false;
     if (kview->nb[1] != (size_t) (HK * D * 2) || kview->nb[2] != (size_t) (D * 2) || kview->view_offs != 0) return false;
     if (mask->ne[0] != n_kv || !ggml_is_contiguous(mask)) return false;
     // the single consumer chain soft_max -> mul_mat(v, p) -> permute -> cont
@@ -571,7 +600,7 @@ static bool plan_attention(const graph_info & G, int soft, std::vector<char> & t
     { std::vector<int> c; real_consumers(G, kq_i, c); if (c.size() != 1 || c[0] != soft) return false; }
     // k side: a ROPE node with the same parameters whose only consumer is a CPY into a view of the same K cache tensor
     int ropek_i = -1, cpyk_i = -1;
-    const int w0 = std::max(0, soft - 96), w1 = std::min(G.n, soft + 16);   // the chain of one layer sits within a few dozen nodes
+    const int w0 = std::max(0, soft - ATTN_WINDOW), w1 = std::min(G.n, soft + ATTN_AHEAD);
     for (int i = w0; i < w1; i++) {
         const ggml_tensor * t = ggml_graph_node(g, i);
         if (t->op != GGML_OP_CPY || !t->src[1] || t->src[1]->view_src != kview->view_src || taken[i]) continue;
@@ -606,9 +635,18 @@ static bool plan_attention(const graph_info & G, int soft, std::vector<char> & t
     if (G.idx(vsrc) > cont_i) return false;
     for (int i : nodes) taken[i] = 1;
     st = b200_step{};
-    st.kind = 2; st.rope_q = ropeq_i; st.rope_k = ropek_i; st.cpy_k = cpyk_i; st.cpy_v = cpyv_i; st.kq = kq_i; st.soft = soft; st.kqv = kqv_i; st.cont = cont_i;
-    st.node = cont_i; st.quant_out = 0;
+    st.kind = step_kind::attn;
+    st.node = cont_i;
+    st.attn = attn_step{ropeq_i, ropek_i, cpyk_i, cpyv_i, kq_i, soft, kqv_i, cont_i, false, false};
     return true;
+}
+// attention chains (anchor: SOFT_MAX; the step runs at its CONT node)
+static void plan_attention_chains(const graph_info & G, fusion & F) {
+    for (int i = 0; i < G.n; i++) {
+        if (ggml_graph_node(G.g, i)->op != GGML_OP_SOFT_MAX || F.taken[i]) continue;
+        b200_step st;
+        if (plan_attention(G, i, F.taken, st)) { F.place(st); F.attn_at.push_back(st.node); }
+    }
 }
 
 // vector added to a mul_mat result by the single consumer ADD (bias or residual): returns the ADD node index or -1
@@ -622,201 +660,185 @@ static int find_add(const graph_info & G, int mm_i, int & vec_src) {
     }
     return -1;
 }
-
-static b200_plan * build_plan(ggml_cgraph * g, uint64_t key) {
-    graph_info G;
-    G.g = g; G.n = ggml_graph_n_nodes(g);
-    G.cons.assign(G.n, {});
-    G.index.reserve((size_t) G.n * 2);
-    for (int i = 0; i < G.n; i++) G.index[ggml_graph_node(g, i)] = i;
-    for (int i = 0; i < G.n; i++) {
-        const ggml_tensor * t = ggml_graph_node(g, i);
-        for (int k = 0; k < GGML_MAX_SRC; k++) {
-            if (!t->src[k]) continue;
-            const int j = G.idx(t->src[k]);
-            if (j >= 0 && j < i) G.cons[j].push_back(i);
+// private buffer that a fused group within FFN_WINDOW nodes before `before` writes node n's result to (-1: none)
+static int private_slot_of(const fusion & F, int n, int before) {
+    int slot = -1;
+    for (int q = std::max(0, before - FFN_WINDOW); q < before; q++) {
+        const gemv_step * s = F.gemv_at(q);
+        if (!s) continue;
+        for (int j = 0; j < s->nmat; j++) if (s->out[j] == n) slot = s->out_slot[j];
+    }
+    return slot;
+}
+// The results of a multi-matrix group are produced at ONE point in time: each must be consumed only inside fused steps (attention:
+// q / k / v; silu prologue: gate / up) so that it can live in a private buffer.  Sets out_slot[]; false when a result has no slot.
+static bool assign_private_slots(const graph_info & G, const fusion & F, gemv_step & s, int first) {
+    ggml_cgraph * g = G.g;
+    bool all = true;
+    for (int j = 0; j < s.nmat; j++) {
+        const ggml_tensor * o = ggml_graph_node(g, s.out[j]);
+        std::vector<int> co; real_consumers(G, s.out[j], co);
+        int slot = -1;
+        if (co.size() == 1) {
+            for (int anchor : F.attn_at) {
+                if (anchor < first || anchor > first + ATTN_WINDOW) continue;
+                const attn_step & A = F.at[anchor].attn;
+                if (co[0] == A.rope_q && strip_views(ggml_graph_node(g, A.rope_q)->src[0]) == o) slot = SCR_Q;
+                if (co[0] == A.rope_k && strip_views(ggml_graph_node(g, A.rope_k)->src[0]) == o) slot = SCR_K;
+                if (co[0] == A.cpy_v && strip_views(ggml_graph_node(g, A.cpy_v)->src[0]) == o) slot = SCR_V;
+            }
+        }
+        if (slot < 0 && co.size() == 1) {
+            const ggml_tensor * c0 = ggml_graph_node(g, co[0]);
+            int mul_i = -1;
+            if (c0->op == GGML_OP_UNARY && ggml_get_unary_op(c0) == GGML_UNARY_OP_SILU) {
+                std::vector<int> cs; real_consumers(G, co[0], cs);
+                if (cs.size() == 1) { slot = SCR_G; mul_i = cs[0]; }
+            } else if (c0->op == GGML_OP_MUL) {
+                const ggml_tensor * other = c0->src[0] == o ? c0->src[1] : c0->src[0];
+                if (other && other->op == GGML_OP_UNARY && ggml_get_unary_op(other) == GGML_UNARY_OP_SILU) { slot = SCR_U; mul_i = co[0]; }
+            }
+            // gate / up may only stay private if silu(gate) * up feeds a down projection the silu-prologue GEMV takes
+            // (an ffn_down of Q5_1 / Q8_0, as for n_ff % 256 != 0, runs 1:1 and reads gate / up from the graph)
+            if (slot >= 0) {
+                std::vector<int> cm; real_consumers(G, mul_i, cm);
+                if (cm.size() != 1 || !gemv_fusable(ggml_graph_node(g, cm[0]))) slot = -1;
+            }
+        }
+        s.out_slot[j] = slot;
+        if (slot < 0) all = false;
+    }
+    return all;
+}
+// the mat-vec group of MUL_MAT i: every k-quant mat-vec fed by its activation, with the producer of that activation as prologue
+static b200_step plan_gemv_group(const graph_info & G, fusion & F, int i) {
+    ggml_cgraph * g = G.g;
+    const ggml_tensor * X = ggml_graph_node(g, i)->src[1];
+    const int64_t K = ggml_graph_node(g, i)->src[0]->ne[0];
+    b200_step st{};
+    st.kind = step_kind::gemv;
+    gemv_step & s = st.gemv;
+    const auto drop_prologue = [&s] { s.prologue = gemv_prologue::quantize; s.p0 = s.p1 = -1; };
+    drop_prologue();
+    const int xi = G.idx(X);
+    if (xi >= 0 && X->op == GGML_OP_MUL && !F.taken[xi]) {
+        // prologue candidates: MUL(RMS_NORM(x), w) or MUL(SILU(g), u), intermediate results read by nobody else
+        for (int k = 0; k < 2; k++) {
+            const ggml_tensor * a = X->src[k], * b = X->src[1 - k];
+            const int ai = G.idx(a);
+            if (ai < 0 || F.taken[ai]) continue;
+            std::vector<int> ca; real_consumers(G, ai, ca);
+            if (ca.size() != 1 || ca[0] != xi) continue;
+            const bool vectors = is_vec_f32(b, K) && ggml_is_contiguous(b) && is_vec_f32(a->src[0], K) && ggml_is_contiguous(a->src[0]);
+            if (a->op == GGML_OP_RMS_NORM && vectors) {
+                s.prologue = gemv_prologue::rms_norm; s.p0 = ai; s.p1 = xi;
+                break;
+            }
+            if (a->op == GGML_OP_UNARY && ggml_get_unary_op(a) == GGML_UNARY_OP_SILU && vectors) {
+                // gate and up must have been redirected to private buffers by the group that produced them (liveness, see above)
+                if (private_slot_of(F, G.idx(a->src[0]), i) == SCR_G && private_slot_of(F, G.idx(b), i) == SCR_U) {
+                    s.prologue = gemv_prologue::silu_mul; s.p0 = ai; s.p1 = xi;
+                }
+                break;
+            }
+        }
+    } else if (xi >= 0 && F.has[xi] && F.at[xi].kind == step_kind::attn) {
+        s.prologue = gemv_prologue::from_attn;   // X is the CONT of a fused attention step
+    }
+    // all k-quant mat-vecs fed by X
+    std::vector<int> cx, group;
+    if (xi >= 0) real_consumers(G, xi, cx); else cx.push_back(i);
+    bool all_mm = true;
+    for (int c : cx) {
+        const ggml_tensor * m = ggml_graph_node(g, c);
+        if (m->op != GGML_OP_MUL_MAT || m->src[1] != X || m->src[0]->ne[0] != K || !pb200_gemv_fused_supported(m->src[0]->type, K) ||
+            !ggml_is_contiguous(m->src[0]) || m->src[0]->ne[2] != 1 || m->src[0]->ne[3] != 1 || !ggml_is_contiguous(m) || F.taken[c]) { all_mm = false; break; }
+    }
+    if (!all_mm || cx.size() > 3) {
+        // somebody else reads the activation (or too many matrices): keep it materialised, one launch per matrix
+        if (s.p0 >= 0 || (s.prologue == gemv_prologue::from_attn && cx.size() != 1)) drop_prologue();
+        group.push_back(i);
+    } else {
+        group = cx;
+        std::sort(group.begin(), group.end());
+    }
+    const auto take_group = [&](const std::vector<int> & mats) {
+        s.nmat = (int) mats.size();
+        for (int j = 0; j < s.nmat; j++) {
+            s.mm[j] = s.out[j] = mats[j]; s.add_src[j] = -1; s.out_slot[j] = -1;
+            int vs = 0;
+            const int ad = find_add(G, mats[j], vs);
+            // with several matrices the step runs later than some of its ADDs: only fold vectors that cannot have been recycled
+            // by the graph allocator in between (leafs: biases)
+            if (ad >= 0 && !F.taken[ad] && (s.nmat == 1 || ggml_graph_node(g, ad)->src[vs]->op == GGML_OP_NONE)) { s.out[j] = ad; s.add_src[j] = vs; }
+        }
+    };
+    take_group(group);
+    if (s.nmat > 1 && !assign_private_slots(G, F, s, i)) {
+        // not the llama / qwen2 motif: one launch per matrix at its own position, activation materialised
+        if (s.p0 >= 0) drop_prologue();
+        take_group({i});
+    }
+    if (s.prologue == gemv_prologue::from_attn) F.at[xi].attn.quant_out = true;
+    st.node = 0;
+    for (int j = 0; j < s.nmat; j++) { F.taken[s.mm[j]] = 1; F.taken[s.out[j]] = 1; st.node = std::max(st.node, s.out[j]); }
+    if (s.p0 >= 0) { F.taken[s.p0] = 1; F.taken[s.p1] = 1; }
+    return st;
+}
+// mat-vec groups (anchor: the activation shared by k-quant MUL_MATs with one column; the step runs at its last output)
+static void plan_gemv_groups(const graph_info & G, fusion & F) {
+    for (int i = 0; i < G.n; i++)
+        if (!F.taken[i] && gemv_fusable(ggml_graph_node(G.g, i))) F.place(plan_gemv_group(G, F, i));
+}
+// Every fused attention must take q / k / v from private buffers filled by a fused group, and every gate / up kept private must be
+// read by a silu·mul step: nothing else sees the private buffers.  False: no fusion for this graph.  Also decides which attention
+// outputs stay private (wo consumes the quantized copy).
+static bool private_buffers_consistent(const graph_info & G, fusion & F) {
+    ggml_cgraph * g = G.g;
+    for (int anchor : F.attn_at) {
+        attn_step & A = F.at[anchor].attn;
+        const ggml_tensor * src[3] = {strip_views(ggml_graph_node(g, A.rope_q)->src[0]), strip_views(ggml_graph_node(g, A.rope_k)->src[0]),
+                                      strip_views(ggml_graph_node(g, A.cpy_v)->src[0])};   // q, k, v: SCR_Q, SCR_K, SCR_V
+        bool found[3] = {false, false, false};
+        for (int q = std::max(0, anchor - ATTN_WINDOW); q < anchor; q++) {
+            const gemv_step * s = F.gemv_at(q);
+            if (!s) continue;
+            for (int j = 0; j < s->nmat; j++)
+                for (int r = 0; r < 3; r++) found[r] = found[r] || (ggml_graph_node(g, s->out[j]) == src[r] && s->out_slot[j] == SCR_Q + r);
+        }
+        if (!found[0] || !found[1] || !found[2]) return false;
+        std::vector<int> co; real_consumers(G, A.cont, co);
+        A.out_private = A.quant_out && co.size() == 1;
+    }
+    for (int q = 0; q < G.n; q++) {
+        const gemv_step * s = F.gemv_at(q);
+        if (!s) continue;
+        for (int j = 0; j < s->nmat; j++) {
+            const int slot = s->out_slot[j];
+            if (slot != SCR_G && slot != SCR_U) continue;
+            const ggml_tensor * o = ggml_graph_node(g, s->out[j]);
+            bool read = false;
+            for (int r = 0; r < G.n && !read; r++) {
+                const gemv_step * c = F.gemv_at(r);
+                if (!c || c->prologue != gemv_prologue::silu_mul) continue;
+                const ggml_tensor * un = ggml_graph_node(g, c->p0), * mul = ggml_graph_node(g, c->p1);
+                const ggml_tensor * up = mul->src[0] == un ? mul->src[1] : mul->src[0];
+                read = slot == SCR_G ? un->src[0] == o : up == o;
+            }
+            if (!read) return false;
         }
     }
-    std::vector<char> taken(G.n, 0);
-    std::vector<b200_step> at(G.n);          // fused step anchored at node i (kind != 0)
-    std::vector<char> has(G.n, 0);
-    static const bool no_fuse = getenv("GGML_B200_NO_FUSE") != nullptr;
-    bool fused_ok = !no_fuse;
-    std::vector<int> attn_anchor;
-    if (fused_ok) {
-        // 1) attention chains (anchor: SOFT_MAX; the step runs at its CONT node)
-        for (int i = 0; i < G.n; i++) {
-            const ggml_tensor * t = ggml_graph_node(g, i);
-            if (t->op != GGML_OP_SOFT_MAX || taken[i]) continue;
-            b200_step st;
-            if (plan_attention(G, i, taken, st)) {
-                st.q_scratch = st.k_scratch = st.v_scratch = -1; st.out_private = 0;
-                at[st.node] = st; has[st.node] = 1; attn_anchor.push_back(st.node);
-            }
-        }
-        // 2) mat-vec groups (anchor: the activation shared by k-quant MUL_MATs with one column)
-        for (int i = 0; i < G.n; i++) {
-            const ggml_tensor * t = ggml_graph_node(g, i);
-            if (taken[i] || !gemv_fusable(t)) continue;
-            const ggml_tensor * W = t->src[0], * X = t->src[1];
-            const int64_t K = W->ne[0];
-            b200_step st{};
-            st.kind = 1; st.prologue = 0; st.p0 = st.p1 = -1; st.ws = 0;
-            for (int j = 0; j < 3; j++) st.out_scratch[j] = -1;
-            st.in_scratch[0] = st.in_scratch[1] = -1;
-            const int xi = G.idx(X);
-            if (xi >= 0 && X->op == GGML_OP_MUL && !taken[xi]) {
-                // prologue candidates: MUL(RMS_NORM(x), w) or MUL(SILU(g), u), intermediate results read by nobody else
-                for (int k = 0; k < 2; k++) {
-                    const ggml_tensor * a = X->src[k], * b = X->src[1 - k];
-                    const int ai = G.idx(a);
-                    if (ai < 0 || taken[ai]) continue;
-                    std::vector<int> ca; real_consumers(G, ai, ca);
-                    if (ca.size() != 1 || ca[0] != xi) continue;
-                    if (a->op == GGML_OP_RMS_NORM && is_vec_f32(b, K) && ggml_is_contiguous(b) && is_vec_f32(a->src[0], K) && ggml_is_contiguous(a->src[0])) {
-                        st.prologue = 1; st.p0 = ai; st.p1 = xi; st.ws = 0; break;
-                    }
-                    if (a->op == GGML_OP_UNARY && ggml_get_unary_op(a) == GGML_UNARY_OP_SILU && is_vec_f32(b, K) && ggml_is_contiguous(b) &&
-                        is_vec_f32(a->src[0], K) && ggml_is_contiguous(a->src[0])) {
-                        // gate and up must have been redirected to private buffers by the group that produced them (liveness, see above)
-                        const int gi = G.idx(a->src[0]), ui = G.idx(b);
-                        int sg = -1, su = -1;
-                        for (int q = std::max(0, i - 64); q < i; q++) {
-                            if (!has[q] || at[q].kind != 1) continue;
-                            for (int j = 0; j < at[q].nmat; j++) {
-                                if (at[q].out[j] == gi) sg = at[q].out_scratch[j];
-                                if (at[q].out[j] == ui) su = at[q].out_scratch[j];
-                            }
-                        }
-                        if (sg >= 0 && su >= 0) { st.prologue = 2; st.p0 = ai; st.p1 = xi; st.ws = 2; st.in_scratch[0] = sg; st.in_scratch[1] = su; }
-                        break;
-                    }
-                }
-            } else if (xi >= 0 && has[xi] && at[xi].kind == 2) {
-                st.prologue = 3; st.ws = 1;                                   // X is the CONT of a fused attention step
-            }
-            // all k-quant mat-vecs fed by X
-            std::vector<int> cx, group;
-            if (xi >= 0) real_consumers(G, xi, cx); else cx.push_back(i);
-            bool all_mm = true;
-            for (int c : cx) {
-                const ggml_tensor * m = ggml_graph_node(g, c);
-                if (m->op != GGML_OP_MUL_MAT || m->src[1] != X || !is_kq(m->src[0]->type) || m->src[0]->ne[0] != K || !ggml_is_contiguous(m->src[0]) ||
-                    m->src[0]->ne[2] != 1 || m->src[0]->ne[3] != 1 || !ggml_is_contiguous(m) || taken[c]) { all_mm = false; break; }
-            }
-            if (!all_mm || cx.size() > 3) {
-                // somebody else reads the activation (or too many matrices): keep it materialised, one launch per matrix
-                if (st.prologue == 1 || st.prologue == 2) { st.prologue = 0; st.p0 = st.p1 = -1; st.in_scratch[0] = st.in_scratch[1] = -1; }
-                if (st.prologue == 3 && cx.size() != 1) st.prologue = 0;
-                group.push_back(i);
-            } else {
-                group = cx;
-                std::sort(group.begin(), group.end());
-            }
-            st.nmat = (int) group.size();
-            int last = 0;
-            bool need_graph_buffers = false;
-            for (int j = 0; j < st.nmat; j++) {
-                st.mm[j] = group[j]; st.out[j] = group[j]; st.add_vec[j] = -1; st.add_src[j] = 0;
-                int vs = 0;
-                const int ad = find_add(G, group[j], vs);
-                // with several matrices the step runs later than some of its ADDs: only fold vectors that cannot have been recycled
-                // by the graph allocator in between (leafs: biases)
-                if (ad >= 0 && !taken[ad] && (st.nmat == 1 || ggml_graph_node(g, ad)->src[vs]->op == GGML_OP_NONE)) { st.out[j] = ad; st.add_vec[j] = ad; st.add_src[j] = vs; }
-                last = std::max(last, st.out[j]);
-            }
-            if (st.nmat > 1) {
-                // results of a multi-matrix group are produced at ONE point in time: each must be consumed only inside fused steps
-                // (attention: q / k / v; silu prologue: gate / up) so that it can live in a private buffer
-                for (int j = 0; j < st.nmat; j++) {
-                    std::vector<int> co; real_consumers(G, st.out[j], co);
-                    int slot = -1;
-                    for (int anchor : attn_anchor) {
-                        if (anchor < i || anchor > i + 96) continue;
-                        const b200_step & A = at[anchor];
-                        const ggml_tensor * o = ggml_graph_node(g, st.out[j]);
-                        if (co.size() == 1 && co[0] == A.rope_q && strip_views(ggml_graph_node(g, A.rope_q)->src[0]) == o) slot = SCR_Q;
-                        if (co.size() == 1 && co[0] == A.rope_k && strip_views(ggml_graph_node(g, A.rope_k)->src[0]) == o) slot = SCR_K;
-                        if (co.size() == 1 && co[0] == A.cpy_v && strip_views(ggml_graph_node(g, A.cpy_v)->src[0]) == o) slot = SCR_V;
-                    }
-                    if (slot < 0 && co.size() == 1) {
-                        const ggml_tensor * c0 = ggml_graph_node(g, co[0]);
-                        int mul_i = -1;
-                        if (c0->op == GGML_OP_UNARY && ggml_get_unary_op(c0) == GGML_UNARY_OP_SILU) {
-                            std::vector<int> cs; real_consumers(G, co[0], cs);
-                            if (cs.size() == 1) { slot = SCR_G; mul_i = cs[0]; }
-                        } else if (c0->op == GGML_OP_MUL) {
-                            const ggml_tensor * other = c0->src[0] == ggml_graph_node(g, st.out[j]) ? c0->src[1] : c0->src[0];
-                            if (other && other->op == GGML_OP_UNARY && ggml_get_unary_op(other) == GGML_UNARY_OP_SILU) { slot = SCR_U; mul_i = co[0]; }
-                        }
-                        // gate / up may only stay private if silu(gate) * up feeds a down projection the silu-prologue GEMV takes
-                        // (an ffn_down of Q5_1 / Q8_0, as for n_ff % 256 != 0, runs 1:1 and reads gate / up from the graph)
-                        if (slot >= 0) {
-                            std::vector<int> cm; real_consumers(G, mul_i, cm);
-                            if (cm.size() != 1 || !gemv_fusable(ggml_graph_node(g, cm[0]))) slot = -1;
-                        }
-                    }
-                    st.out_scratch[j] = slot;
-                    if (slot < 0) need_graph_buffers = true;
-                }
-                if (need_graph_buffers) {   // not the llama / qwen2 motif: one launch per matrix at its own position, activation materialised
-                    if (st.prologue == 1 || st.prologue == 2) { st.prologue = 0; st.p0 = st.p1 = -1; }
-                    st.nmat = 1; st.mm[0] = i; st.out[0] = i; st.add_vec[0] = -1; st.out_scratch[0] = -1;
-                    int vs = 0;
-                    const int ad = find_add(G, i, vs);
-                    if (ad >= 0 && !taken[ad]) { st.out[0] = ad; st.add_vec[0] = ad; st.add_src[0] = vs; }
-                    last = st.out[0];
-                }
-            }
-            if (st.prologue == 3) at[xi].quant_out = 1;
-            for (int j = 0; j < st.nmat; j++) { taken[st.mm[j]] = 1; taken[st.out[j]] = 1; }
-            if (st.p0 >= 0) { taken[st.p0] = 1; taken[st.p1] = 1; }
-            st.node = last;
-            at[last] = st; has[last] = 1;
-        }
-        // 3) every fused attention must take q / k / v from private buffers filled by a fused group, and its f32 result is private when
-        //    wo consumes the quantized copy; a SILU prologue needs its producer likewise.  Anything else: no fusion for this graph.
-        for (int anchor : attn_anchor) {
-            b200_step & A = at[anchor];
-            const ggml_tensor * qs = strip_views(ggml_graph_node(g, A.rope_q)->src[0]), * ks = strip_views(ggml_graph_node(g, A.rope_k)->src[0]);
-            const ggml_tensor * vs = strip_views(ggml_graph_node(g, A.cpy_v)->src[0]);
-            for (int q = std::max(0, anchor - 96); q < anchor; q++) {
-                if (!has[q] || at[q].kind != 1) continue;
-                for (int j = 0; j < at[q].nmat; j++) {
-                    const ggml_tensor * o = ggml_graph_node(g, at[q].out[j]);
-                    if (o == qs && at[q].out_scratch[j] == SCR_Q) A.q_scratch = SCR_Q;
-                    if (o == ks && at[q].out_scratch[j] == SCR_K) A.k_scratch = SCR_K;
-                    if (o == vs && at[q].out_scratch[j] == SCR_V) A.v_scratch = SCR_V;
-                }
-            }
-            if (A.q_scratch < 0 || A.k_scratch < 0 || A.v_scratch < 0) fused_ok = false;
-            std::vector<int> co; real_consumers(G, A.cont, co);
-            A.out_private = (A.quant_out && co.size() == 1) ? 1 : 0;
-        }
-        // and every gate / up kept private must be read by a silu-prologue step: nothing else sees the private buffers
-        for (int q = 0; q < G.n; q++) {
-            if (!has[q] || at[q].kind != 1) continue;
-            for (int j = 0; j < at[q].nmat; j++) {
-                const int slot = at[q].out_scratch[j];
-                if (slot != SCR_G && slot != SCR_U) continue;
-                const ggml_tensor * o = ggml_graph_node(g, at[q].out[j]);
-                bool read = false;
-                for (int r = 0; r < G.n && !read; r++) {
-                    if (!has[r] || at[r].kind != 1 || at[r].prologue != 2) continue;
-                    const ggml_tensor * un = ggml_graph_node(g, at[r].p0), * mul = ggml_graph_node(g, at[r].p1);
-                    const ggml_tensor * up = mul->src[0] == un ? mul->src[1] : mul->src[0];
-                    read = slot == SCR_G ? (un->src[0] == o && at[r].in_scratch[0] == SCR_G) : (up == o && at[r].in_scratch[1] == SCR_U);
-                }
-                if (!read) fused_ok = false;
-            }
-        }
-    }
+    return true;
+}
+// the steps in graph order: a fused step at its node, every other node not folded into one 1:1
+static b200_plan * emit_plan(const graph_info & G, const fusion & F, bool fused, uint64_t key) {
+    ggml_cgraph * g = G.g;
     b200_plan * plan = new b200_plan();
     plan->key = key; plan->n_nodes = G.n;
-    if (fused_ok) {
-        for (int anchor : attn_anchor) {
+    if (fused) {
+        for (int anchor : F.attn_at) {
             plan->has_attn = true;
-            for (int i : {at[anchor].cpy_k, at[anchor].cpy_v}) {
+            for (int i : {F.at[anchor].attn.cpy_k, F.at[anchor].attn.cpy_v}) {
                 plan->store_nodes.push_back(i);
                 const int v = G.idx(ggml_graph_node(g, i)->src[1]);
                 if (v >= 0) plan->store_nodes.push_back(v);
@@ -824,84 +846,82 @@ static b200_plan * build_plan(ggml_cgraph * g, uint64_t key) {
         }
     }
     for (int i = 0; i < G.n; i++) {
-        if (fused_ok && has[i]) { plan->steps.push_back(at[i]); continue; }
-        if (fused_ok && taken[i]) continue;
+        if (fused && F.has[i]) { plan->steps.push_back(F.at[i]); continue; }
+        if (fused && F.taken[i]) continue;
         const ggml_tensor * t = ggml_graph_node(g, i);
         if (ggml_is_empty(t) || is_noop(t->op)) continue;
         b200_step st{};
-        st.kind = 0; st.node = i;
+        st.kind = step_kind::node; st.node = i;
         plan->steps.push_back(st);
     }
     return plan;
 }
+static b200_plan * build_plan(ggml_cgraph * g, uint64_t key) {
+    const graph_info G = index_graph(g);
+    fusion F(G.n);
+    static const bool no_fuse = getenv("GGML_B200_NO_FUSE") != nullptr;
+    bool fused = !no_fuse;
+    if (fused) {
+        plan_attention_chains(G, F);
+        plan_gemv_groups(G, F);
+        fused = private_buffers_consistent(G, F);
+    }
+    return emit_plan(G, F, fused, key);
+}
 
-static float * grow_scratch(b200_backend_ctx * ctx, int slot, size_t floats) {
-    if (floats > ctx->scratch_floats[slot] && ctx->capturing) { ctx->capture_failed = true; return ctx->scratch[slot]; }
-    if (floats > ctx->scratch_floats[slot]) {
-        if (ctx->scratch[slot]) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->scratch[slot]); }
-        CUDA_OK(cudaMalloc((void **) &ctx->scratch[slot], floats * 4 + 256));
-        ctx->scratch_floats[slot] = floats;
-        ctx->ws_gen++;
-    }
-    return ctx->scratch[slot];
-}
-static void * grow_ws(b200_backend_ctx * ctx, int role, size_t need) {
-    if (need > ctx->fact_bytes[role] && ctx->capturing) { ctx->capture_failed = true; return ctx->fact_ws[role]; }   // no allocation inside a capture
-    if (need > ctx->fact_bytes[role]) {
-        if (ctx->fact_ws[role]) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->fact_ws[role]); }
-        CUDA_OK(cudaMalloc(&ctx->fact_ws[role], need + 256));
-        ctx->fact_bytes[role] = need;
-        ctx->ws_gen++;
-    }
-    return ctx->fact_ws[role];
-}
 static bool overlaps(const void * a, size_t na, const void * b, size_t nb) {
     const char * pa = (const char *) a, * pb = (const char *) b;
     return pa < pb + nb && pb < pa + na;
 }
 
-static bool run_gemv_step(b200_backend_ctx * ctx, ggml_cgraph * g, const b200_step & st) {
-    const ggml_tensor * m0 = ggml_graph_node(g, st.mm[0]);
+// Each run_*_step returns false when it enqueued nothing because the library refused the launch, true otherwise (also when a
+// workspace would have to grow inside a capture: that capture is abandoned).
+static bool run_gemv_step(b200_backend_ctx * ctx, ggml_cgraph * g, const gemv_step & s) {
+    const ggml_tensor * m0 = ggml_graph_node(g, s.mm[0]);
     const int64_t K = m0->src[0]->ne[0];
     pb200_gemv_mat mats[3];
-    for (int j = 0; j < st.nmat; j++) {
-        const ggml_tensor * mm = ggml_graph_node(g, st.mm[j]);
-        const ggml_tensor * out = ggml_graph_node(g, st.out[j]);
+    for (int j = 0; j < s.nmat; j++) {
+        const ggml_tensor * mm = ggml_graph_node(g, s.mm[j]);
+        const ggml_tensor * out = ggml_graph_node(g, s.out[j]);
+        const int64_t n = mm->src[0]->ne[1];
+        if (s.out_slot[j] >= 0 && !grow_buf(ctx, ctx->scratch[s.out_slot[j]], (size_t) n * sizeof(float))) return true;
         mats[j].type = (int32_t) mm->src[0]->type; mats[j]._pad = 0;
-        mats[j].W = mm->src[0]->data; mats[j].n = mm->src[0]->ne[1];
-        mats[j].y = st.out_scratch[j] >= 0 ? grow_scratch(ctx, st.out_scratch[j], (size_t) mm->src[0]->ne[1]) : (float *) out->data;
-        mats[j].add = st.add_vec[j] >= 0 ? (const float *) out->src[st.add_src[j]]->data : nullptr;
+        mats[j].W = mm->src[0]->data; mats[j].n = n;
+        mats[j].y = s.out_slot[j] >= 0 ? (float *) ctx->scratch[s.out_slot[j]].p : (float *) out->data;
+        mats[j].add = s.add_src[j] >= 0 ? (const float *) out->src[s.add_src[j]]->data : nullptr;
     }
-    void * ws = grow_ws(ctx, st.ws, pb200_act_workspace_bytes(K));
-    if (!ctx->sync_ws && ctx->capturing) { ctx->capture_failed = true; return true; }
-    if (!ctx->sync_ws) { CUDA_OK(cudaMalloc(&ctx->sync_ws, 256)); CUDA_OK(cudaMemsetAsync(ctx->sync_ws, 0, 256, ctx->stream)); ctx->ws_gen++; }
-    int rc;
-    if (st.prologue == 1) {
-        const ggml_tensor * nrm = ggml_graph_node(g, st.p0), * mul = ggml_graph_node(g, st.p1);
-        float eps; memcpy(&eps, nrm->op_params, 4);
-        const ggml_tensor * w = mul->src[0] == nrm ? mul->src[1] : mul->src[0];
-        rc = pb200_gemv_fused(st.nmat, mats, K, ws, 1, (const float *) nrm->src[0]->data, (const float *) w->data, eps, ctx->sync_ws, 1, ctx->stream);
-    } else if (st.prologue == 2) {
-        const ggml_tensor * un = ggml_graph_node(g, st.p0), * mul = ggml_graph_node(g, st.p1);
-        const ggml_tensor * u = mul->src[0] == un ? mul->src[1] : mul->src[0];
-        (void) un; (void) mul; (void) u;
-        rc = pb200_gemv_fused(st.nmat, mats, K, ws, 2, ctx->scratch[st.in_scratch[0]], ctx->scratch[st.in_scratch[1]], 0.f, ctx->sync_ws, 1, ctx->stream);
-    } else {
-        if (st.prologue == 0) {
-            PB_OK(pb200_quantize_act((int) m0->src[0]->type, (const float *) m0->src[1]->data, K, ws, ctx->stream));
+    dev_buf & ws = ctx->fact_ws[act_role(s.prologue)];
+    if (!grow_buf(ctx, ws, pb200_act_workspace_bytes(K)) || !grow_buf(ctx, ctx->sync_ws, 16)) return true;
+    int rc = PB200_EINVAL;
+    switch (s.prologue) {
+        case gemv_prologue::rms_norm: {
+            const ggml_tensor * nrm = ggml_graph_node(g, s.p0), * mul = ggml_graph_node(g, s.p1);
+            float eps; memcpy(&eps, nrm->op_params, 4);
+            const ggml_tensor * w = mul->src[0] == nrm ? mul->src[1] : mul->src[0];
+            rc = pb200_gemv_fused(s.nmat, mats, K, ws.p, 1, (const float *) nrm->src[0]->data, (const float *) w->data, eps, ctx->sync_ws.p, 1, ctx->stream);
+            break;
         }
-        rc = pb200_gemv_fused(st.nmat, mats, K, ws, 0, nullptr, nullptr, 0.f, ctx->sync_ws, 1, ctx->stream);
+        case gemv_prologue::silu_mul:
+            rc = pb200_gemv_fused(s.nmat, mats, K, ws.p, 2, (const float *) ctx->scratch[SCR_G].p, (const float *) ctx->scratch[SCR_U].p, 0.f, ctx->sync_ws.p,
+                                  1, ctx->stream);
+            break;
+        case gemv_prologue::quantize:
+            PB_OK(pb200_quantize_act((int) m0->src[0]->type, (const float *) m0->src[1]->data, K, ws.p, ctx->stream));
+            [[fallthrough]];
+        case gemv_prologue::from_attn:
+            rc = pb200_gemv_fused(s.nmat, mats, K, ws.p, 0, nullptr, nullptr, 0.f, ctx->sync_ws.p, 1, ctx->stream);
+            break;
     }
     if (rc == PB200_ENOTSUP) return false;
     PB_OK(rc);
     return true;
 }
 
-static bool run_attn_step(b200_backend_ctx * ctx, ggml_cgraph * g, const b200_step & st) {
-    const ggml_tensor * ropeq = ggml_graph_node(g, st.rope_q), * ropek = ggml_graph_node(g, st.rope_k);
-    const ggml_tensor * cpyk = ggml_graph_node(g, st.cpy_k), * cpyv = ggml_graph_node(g, st.cpy_v);
-    const ggml_tensor * kq = ggml_graph_node(g, st.kq), * sm = ggml_graph_node(g, st.soft), * kqv = ggml_graph_node(g, st.kqv);
-    ggml_tensor * cont = ggml_graph_node(g, st.cont);
+static bool run_attn_step(b200_backend_ctx * ctx, ggml_cgraph * g, const attn_step & a) {
+    const ggml_tensor * ropeq = ggml_graph_node(g, a.rope_q);
+    const ggml_tensor * cpyk = ggml_graph_node(g, a.cpy_k), * cpyv = ggml_graph_node(g, a.cpy_v);
+    const ggml_tensor * kq = ggml_graph_node(g, a.kq), * sm = ggml_graph_node(g, a.soft), * kqv = ggml_graph_node(g, a.kqv);
+    ggml_tensor * cont = ggml_graph_node(g, a.cont);
     const ggml_tensor * kview = kq->src[0], * vview = kqv->src[0], * mask = sm->src[1];
     const int64_t D = 128, H = kq->src[1]->ne[2], HK = kview->ne[2], n_kv = kview->ne[1];
     const int64_t vt_stride = (int64_t) (vview->nb[1] / 2);
@@ -914,27 +934,25 @@ static bool run_attn_step(b200_backend_ctx * ctx, ggml_cgraph * g, const b200_st
     float fb, fs, ef, af, bf, bsl, scale;
     memcpy(&fb, p + 5, 4); memcpy(&fs, p + 6, 4); memcpy(&ef, p + 7, 4); memcpy(&af, p + 8, 4); memcpy(&bf, p + 9, 4); memcpy(&bsl, p + 10, 4);
     memcpy(&scale, sm->op_params, 4);
-    const float * q = ctx->scratch[st.q_scratch], * k = ctx->scratch[st.k_scratch], * v = ctx->scratch[st.v_scratch];   // filled by the fused q|k|v group
-    float * out = st.out_private ? grow_scratch(ctx, SCR_ATT, (size_t) (H * D)) : (float *) cont->data;
-    const size_t out_bytes = (size_t) (H * D) * 4;
-    // the graph allocator may have placed the CONT result on top of q / k / v (their last readers are folded into this launch):
-    // heads finish at different times, so only the exact q <-> out aliasing (head h reads and writes its own slice) is safe
-    // q / k / v are private; the only graph tensor read while heads finish at different times is the mask row
-    bool via_tmp = !st.out_private && overlaps(out, out_bytes, mask->data, (size_t) n_kv * 4);
-    if (via_tmp) {
-        if (ctx->attn_tmp_floats < (size_t) (H * D) && ctx->capturing) { ctx->capture_failed = true; return false; }
-        if (ctx->attn_tmp_floats < (size_t) (H * D)) {
-            if (ctx->attn_tmp) { CUDA_OK(cudaStreamSynchronize(ctx->stream)); cudaFree(ctx->attn_tmp); }
-            CUDA_OK(cudaMalloc((void **) &ctx->attn_tmp, out_bytes + 256));
-            ctx->attn_tmp_floats = (size_t) (H * D);
-            ctx->ws_gen++;
-        }
-        out = ctx->attn_tmp;
+    const size_t out_bytes = (size_t) (H * D) * sizeof(float);
+    float * out = (float *) cont->data;
+    if (a.out_private) {
+        if (!grow_buf(ctx, ctx->scratch[SCR_ATT], out_bytes)) return true;
+        out = (float *) ctx->scratch[SCR_ATT].p;
     }
-    void * ws = st.quant_out ? grow_ws(ctx, 1, pb200_act_workspace_bytes(H * D)) : nullptr;
-    const int rc = pb200_attn_ggml(q, k, v, (void *) kview->data, (void *) vview->data, vt_stride, out, ws, (int) H, (int) HK, (int) D,
-                                   (const int32_t *) ropeq->src[1]->data, (int) n_kv, kv_head, ctx->capturing ? ctx->kvh_dev : nullptr, (const float *) mask->data, p[1], p[2],
-                                   fb, fs, ef, af, bf, bsl, p[4],
+    // q / k / v are private; the only graph tensor read while heads finish at different times is the mask row, on which the graph
+    // allocator may have placed the CONT result
+    const bool via_tmp = !a.out_private && overlaps(out, out_bytes, mask->data, (size_t) n_kv * 4);
+    if (via_tmp) {
+        if (!grow_buf(ctx, ctx->attn_tmp, out_bytes)) return true;
+        out = (float *) ctx->attn_tmp.p;
+    }
+    dev_buf & ws = ctx->fact_ws[act_role(gemv_prologue::from_attn)];
+    if (a.quant_out && !grow_buf(ctx, ws, pb200_act_workspace_bytes(H * D))) return true;
+    const int rc = pb200_attn_ggml((const float *) ctx->scratch[SCR_Q].p, (const float *) ctx->scratch[SCR_K].p, (const float *) ctx->scratch[SCR_V].p,
+                                   (void *) kview->data, (void *) vview->data, vt_stride, out, a.quant_out ? ws.p : nullptr, (int) H, (int) HK, (int) D,
+                                   (const int32_t *) ropeq->src[1]->data, (int) n_kv, kv_head, ctx->capturing ? (const int32_t *) ctx->kvh_dev.p : nullptr,
+                                   (const float *) mask->data, p[1], p[2], fb, fs, ef, af, bf, bsl, p[4],
                                    ropeq->src[2] ? (const float *) ropeq->src[2]->data : nullptr, scale, 1, ctx->stream);
     if (rc == PB200_ENOTSUP) return false;
     PB_OK(rc);
@@ -955,24 +973,37 @@ static void run_nodes_unfused(b200_backend_ctx * ctx, ggml_cgraph * g, const int
     }
 }
 
+// a fused step that reads or writes a private buffer: its nodes cannot run one by one, the graph's tensors never see those results
+static bool uses_private_buffers(const b200_step & st) {
+    if (st.kind == step_kind::attn) return true;   // q / k / v
+    const gemv_step & s = st.gemv;
+    if (s.prologue == gemv_prologue::silu_mul || s.prologue == gemv_prologue::from_attn) return true;   // gate / up; the quantized attention output
+    for (int j = 0; j < s.nmat; j++) if (s.out_slot[j] >= 0) return true;
+    return false;
+}
+
 static void run_plan(b200_backend_ctx * ctx, ggml_cgraph * cgraph, b200_plan * plan) {
     for (const b200_step & st : plan->steps) {
-        if (st.kind == 0) {
-            run_nodes_unfused(ctx, cgraph, &st.node, 1);
-        } else if (st.kind == 1) {
-            if (run_gemv_step(ctx, cgraph, st)) { g_nodes += st.nmat; g_fused_steps++; continue; }
-            // shape outside the fused kernel: the nodes of the group, in graph order
-            std::vector<int> nodes;
-            if (st.p0 >= 0) { nodes.push_back(st.p0); nodes.push_back(st.p1); }
-            for (int j = 0; j < st.nmat; j++) { nodes.push_back(st.mm[j]); if (st.out[j] != st.mm[j]) nodes.push_back(st.out[j]); }
-            std::sort(nodes.begin(), nodes.end());
-            run_nodes_unfused(ctx, cgraph, nodes.data(), (int) nodes.size());
-        } else {
-            if (run_attn_step(ctx, cgraph, st)) { g_nodes += 8; g_fused_steps++; continue; }
-            int nodes[8] = {st.rope_q, st.rope_k, st.cpy_k, st.cpy_v, st.kq, st.soft, st.kqv, st.cont};
-            std::sort(nodes, nodes + 8);
-            run_nodes_unfused(ctx, cgraph, nodes, 8);
+        if (st.kind == step_kind::node) { run_nodes_unfused(ctx, cgraph, &st.node, 1); continue; }
+        const bool gemv = st.kind == step_kind::gemv;
+        if (gemv ? run_gemv_step(ctx, cgraph, st.gemv) : run_attn_step(ctx, cgraph, st.attn)) {
+            g_nodes += gemv ? st.gemv.nmat : 8;
+            g_fused_steps++;
+            continue;
         }
+        if (uses_private_buffers(st)) {   // the planner fused a shape the library does not take
+            const ggml_tensor * t = ggml_graph_node(cgraph, st.node);
+            fprintf(stderr, "ggml-b200: the fused step at node %d (%s \"%s\") was refused and its nodes cannot run one by one\n", st.node,
+                    ggml_op_name(t->op), t->name);
+            GGML_ABORT("fused step refused");
+        }
+        // shape outside the fused kernel: the nodes of the group, in graph order
+        const gemv_step & s = st.gemv;
+        std::vector<int> nodes;
+        if (s.p0 >= 0) { nodes.push_back(s.p0); nodes.push_back(s.p1); }
+        for (int j = 0; j < s.nmat; j++) { nodes.push_back(s.mm[j]); if (s.out[j] != s.mm[j]) nodes.push_back(s.out[j]); }
+        std::sort(nodes.begin(), nodes.end());
+        run_nodes_unfused(ctx, cgraph, nodes.data(), (int) nodes.size());
     }
 }
 
@@ -980,8 +1011,8 @@ static void run_plan(b200_backend_ctx * ctx, ggml_cgraph * cgraph, b200_plan * p
 static int plan_kv_head(ggml_cgraph * g, const b200_plan * plan) {
     int kvh = -1;
     for (const b200_step & st : plan->steps) {
-        if (st.kind != 2) continue;
-        const ggml_tensor * cpyk = ggml_graph_node(g, st.cpy_k), * kq = ggml_graph_node(g, st.kq);
+        if (st.kind != step_kind::attn) continue;
+        const ggml_tensor * cpyk = ggml_graph_node(g, st.attn.cpy_k), * kq = ggml_graph_node(g, st.attn.kq);
         const ggml_tensor * kview = kq->src[0];
         const int64_t row = kview->ne[2] * 128 * 2;
         const int64_t off = (const char *) cpyk->data - (const char *) kview->data;
@@ -1019,16 +1050,15 @@ static enum ggml_status b200_backend_graph_compute(ggml_backend_t backend, ggml_
     const uint64_t bind = fnv(addr_bind, ctx->ws_gen);   // an exec captured before a workspace moved must not be replayed
     const int kvh = has_attn ? plan_kv_head(cgraph, plan) : -1;
     const bool graphable = use_graphs && kvh != -2 && plan->steps.size() >= 8;
-    if (graphable && !ctx->kvh_dev) {
-        CUDA_OK(cudaMalloc((void **) &ctx->kvh_dev, 256));
-        CUDA_OK(cudaMallocHost((void **) &ctx->kvh_host, 64 * sizeof(int32_t)));
-        ctx->ws_gen++;
+    if (graphable) {
+        grow_buf(ctx, ctx->kvh_dev, sizeof(int32_t));   // outside a capture: cannot refuse
+        if (!ctx->kvh_host) CUDA_OK(cudaMallocHost((void **) &ctx->kvh_host, 64 * sizeof(int32_t)));
     }
     auto push_cell = [&]() {
         if (kvh >= 0) {   // a ring of pinned words: the host may run several calls ahead of the copies
             int32_t * w = ctx->kvh_host + (ctx->kvh_idx++ & 63);
             *w = kvh;
-            CUDA_OK(cudaMemcpyAsync(ctx->kvh_dev, w, 4, cudaMemcpyHostToDevice, ctx->stream));
+            CUDA_OK(cudaMemcpyAsync(ctx->kvh_dev.p, w, 4, cudaMemcpyHostToDevice, ctx->stream));
         }
     };
     if (graphable && plan->exec && plan->bind == bind) {

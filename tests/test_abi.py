@@ -53,6 +53,17 @@ def test_argument_validation_no_gpu(lib, pkg):
     assert c.pb200_attn_prefill(None, None, None, None, 8, 2, 128, None, 4, 4, 0.1, None) == -1
 
 
+def test_fused_path_limits(lib):
+    """What the ggml-backend plugin plans with: the fused GEMV takes k-quant rows up to K = 29 696 (116 super-blocks), the
+    tensor-core product Q8_0 rows in 64-element steps."""
+    c = lib.c
+    assert c.pb200_gemv_fused_supported(12, C.c_int64(29696)) == 1
+    assert c.pb200_gemv_fused_supported(12, C.c_int64(29952)) == 0
+    assert c.pb200_gemv_fused_supported(8, C.c_int64(4096)) == 0     # Q8_0 is not a k-quant
+    assert c.pb200_mul_mat_q_supported(8, C.c_int64(4096)) == 1
+    assert c.pb200_mul_mat_q_supported(8, C.c_int64(4064)) == 0
+
+
 def test_hparams_layout_matches_header(pkg):
     assert C.sizeof(pkg.HParams) == 10 * 4 + 3 * 4
 

@@ -196,7 +196,9 @@ def test_attn_ggml_vs_oracle(cuda, lib, port, attn2_max_cells, heads, n_cells, k
 
 
 def test_attn_ggml_cell_limit(cuda, lib, attn2_max_cells):
-    """The next multiple of 32 past the largest accepted n_cells is refused with PB200_ENOTSUP, not launched."""
+    """The next multiple of 32 past the largest accepted n_cells is refused with PB200_ENOTSUP, not launched, and the library
+    reports that largest n_cells itself (the ggml-backend plugin plans with it)."""
+    assert lib.c.pb200_attn_ggml_max_cells() == attn2_max_cells
     case = AttnGgmlCase(lib, 8, 2, 32, 0, 0, False, D, "none", seed=2)
     n = attn2_max_cells + 32
     case.n_cells, case.mask = n, np.zeros(n, np.float32)

@@ -23,9 +23,11 @@ def run(arch, n_tok, dims=None, env=None):
     return json.loads(p.stdout.strip().splitlines()[-1])
 
 
-@pytest.mark.parametrize("arch", ["llama", "qwen2"])
-def test_whole_graph_matches_cpu_backend_and_is_fused(cuda, arch):
-    r = run(arch, 40)
+# n_ff 29 184 (114 super-blocks): an ffn_down the fused GEMV takes, past the 28 672 of Llama-3-70B
+@pytest.mark.parametrize("arch,dims", [("llama", None), ("qwen2", None), ("llama", [3, 1024, 8, 2, 29184, 384, 96])],
+                         ids=["llama", "qwen2", "llama-ff29184"])
+def test_whole_graph_matches_cpu_backend_and_is_fused(cuda, arch, dims):
+    r = run(arch, 40, dims)
     # same bar as the engine's multi-token parity (tests/test_gpu_engine.py::check_decode_parity): first token to fp32 summation
     # order, then the quantization-flip noise that the reference's own SIMD variants show against each other
     assert r["first_token_err"] < 1e-4, r
@@ -232,6 +234,25 @@ def test_supports_op_boundary(cuda, tmp_path):
     assert all(s["fused_steps"] >= 5 * r["n_layer"] for s in st[1:]), [s["fused_steps"] for s in st]
     check_logits(st)
     Layer0("qwen2", dims).check(np.load(tmp_path / "d.npz"), 1, 0, 100)
+
+
+def test_decode_past_attention_cell_limit(cuda, lib):
+    """n_ctx beyond the largest n_kv the fused attention launch takes: the planner fuses the attention chain up to that limit and
+    leaves it to the single ops past it, so q / k / v then reach them through the graph's tensors.  After a clear the stand-in
+    puts the token of position p in cell p, so decode steps at positions around the limit need no long prompt."""
+    max_cells = lib.c.pb200_attn_ggml_max_cells()
+    assert max_cells >= 4096, max_cells
+    dims = [3, 1024, 8, 2, 2816, 384, max_cells + 96]
+    r = run_script("llama", ["clear"] + decodes(max_cells - 2, 6), dims=dims)
+    st = r["steps"][1:]
+    assert [s["pos"] for s in st] == list(range(max_cells - 2, max_cells + 4))
+    for s in st:
+        assert s["unsupported_nodes"] == 0, s
+    # n_kv = max_cells: the fused plan (the bar of test_whole_graph_matches_cpu_backend_and_is_fused); n_kv = max_cells + 32: the
+    # attention chain and q / k / v one launch per node
+    per_layer = [(s["launches"] - 4) / r["n_layer"] for s in st]
+    assert max(per_layer[:2]) <= 6.0 and min(per_layer[2:]) > 6.0, per_layer
+    check_logits(st)
 
 
 REPLAY_SCRIPT = (["clear", prompt(16, 0)] * 3 + decodes(16, 12) + ["clear", prompt(40, 0)] + ["clear", prompt(16, 0)] * 3 + decodes(16, 12))
