@@ -177,7 +177,12 @@ def test_attn_ggml_vs_oracle(cuda, lib, port, attn2_max_cells, heads, n_cells, k
         assert n_cells >= 4096, n_cells
     if kv_head == "last":
         kv_head = n_cells - 1
-    case = AttnGgmlCase(lib, H, HK, n_cells, kv_head, mode, ff, n_dims, mask_kind, seed=n_cells * 7 + kv_head)
+    check_attn_ggml_case(lib, port, AttnGgmlCase(lib, H, HK, n_cells, kv_head, mode, ff, n_dims, mask_kind, seed=n_cells * 7 + kv_head))
+
+
+def check_attn_ggml_case(lib, port, case):
+    """One AttnGgmlCase against the oracle (fp32-order bar), its cache bytes and q8_K output bit for bit, and the kv_head_dev replay bit
+    for bit against the direct launch."""
     want, Kw, VTw = case.expected(lib, port)
     rc, out, act, Kc, VT = case.run(lib)
     assert rc == 0, rc
@@ -189,7 +194,7 @@ def test_attn_ggml_vs_oracle(cuda, lib, port, attn2_max_cells, heads, n_cells, k
     assert np.array_equal(VT.view(np.uint16), VTw.view(np.uint16)), "transposed V cache bytes"
     assert np.array_equal(act, port.quantize_act(O.Q4_K, out)), "q8_K of the output"
     # a captured graph replays with the cell in device memory: kv_head = 0 plus kv_head_dev must give the same bytes
-    rc2, out2, act2, Kc2, VT2 = case.run(lib, kv_head=0, kv_head_dev=kv_head)
+    rc2, out2, act2, Kc2, VT2 = case.run(lib, kv_head=0, kv_head_dev=case.kv_head)
     assert rc2 == 0
     assert np.array_equal(out2.view(np.uint32), out.view(np.uint32)) and np.array_equal(act2, act)
     assert np.array_equal(Kc2.view(np.uint16), Kc.view(np.uint16)) and np.array_equal(VT2.view(np.uint16), VT.view(np.uint16))

@@ -265,9 +265,12 @@ def test_prefill_matches_sequential_decode_and_oracle(cuda, pkg, port, arch, fty
     for i in range(T, len(toks)):
         eng.decode(int(toks[i]), i, got[i])
     eng.close()
+    check_prefill_parity(got, seq, want, T)
 
-    def nmse(a, b):
-        return float(np.sum((a - b) ** 2) / np.sum(b ** 2))
+
+def check_prefill_parity(got, seq, want, T):
+    """The bars above for a T-token prefill followed by decode steps: got[T - 1] holds the prefill's last-token logits and got[T:] the
+    decode steps after it; seq holds the engine's sequential decode of the same tokens and want the oracle's."""
     assert nmse(got[T - 1], seq[T - 1]) < 1e-3, nmse(got[T - 1], seq[T - 1])
     assert nmse(got[T - 1], want[T - 1]) < 2e-3
     assert seq[T - 1][got[T - 1].argmax()] >= seq[T - 1].max() - 0.1 and want[T - 1][got[T - 1].argmax()] >= want[T - 1].max() - 0.1
