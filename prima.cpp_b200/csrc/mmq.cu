@@ -502,7 +502,7 @@ __global__ void __launch_bounds__(MMQ_THREADS, 1) k_mmq_tc(const __grid_constant
 // as f16, q = round-half-even(x * 127 / amax), quantize_row_q8_0 ggml-quants.c:943-1010) instead of per 256 (q8_K).
 // Fused producers of the activation (pre_kind): PRO_SILU_MUL = silu(x) * aux[t][k] (llm_build_ffn's SILU + MUL in front of ffn_down, the f32
 // product never goes to HBM), PRO_RMSNORM = rms_norm(x) * aux[k] (llm_build_norm in front of q|k|v and gate|up): the same arithmetic, rounding for rounding, as
-// k_silu_mul / k_rms_norm_rows followed by the plain pass.
+// k_silu_mul / k_rms_norm_rows followed by the plain pass (tests/test_gpu_prefill_layers.py checks it bit for bit).
 // Operand range: the values d*q of row t are written as fp16 of d*q*2^e_t, e_t chosen so that the row's largest |d*q| lands in
 // [2^14, 2^15) (e_t <= 126: rows whose largest value is below 2^-112 stay below that), and rscale[t] = 2^-e_t, which the consumers'
 // epilogue applies to the fp32 accumulators.  So no activation overflows fp16 (|x| >= 65 520 was inf) or falls into its subnormals
