@@ -13,10 +13,11 @@
 namespace pb {
 
 // enum ggml_type values (ggml/include/ggml.h:356-395)
-enum : int { T_F32 = 0, T_F16 = 1, T_Q5_1 = 7, T_Q8_0 = 8, T_Q4_K = 12, T_Q5_K = 13, T_Q6_K = 14 };
+enum : int { T_F32 = 0, T_F16 = 1, T_Q4_0 = 2, T_Q4_1 = 3, T_Q5_0 = 6, T_Q5_1 = 7, T_Q8_0 = 8, T_Q4_K = 12, T_Q5_K = 13, T_Q6_K = 14 };
 
 constexpr int QK_K = 256;
 constexpr int BYTES_Q4_K = 144, BYTES_Q5_K = 176, BYTES_Q6_K = 210, BYTES_Q8_0 = 34, BYTES_Q5_1 = 24;
+constexpr int BYTES_Q4_0 = 18, BYTES_Q4_1 = 20, BYTES_Q5_0 = 22;   // ggml-common.h:143-170
 
 __host__ __device__ inline int64_t row_bytes(int type, int64_t k) {
     switch (type) {
@@ -27,19 +28,24 @@ __host__ __device__ inline int64_t row_bytes(int type, int64_t k) {
         case T_Q6_K: return k / 256 * BYTES_Q6_K;
         case T_Q8_0: return k / 32 * BYTES_Q8_0;
         case T_Q5_1: return k / 32 * BYTES_Q5_1;
+        case T_Q4_0: return k / 32 * BYTES_Q4_0;
+        case T_Q4_1: return k / 32 * BYTES_Q4_1;
+        case T_Q5_0: return k / 32 * BYTES_Q5_0;
     }
     return -1;
 }
 __host__ __device__ inline bool is_kquant(int t) { return t == T_Q4_K || t == T_Q5_K || t == T_Q6_K; }
-__host__ __device__ inline bool is_quant_type(int t) { return is_kquant(t) || t == T_Q8_0 || t == T_Q5_1; }   // the quantized weight types
-__host__ __device__ inline int block_elems(int t) { return is_kquant(t) ? 256 : ((t == T_Q8_0 || t == T_Q5_1) ? 32 : 1); }
+// the 32-element block types: one fp16 scale (and offset) per 32 weights
+__host__ __device__ inline bool is_blk32_type(int t) { return t == T_Q8_0 || t == T_Q5_1 || t == T_Q4_0 || t == T_Q4_1 || t == T_Q5_0; }
+__host__ __device__ inline bool is_quant_type(int t) { return is_kquant(t) || is_blk32_type(t); }   // the quantized weight types
+__host__ __device__ inline int block_elems(int t) { return is_kquant(t) ? 256 : (is_blk32_type(t) ? 32 : 1); }
 
 // ---------------------------------------------------------------------------------------------
 // Quantized activation vector in HBM (SoA so that a lane can pull its super-block with 128-bit loads).
 //   mode Q8_K (for Q4_K/Q5_K/Q6_K weights; mirrors block_q8_K, ggml-common.h:330-335):
 //       qs[K] int8, d[K/256] f32, bsums[K/16] int16
-//   mode Q8_0 (for Q8_0 weights; block_q8_0): qs[K], d[K/32] = fp16-rounded scale widened to f32
-//   mode Q8_1 (for Q5_1 weights; block_q8_1): qs[K], d[K/32], s[K/32] (both fp16-rounded, widened)
+//   mode Q8_0 (for Q8_0 / Q4_0 / Q5_0 weights; block_q8_0): qs[K], d[K/32] = fp16-rounded scale widened to f32
+//   mode Q8_1 (for Q5_1 / Q4_1 weights; block_q8_1): qs[K], d[K/32], s[K/32] (both fp16-rounded, widened)
 struct ActQ {
     int8_t * qs;      // [K]           16-B aligned
     float * d;        // [K/256] or [K/32]
@@ -55,7 +61,11 @@ __host__ __device__ inline int act_qs_stride(const ActQ & a) { return a.qs_strid
 __host__ __device__ inline int act_bs_stride(const ActQ & a) { return a.bs_stride ? a.bs_stride : 16; }
 constexpr int ACT_SMEM_QS_STRIDE = 272, ACT_SMEM_BS_STRIDE = 24;
 enum : int { ACT_Q8_K = 0, ACT_Q8_0 = 1, ACT_Q8_1 = 2 };
-__host__ __device__ inline int act_mode_for(int wtype) { return is_kquant(wtype) ? ACT_Q8_K : (wtype == T_Q8_0 ? ACT_Q8_0 : ACT_Q8_1); }
+// the weight type's vec_dot_type on the CPU (ggml/src/ggml.c:785-850): the offset types Q4_1 / Q5_1 take q8_1, whose s = d * sum(q)
+// pays for the offset term
+__host__ __device__ inline int act_mode_for(int wtype) {
+    return is_kquant(wtype) ? ACT_Q8_K : ((wtype == T_Q5_1 || wtype == T_Q4_1) ? ACT_Q8_1 : ACT_Q8_0);
+}
 
 // ---------------------------------------------------------------------------------------------
 // small PTX wrappers

@@ -128,7 +128,7 @@ __global__ void k_synth_blocks(uint8_t * p, int type, int64_t nblocks, int64_t K
     if (b >= nblocks) return;
     uint64_t s = seed * 0x100000001B3ull + (uint64_t) b * 0x9E3779B97F4A7C15ull;
     const float sc = rsqrtf((float) K);
-    const int bytes = type == T_Q4_K ? 144 : type == T_Q5_K ? 176 : type == T_Q6_K ? 210 : type == T_Q8_0 ? 34 : 24;
+    const int bytes = (int) row_bytes(type, block_elems(type));
     uint8_t * o = p + b * bytes;
     auto put16 = [&](int off, float v) { __half h = __float2half_rn(v); *reinterpret_cast<uint16_t *>(o + off) = __half_as_ushort(h); };
     auto fill = [&](int off, int n) {
@@ -146,6 +146,14 @@ __global__ void k_synth_blocks(uint8_t * p, int type, int64_t nblocks, int64_t K
     } else if (type == T_Q8_0) {
         put16(0, (0.5f + u01(s)) * sc / 73.f);
         fill(2, 32);
+    } else if (type == T_Q4_0 || type == T_Q5_0) {   // d (q - 8) / d (q - 16): symmetric around 0
+        put16(0, (0.5f + u01(s)) * sc / (type == T_Q4_0 ? 4.5f : 9.f));
+        fill(2, bytes - 2);
+    } else if (type == T_Q4_1) {
+        const float d = (0.5f + u01(s)) * sc / 4.5f;
+        put16(0, d);
+        put16(2, -d * 7.5f * (0.9f + 0.2f * u01(s)));
+        fill(4, 16);
     } else {
         const float d = (0.5f + u01(s)) * sc / 9.f;
         put16(0, d);
@@ -166,10 +174,10 @@ static bool use_more_bits(int i_layer, int n_layers) {   // src/llama.cpp:19278-
     return i_layer < n_layers / 8 || i_layer >= 7 * n_layers / 8 || (i_layer - n_layers / 8) % 3 == 2;
 }
 static int fallback_type(int t, int64_t k) {   // src/llama.cpp:19516-19551
-    if (k % 256 == 0) return t;
+    if (!is_kquant(t) || k % 256 == 0) return t;
+    if (t == T_Q4_K) return T_Q5_0;
     if (t == T_Q5_K) return T_Q5_1;
-    if (t == T_Q6_K) return T_Q8_0;
-    return -1;   // Q4_K -> Q5_0: not on this path
+    return T_Q8_0;   // Q6_K
 }
 
 static Tensor * find_tensor(pb200_model * m, const std::string & name, bool & is_f32, float *** f32slot, int64_t & n_f32) {
@@ -284,7 +292,8 @@ int pb200_model_synth(pb200_model * m, int ftype, uint64_t seed) {
     if (m->finalized) return PB200_ESTATE;
     cudaSetDevice(m->device);
     const pb200_hparams & hp = m->hp;
-    const int def = ftype == 0 ? T_Q4_K : T_Q5_K;
+    const int def = ftype == 0 ? T_Q4_K : ftype == 2 ? T_Q4_0 : T_Q5_K;
+    const bool kq = ftype != 2;   // Q4_0 (no imatrix): every matrix and the embedding Q4_0, only the head Q6_K (src/llama.cpp:19296-19460)
     const bool is70b = hp.n_layer == 80;   // MODEL_70B (src/llama.cpp:19385-19390)
     uint64_t sd = seed;
     auto synth = [&](Tensor & t, int type, int64_t N, int64_t K) -> int {
@@ -308,9 +317,9 @@ int pb200_model_synth(pb200_model * m, int ftype, uint64_t seed) {
     for (int il = m->l0; il < m->l1; il++) {
         Layer & L = m->layers[il - m->l0];
         const bool more = use_more_bits(il, hp.n_layer);
-        int tv = more ? T_Q6_K : def;
+        int tv = more && kq ? T_Q6_K : def;
         if (is70b && tv == T_Q4_K) tv = T_Q5_K;
-        const int td = more ? T_Q6_K : def;
+        const int td = more && kq ? T_Q6_K : def;
         CK(fvec(&L.attn_norm, E, 1.0f, 0.04f));
         CK(fvec(&L.ffn_norm, E, 1.0f, 0.04f));
         CK(synth(L.wq, def, QD, E));

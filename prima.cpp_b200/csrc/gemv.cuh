@@ -94,6 +94,7 @@ struct ActRegs {
     // 32-element block weight types (Q8_0 / Q5_1): the column = 8 consecutive blocks, activation q8_0 / q8_1 with one scale (and one
     // d * sum) per block; nb = how many of the 8 blocks exist (the last column of a K % 256 != 0 row is short)
     float d8[8], s8[8];
+    int as8[8];     // Q4_0 only: sum of the 32 activation q of each block (pays for the weights' -8 offset)
     int nb;
 };
 
@@ -320,6 +321,96 @@ __device__ __forceinline__ float dot_q5_1x8(const uint8_t * col, const ActRegs &
             }
             sumi += 16 * sumb;
             acc += (d * r.d8[j]) * (float) sumi + mm * r.s8[j];
+        }
+    }
+    return acc;
+}
+
+// ---- the legacy 4/5-bit types on the same ring (ggml_vec_dot_q4_0_q8_0 ggml-quants.c:3921, _q4_1_q8_1 :4502, _q5_0_q8_0 :4789) ----
+// Element j < 16 of a block is the low nibble of qs[j], element j + 16 the high nibble; the integer block sum is exact, the fp32 scale
+// product and the running sum are formed in the CPU's order.  Columns (144 / 160 / 176 B) start 8-byte aligned in the stage, so the
+// phase of every block inside a column is a compile-time constant: 64-bit loads, one PRMT per word where a field straddles two words.
+// Q4_0: 18-byte blocks [d f16][16 x 2 nibbles], value d * (q - 8): sum (q - 8) a = sum q a - 8 sum a, sum a precomputed per block (as8).
+__device__ __forceinline__ float dot_q4_0x8(const uint8_t * col, const ActRegs & r) {
+    const uint2 * c2 = reinterpret_cast<const uint2 *>(col);
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        if (j < r.nb) {
+            const int wj = (18 * j) >> 2;            // word holding d: even blocks start on it, odd ones 2 bytes into it
+            const bool odd = (j & 1) != 0;
+            uint32_t w[6];
+#pragma unroll
+            for (int i = 0; i < 3; i++) { const uint2 t = c2[(wj >> 1) + i]; w[2 * i] = t.x; w[2 * i + 1] = t.y; }
+            const int o = wj & 1;
+            const float d = __half2float(__ushort_as_half((unsigned short) (odd ? (w[o] >> 16) : (w[o] & 0xffffu))));
+            int sumi = 0;
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const uint32_t q = odd ? w[o + 1 + i] : __byte_perm(w[o + i], w[o + i + 1], 0x5432);
+                sumi = dp4a_us(q & 0x0f0f0f0fu, r.a[8 * j + i], sumi);
+                sumi = dp4a_us((q >> 4) & 0x0f0f0f0fu, r.a[8 * j + 4 + i], sumi);
+            }
+            sumi -= 8 * r.as8[j];
+            acc += (float) sumi * d * r.d8[j];
+        }
+    }
+    return acc;
+}
+// Q4_1: 20-byte blocks [d f16][m f16][16 x 2 nibbles] (word-aligned), value d * q + m; the offset rides on the q8_1 s = d_a * sum a
+__device__ __forceinline__ float dot_q4_1x8(const uint8_t * col, const ActRegs & r) {
+    const uint2 * c2 = reinterpret_cast<const uint2 *>(col);
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        if (j < r.nb) {
+            const int o = j & 1;                     // block j = words 5j .. 5j + 4
+            uint32_t w[6];
+#pragma unroll
+            for (int i = 0; i < 3; i++) { const uint2 t = c2[((5 * j) >> 1) + i]; w[2 * i] = t.x; w[2 * i + 1] = t.y; }
+            const float d = __half2float(__ushort_as_half((unsigned short) (w[o] & 0xffffu)));
+            const float mm = __half2float(__ushort_as_half((unsigned short) (w[o] >> 16)));
+            int sumi = 0;
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const uint32_t q = w[o + 1 + i];
+                sumi = dp4a_us(q & 0x0f0f0f0fu, r.a[8 * j + i], sumi);
+                sumi = dp4a_us((q >> 4) & 0x0f0f0f0fu, r.a[8 * j + 4 + i], sumi);
+            }
+            acc += (d * r.d8[j]) * (float) sumi + mm * r.s8[j];
+        }
+    }
+    return acc;
+}
+// Q5_0: 22-byte blocks [d f16][qh u32][16 x 2 nibbles], value d * ((q | h << 4) - 16).  sum (q + 16 h - 16) a = sum q a - 16 sum (1 - h) a:
+// the inverted fifth bits get their own dp4a, as Q5_1's do, so the -16 offset costs nothing
+__device__ __forceinline__ float dot_q5_0x8(const uint8_t * col, const ActRegs & r) {
+    const uint2 * c2 = reinterpret_cast<const uint2 *>(col);
+    float acc = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        if (j < r.nb) {
+            const int wj = (22 * j) >> 2;            // word holding d: even blocks start on it, odd ones 2 bytes into it
+            const bool odd = (j & 1) != 0;
+            uint32_t w[8];
+#pragma unroll
+            for (int i = 0; i < 4; i++) { const uint2 t = c2[(wj >> 1) + i]; w[2 * i] = t.x; w[2 * i + 1] = t.y; }
+            const int o = wj & 1;
+            const float d = __half2float(__ushort_as_half((unsigned short) (odd ? (w[o] >> 16) : (w[o] & 0xffffu))));
+            const uint32_t qn = ~(odd ? w[o + 1] : __byte_perm(w[o], w[o + 1], 0x5432));
+            int sumi = 0, sumb = 0;
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const uint32_t q = odd ? w[o + 2 + i] : __byte_perm(w[o + 1 + i], w[o + 2 + i], 0x5432);
+                const uint32_t hb_lo = (((qn >> (4 * i)) & 0xFu) * 0x00204081u) & 0x01010101u;
+                const uint32_t hb_hi = (((qn >> (4 * i + 16)) & 0xFu) * 0x00204081u) & 0x01010101u;
+                sumi = dp4a_us(q & 0x0f0f0f0fu, r.a[8 * j + i], sumi);
+                sumb = dp4a_us(hb_lo, r.a[8 * j + i], sumb);
+                sumi = dp4a_us((q >> 4) & 0x0f0f0f0fu, r.a[8 * j + 4 + i], sumi);
+                sumb = dp4a_us(hb_hi, r.a[8 * j + 4 + i], sumb);
+            }
+            sumi -= 16 * sumb;
+            acc += (d * r.d8[j]) * (float) sumi;
         }
     }
     return acc;

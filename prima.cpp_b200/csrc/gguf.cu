@@ -118,7 +118,7 @@ double read_num(Reader & r, uint32_t t) {
 }
 
 int64_t type_nbytes(int type, const int64_t ne[4]) {
-    if (type != pb::T_F32 && type != pb::T_F16 && !pb::is_kquant(type) && type != pb::T_Q8_0 && type != pb::T_Q5_1) return -1;
+    if (type != pb::T_F32 && type != pb::T_F16 && !pb::is_quant_type(type)) return -1;
     const int be = pb::block_elems(type);
     if (ne[0] % be != 0) return -1;
     return row_bytes(type, ne[0]) * ne[1] * ne[2] * ne[3];

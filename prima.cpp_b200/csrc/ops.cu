@@ -909,6 +909,20 @@ __device__ float dequant_elem(int type, const uint8_t * row, int e) {
             const int q = j < 16 ? ((b[8 + j] & 0xF) | (((qh >> j) & 1) << 4)) : ((b[8 + j - 16] >> 4) | (((qh >> j) & 1) << 4));
             return __fadd_rn(__fmul_rn((float) q, d), m);
         }
+        case T_Q4_0:
+        case T_Q4_1:
+        case T_Q5_0: {   // dequantize_row_q4_0 / _q4_1 / _q5_0, ggml-quants.c:1522-1580
+            const int bb = type == T_Q4_0 ? BYTES_Q4_0 : type == T_Q4_1 ? BYTES_Q4_1 : BYTES_Q5_0;
+            const uint8_t * b = row + (int64_t) (e / 32) * bb;
+            const float d = __half2float(__ushort_as_half((uint16_t) (b[0] | (b[1] << 8))));
+            const int j = e & 31;
+            const uint8_t * qs = b + (type == T_Q4_0 ? 2 : type == T_Q4_1 ? 4 : 6);
+            int q = j < 16 ? (qs[j] & 0xF) : (qs[j - 16] >> 4);
+            if (type == T_Q4_1) return __fadd_rn(__fmul_rn((float) q, d), __half2float(__ushort_as_half((uint16_t) (b[2] | (b[3] << 8)))));
+            if (type == T_Q5_0) q = (q | (((b[2 + j / 8] >> (j & 7)) & 1) << 4)) - 16;
+            else q -= 8;
+            return __fmul_rn((float) q, d);
+        }
         case T_Q4_K:
         case T_Q5_K: {
             const bool q5 = type == T_Q5_K;

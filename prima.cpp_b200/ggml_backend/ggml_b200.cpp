@@ -145,7 +145,8 @@ static bool grow_buf(b200_backend_ctx * ctx, dev_buf & b, size_t need) {
 
 static const int64_t MMQ_MIN_COLS = 8;
 static bool type_is_quant(enum ggml_type t) {
-    return t == GGML_TYPE_Q4_K || t == GGML_TYPE_Q5_K || t == GGML_TYPE_Q6_K || t == GGML_TYPE_Q8_0 || t == GGML_TYPE_Q5_1;
+    return t == GGML_TYPE_Q4_K || t == GGML_TYPE_Q5_K || t == GGML_TYPE_Q6_K || t == GGML_TYPE_Q8_0 || t == GGML_TYPE_Q5_1 || t == GGML_TYPE_Q4_0 ||
+           t == GGML_TYPE_Q4_1 || t == GGML_TYPE_Q5_0;
 }
 
 // ---------------------------------------------------------------------------------------------------- buffer

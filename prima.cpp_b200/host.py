@@ -8,7 +8,7 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 ROOT = PKG.parent
 
-TYPES = {"f32": 0, "f16": 1, "q5_1": 7, "q8_0": 8, "q4_K": 12, "q5_K": 13, "q6_K": 14}
+TYPES = {"f32": 0, "f16": 1, "q4_0": 2, "q4_1": 3, "q5_0": 6, "q5_1": 7, "q8_0": 8, "q4_K": 12, "q5_K": 13, "q6_K": 14}
 
 
 def lib_path() -> Path:
