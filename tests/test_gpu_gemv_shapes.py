@@ -19,12 +19,14 @@ import numpy as np
 import pytest
 import torch
 
+import legacy_types as L
 import oracle_lib as O
 from gpu_util import act_ws, act_ws_fields, dev_f32, ptr, sync
 from test_gpu_fallbacks import GemvMat
 
 KQ = [O.Q4_K, O.Q5_K, O.Q6_K]
-TN = O.TYPE_NAME
+BLK32 = [O.Q8_0, O.Q5_1, L.Q4_0, L.Q4_1, L.Q5_0]   # the 32-element block types (common.cuh is_blk32_type)
+TN = O.TYPE_NAME | L.NAME
 ENOTSUP = -3
 U_ROWS = 2048              # unique rows per matrix
 SWEEP_BYTES = 192 << 20    # weight bytes per sweep case: >= 3 turns of every CTA's ring whatever depth the plan picks
@@ -37,7 +39,7 @@ Plan = namedtuple("Plan", "wpr rpw rows nstage nstage_init owner_only ntiles")
 
 def gemv_plan(types, Ns, K):
     """The ring geometry launch_gemv gives a group, or None where the group does not fit the ring kernel."""
-    b32 = len(types) == 1 and types[0] in (O.Q8_0, O.Q5_1)
+    b32 = len(types) == 1 and types[0] in BLK32
     nblk = (K + 255) // 256
     if not (K % (32 if b32 else 256) == 0 and nblk <= ACT_MAX_NBLK):
         return None
@@ -51,8 +53,8 @@ def gemv_plan(types, Ns, K):
     rpw = 1 if wpr > 1 else 32 // nbp
     rows, biggest = [], 0
     for t, N in zip(types, Ns):
-        rb = O.row_size(t, K)
-        if not (t in KQ or b32) or (b32 and rb % 8):
+        rb = L.row_size(t, K)
+        if not (t in KQ or b32) or (b32 and rb % 8):           # the column dots read 64-bit words
             return None
         R = max(rpw, max(1, STAGE_TARGET // rb) // rpw * rpw)
         if wpr > 1:
@@ -92,7 +94,7 @@ def ring_turns(p, sms):
 
 # ---- sweep cases: (weight types of the group, K, rows of each matrix) ----
 def _n_for(t, K, n_min=1):
-    return max(n_min, -(-SWEEP_BYTES // O.row_size(t, K)))
+    return max(n_min, -(-SWEEP_BYTES // L.row_size(t, K)))
 
 
 SWEEP_K = [768, 1280, 1536, 3072, 3584, 4096, 5120, 8192, 8448, 8960, 13824, 14336, 16384, 16640, 18944, 27648, 28672, 29696]
@@ -101,6 +103,9 @@ SWEEP += [((t,), K, (_n_for(t, K, n),)) for t in (O.Q8_0, O.Q5_1) for n, K in ((
 SWEEP += [((O.Q5_1,), 7392, (_n_for(O.Q5_1, 7392, 8192),))]
 # q|k|v-like groups at K 8192: mixed types (the TYPE = 0 instantiation, unequal R), one type with R 5 and a 1-row last tile (owner_only off)
 SWEEP += [((O.Q4_K, O.Q4_K, O.Q6_K), 8192, (24576, 8192, 8192)), ((O.Q5_K, O.Q5_K, O.Q5_K), 8192, (24576, 4096, 4101))]
+# Q4_0 / Q4_1 / Q5_0 at Llama-3-8B's K, a Q4_1 K whose last 8-block column holds 2 blocks, and Qwen2.5-72B Q4_K_M's Q5_0 ffn_down
+SWEEP += [((t,), K, (_n_for(t, K),)) for t in L.LEGACY_TYPES for K in (4096, 8192, 14336)]
+SWEEP += [((L.Q4_1,), 4160, (_n_for(L.Q4_1, 4160),)), ((L.Q5_0,), 29568, (_n_for(L.Q5_0, 29568, 8192),))]
 
 
 def sweep_id(case):
@@ -121,6 +126,9 @@ FAMILIES = {
     ((O.Q4_K,), 18944): dict(wpr=4, rows=[2]),
     ((O.Q4_K, O.Q4_K, O.Q6_K), 8192): dict(owner_only=False),
     ((O.Q5_K, O.Q5_K, O.Q5_K), 8192): dict(owner_only=False),
+    ((L.Q4_0,), 4096): dict(wpr=1, rpw=2, rows=[12], nstage=4, owner_only=True),              # Llama-3-8B Q4_0 q, k, v, wo, gate, up
+    ((L.Q4_0,), 14336): dict(wpr=2, rows=[2], nstage=6, nstage_init=4, owner_only=True),       # Llama-3-8B Q4_0 ffn_down
+    ((L.Q5_0,), 29568): dict(wpr=4, rows=[1], nstage=4, nstage_init=2, owner_only=True),       # Qwen2.5-72B Q4_K_M ffn_down
 }
 
 
@@ -135,11 +143,24 @@ def test_sweep_cases_wrap_their_rings():
         case = next(c for c in SWEEP if c[0] == types and c[1] == K)
         p = gemv_plan(types, case[2], K)._asdict()
         assert {k: p[k] for k in want} == want, (sweep_id(case), p)
-    # Q8_0 rows at K 7392 are not 8-byte multiples: that shape leaves the ring
+    # rows that are not 8-byte multiples leave the ring: Q8_0 at K 7392, Q4_0 / Q5_0 at K 4160 (130 blocks of 18 / 22 bytes)
     assert gemv_plan((O.Q8_0,), (4096,), 7392) is None and gemv_plan((O.Q5_1,), (4096,), 7392) is not None
+    assert gemv_plan((L.Q4_0,), (4096,), 4160) is None and gemv_plan((L.Q5_0,), (4096,), 4160) is None
+    assert gemv_plan((L.Q4_1,), (4096,), 4160) is not None
+    # 32-element block types take the ring one matrix at a time
+    assert gemv_plan((L.Q4_0, L.Q4_0), (4096, 1024), 4096) is None and gemv_plan((O.Q4_K, O.Q4_K), (4096, 1024), 4096) is not None
 
 
 # ---- device helpers ----
+def oracle_mul_mat(port, t, W, N, K, x):
+    """The CPU's mat-vec for any weight type: the C port, or legacy_types' restatement for Q4_0 / Q4_1 / Q5_0."""
+    return L.mul_mat(port, t, W, N, K, x) if t in L.LEGACY_TYPES else port.mul_mat(t, W, N, K, x)
+
+
+def oracle_quantize_act(port, t, x):
+    return L.quantize_act(port, t, x) if t in L.LEGACY_TYPES else port.quantize_act(t, x)
+
+
 def _fused(lib):
     fn = lib.c.pb200_gemv_fused
     fn.argtypes = [C.c_int, C.POINTER(GemvMat), C.c_int64, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int,
@@ -155,8 +176,8 @@ class Scattered:
     def __init__(self, t, N, K, seed, with_add=False, U=U_ROWS):
         self.t, self.N, self.K = t, N, K
         self.U = U = min(U, N)
-        rb = O.row_size(t, K)
-        self.Wu = O.synth_blocks(t, U, K, seed=seed)
+        rb = L.row_size(t, K)
+        self.Wu = L.synth_blocks(t, U, K, seed=seed)
         self.src = (torch.randperm(N, generator=torch.Generator().manual_seed(seed)) % U).numpy()
         Wud = torch.from_numpy(self.Wu.reshape(U, rb)).cuda()
         self.W = torch.zeros(N * rb + 64, dtype=torch.uint8, device="cuda")
@@ -173,7 +194,7 @@ class Scattered:
 
     def check(self, port, x, what, add_rows=None):
         """y against the oracle's mat-vec of the source rows on activation x (+ the per-source add, or add_rows per row)."""
-        want_u = port.mul_mat(self.t, self.Wu, self.U, self.K, x)[0]
+        want_u = oracle_mul_mat(port, self.t, self.Wu, self.U, self.K, x)[0]
         if self.add_u is not None:
             want_u = want_u + self.add_u
         want = want_u[self.src]
@@ -240,17 +261,21 @@ def run_fused(lib, port, ms, K, prologue, eps=1e-5, seed=0, what=""):
         m.check(port, x, f"{what} matrix {i}")
 
 
-def run_blk32_down(lib, port, m, seed, what):
-    """Qwen2.5-72B's ffn_down on Q8_0 / Q5_1 (n_ff % 256 != 0): silu * mul, the q8_0 / q8_1 producer, the mat-vec with the residual."""
-    K = m.K
-    _, _, x = _prologue_input(lib, port, 2, K, 0.0, seed)
+def run_blk32(lib, port, ms, K, prologue, eps=1e-5, seed=0, what=""):
+    """32-element block type matrices, which pb200_gemv_fused does not take: the q8_0 / q8_1 producer of the prologue's f32 output, then
+    one mat-vec per matrix (+ its residual).  A 32-element ffn_down comes from n_ff % 256 != 0 (Qwen2.5-72B: Q5_0 / Q8_0 in Q4_K_M,
+    Q5_1 / Q8_0 in Q5_K_M); Q4_0 models have them everywhere but the head."""
+    _, _, x = _prologue_input(lib, port, prologue, K, eps, seed)
     xd = dev_f32(x)
     ws = act_ws(lib, K)
-    lib.check(lib.c.pb200_quantize_act(m.t, ptr(xd), K, ptr(ws), None), "quantize_act")
-    lib.check(lib.c.pb200_mul_mat_vec_q(m.t, ptr(m.W), m.N, K, ptr(ws), ptr(m.y), None, ptr(m.add), None), "mul_mat_vec_q")
-    _no_abort(lib, what)
-    assert np.array_equal(act_ws_fields(ws, K, "q8_0" if m.t == O.Q8_0 else "q8_1"), port.quantize_act(m.t, x)), f"{what}: act_ws differs"
-    m.check(port, x, what)
+    for i, m in enumerate(ms):
+        lib.check(lib.c.pb200_quantize_act(m.t, ptr(xd), K, ptr(ws), None), "quantize_act")
+        lib.check(lib.c.pb200_mul_mat_vec_q(m.t, ptr(m.W), m.N, K, ptr(ws), ptr(m.y), None, ptr(m.add) if m.add is not None else None, None),
+                  "mul_mat_vec_q")
+        _no_abort(lib, what)
+        mode = "q8_1" if m.t in (O.Q5_1, L.Q4_1) else "q8_0"
+        assert np.array_equal(act_ws_fields(ws, K, mode), oracle_quantize_act(port, m.t, x)), f"{what} matrix {i}: act_ws differs"
+        m.check(port, x, f"{what} matrix {i}")
 
 
 # ---- a. the launches of one decode step of each served model (engine.cu enqueue_step), at their real shapes ----
@@ -258,18 +283,29 @@ MODELS = {   # bench.py's hyper-parameters; default weight type of the mixture (
     "llama3-8b": dict(E=4096, QD=4096, EK=1024, F=14336, V=128256, t=O.Q4_K, eps=1e-5, qwen=False),
     "llama3-70b": dict(E=8192, QD=8192, EK=1024, F=28672, V=128256, t=O.Q4_K, eps=1e-5, qwen=False),
     "qwen2.5-72b": dict(E=8192, QD=8192, EK=1024, F=29568, V=152064, t=O.Q5_K, eps=1e-6, qwen=True),
+    "llama3-8b-q4_0": dict(E=4096, QD=4096, EK=1024, F=14336, V=128256, t=L.Q4_0, eps=1e-5, qwen=False),
+    "qwen2.5-72b-q4_K_M": dict(E=8192, QD=8192, EK=1024, F=29568, V=152064, t=O.Q4_K, eps=1e-6, qwen=True),
 }
 LAUNCHES = ["qkv-v_q5_K", "qkv-v_q6_K", "wo", "gate_up", "down-default", "down-q6_K", "head"]
+# the Q4_0 mixture: every matrix Q4_0 but the Q6_K head, and with an imatrix Q4_1 ffn_down layers
+Q4_0_LAUNCHES = ["qkv", "wo", "gate_up", "down-default", "down-q4_1", "head"]
+# Qwen2.5-72B Q4_K_M adds only its 32-element ffn_down (Q5_0, and Q8_0 in the use_more_bits layers) to the k-quant launches above
+MODEL_LAUNCH_LISTS = {"llama3-8b-q4_0": Q4_0_LAUNCHES, "qwen2.5-72b-q4_K_M": ["down-default", "down-q6_K"]}
+MODEL_LAUNCHES = [(m, la) for m in MODELS for la in MODEL_LAUNCH_LISTS.get(m, LAUNCHES)]
+ALL_LAUNCHES = LAUNCHES + ["qkv", "down-q4_1"]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("launch", LAUNCHES)
-@pytest.mark.parametrize("model", list(MODELS))
+@pytest.mark.parametrize("model,launch", MODEL_LAUNCHES, ids=[f"{m}-{la}" for m, la in MODEL_LAUNCHES])
 def test_model_launch_vs_oracle(cuda, lib, port, model, launch):
     h = MODELS[model]
-    E, t, eps, seed = h["E"], h["t"], h["eps"], 1000 * list(MODELS).index(model) + 10 * LAUNCHES.index(launch)
+    E, t, eps, seed = h["E"], h["t"], h["eps"], 1000 * list(MODELS).index(model) + 10 * ALL_LAUNCHES.index(launch)
     what = f"{model} {launch}"
-    if launch.startswith("qkv"):
+    if t == L.Q4_0 and launch != "head":
+        K, ms, pro = {"qkv": (E, [(t, h["QD"]), (t, h["EK"]), (t, h["EK"])], 1), "wo": (h["QD"], [(t, E)], 0), "gate_up": (E, [(t, h["F"])] * 2, 1),
+                      "down-default": (h["F"], [(t, E)], 2), "down-q4_1": (h["F"], [(L.Q4_1, E)], 2)}[launch]
+        run_blk32(lib, port, [Scattered(tt, n, K, seed + i, with_add=pro != 1) for i, (tt, n) in enumerate(ms)], K, pro, eps, seed, what)
+    elif launch.startswith("qkv"):
         tv = O.Q5_K if launch.endswith("q5_K") else O.Q6_K
         ms = [Scattered(tt, n, E, seed + i, with_add=h["qwen"]) for i, (tt, n) in enumerate(((t, h["QD"]), (t, h["EK"]), (tv, h["EK"])))]
         run_fused(lib, port, ms, E, 1, eps, seed, what)          # Qwen2's q / k / v biases ride in the epilogue
@@ -280,8 +316,8 @@ def test_model_launch_vs_oracle(cuda, lib, port, model, launch):
     elif launch.startswith("down"):
         td = O.Q6_K if launch.endswith("q6_K") else t
         if h["F"] % 256:
-            td = {O.Q5_K: O.Q5_1, O.Q6_K: O.Q8_0}[td]             # the mixture's fallback types for n_ff % 256 != 0
-            run_blk32_down(lib, port, Scattered(td, E, h["F"], seed, with_add=True), seed, f"{what} ({TN[td]})")
+            td = {O.Q4_K: L.Q5_0, O.Q5_K: O.Q5_1, O.Q6_K: O.Q8_0}[td]   # the mixture's fallback types for n_ff % 256 != 0
+            run_blk32(lib, port, [Scattered(td, E, h["F"], seed, with_add=True)], h["F"], 2, seed=seed, what=f"{what} ({TN[td]})")
         else:
             run_fused(lib, port, [Scattered(td, E, h["F"], seed, with_add=True)], h["F"], 2, eps, seed, what)
     else:

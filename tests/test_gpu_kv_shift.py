@@ -58,13 +58,16 @@ def _dev(ptr, shape, typestr):
     return torch.as_tensor(V(), device="cuda")
 
 
-def kv_tensors(eng, tm, n_seq, n_layer):
-    shape = (n_seq, n_layer, tm.hp["n_ctx"], tm.hp["n_head_kv"] * 128)
+def kv_tensors(eng, tm, n_seq, n_layer, hp=None):
+    """Views of the engine's f16 K / V caches as int16 [n_seq][n_layer][n_ctx][n_head_kv * 128]; hp: the shard's own hyper-parameters
+    when they differ from the model's (another n_ctx)."""
+    hp = hp or tm.hp
+    shape = (n_seq, n_layer, hp["n_ctx"], hp["n_head_kv"] * 128)
     return _dev(eng.kv_ptr(False), shape, "<i2"), _dev(eng.kv_ptr(True), shape, "<i2")
 
 
-def load(tm, pkg, n_seq=1, layers=None, with_embd=True, with_head=True):
-    eng = pkg.Model(pkg.HParams(**tm.hp), 0, layers, with_embd, with_head)
+def load(tm, pkg, n_seq=1, layers=None, with_embd=True, with_head=True, hp=None):
+    eng = pkg.Model(pkg.HParams(**(hp or tm.hp)), 0, layers, with_embd, with_head)
     for name, (t, a) in tm.tensors.items():
         eng.set_tensor(name, t, a)
     eng.set_n_seq(n_seq)
