@@ -140,8 +140,9 @@ PB200_API int pb200_flash_attn_ext(const float * q, const void * k_f16, const vo
  * top_k <= 0: the whole vocabulary; top_p 1: off; min_p 0: off; min_keep as in the reference; temp <= 0: greedy (first index of
  * the maximum, the same kernel as pb200_argmax_seq).  The draw is std::mt19937(seed) through std::discrete_distribution (two 32-bit
  * outputs per draw; nothing is drawn when one token survives), so a sequence of draws follows the reference's generator.  Equal
- * logits are ordered by ascending token id.  Penalties, logit bias, tail-free, typical, dynamic temperature, mirostat and grammars
- * are not part of this chain.  Invalid parameters (NaN / inf, top_p outside (0, 1], min_p outside [0, 1), min_keep < 0) return
+ * logits are ordered by ascending token id.  Logit bias and the repeat / frequency / presence penalties, the two samplers the
+ * reference puts in front of every chain, are pb200_penalty_apply below: a penalised copy of the row that this call then reads.
+ * Tail-free, typical, dynamic temperature, mirostat and grammars are not provided.  Invalid parameters (NaN / inf, top_p outside (0, 1], min_p outside [0, 1), min_keep < 0) return
  * PB200_EINVAL.  Where every softmax weight vanishes (a temperature so small that logit / temp overflows, a row of -inf) the token
  * is the top one.  Top-p is cut where the exact running mass reaches p; the reference's float running sum over a whole vocabulary
  * (top_k <= 0) can stop a little earlier (up to about 5e-4 of mass measured, a few dozen tokens of 130 000). */
@@ -159,6 +160,40 @@ PB200_API int pb200_sampler_seed(void * state_dev, uint32_t seed, void * stream)
  * capturable in a CUDA graph.  p->seed is not used here (pb200_sampler_seed seeds).  PB200_ENOTSUP when n_vocab / 16 logits exceed
  * the device's shared memory per block (n_vocab above about 880 000 on an H100). */
 PB200_API int pb200_sample(const float * logits, int n_vocab, const pb200_sampling * p, void * state_dev, int32_t * token_dev, void * stream);
+
+/* ---- logit bias and repeat / frequency / presence penalties: llama_sampler_init_logit_bias (src/llama-sampling.cpp:1568-1645) and
+ * llama_sampler_init_penalties (:1373-1566), which gpt_sampler_init puts ahead of every chain, greedy included (common/sampling.cpp:156-172).
+ * pb200_penalty_apply writes a penalised COPY of the row, in the reference's order:
+ *   1. logit[token] += bias for each list entry in list order (one rounded f32 add each; ids outside [0, n_vocab) are ignored);
+ *   2. ignore_eos with eos_token >= 0: logit[eos] = -inf;
+ *   3. stop here when last_n == 0 or repeat == 1 && freq == 0 && present == 0;
+ *   4. for every id occurring count > 0 times among the last min(last_n, accepted) accepted tokens (ids outside [0, n_vocab) ignored):
+ *      logit = logit <= 0 ? logit * repeat : logit / repeat, then logit -= count * freq + present, each operation rounded separately;
+ *      with !penalize_nl the newline keeps the logit it had after step 2.
+ * last_n < 0 behaves as 0 (llama_sampler_init_penalties clamps it; it is not "context size").  eos_token / nl_token -1: the vocabulary
+ * has none (ignore_eos off / penalize_nl on).  Then pb200_sample (or, greedy, its temp <= 0 form) on the copy, then
+ * pb200_penalty_accept of the token: that is gpt_sampler_sample + gpt_sampler_accept. */
+typedef struct pb200_logit_bias { int32_t token; float bias; } pb200_logit_bias;          /* llama_logit_bias */
+typedef struct pb200_penalties {
+    int32_t last_n;                     /* penalty_last_n; < 0 behaves as 0, like the reference */
+    float   repeat, freq, present;      /* 1 / 0 / 0: off */
+    int32_t penalize_nl, ignore_eos;
+    int32_t nl_token, eos_token;        /* -1: the vocabulary has none */
+    int32_t n_logit_bias;
+    const pb200_logit_bias * logit_bias;   /* host array, copied by the call */
+} pb200_penalties;
+/* device bytes of one penalty state: configuration, bias list, a history ring of last_n tokens and its count */
+PB200_API size_t pb200_penalty_state_bytes(int n_vocab, int last_n, int n_logit_bias);
+/* a fresh penalties sampler in state_dev (pb200_penalty_state_bytes(n_vocab, p->last_n, p->n_logit_bias) bytes): configuration and bias
+ * list uploaded, history cleared.  The list travels in the launches' arguments (one launch per 256 entries, at least one), so p may be
+ * freed when the call returns.  PB200_EINVAL: repeat not finite or <= 0, freq / present not finite, a NaN bias, n_logit_bias < 0, or
+ * a NULL list with n_logit_bias > 0. */
+PB200_API int pb200_penalty_init(void * state_dev, int n_vocab, const pb200_penalties * p, void * stream);
+/* llama_sampler_accept for n tokens in device memory: only the last last_n of them are kept.  One launch. */
+PB200_API int pb200_penalty_accept(void * state_dev, const int32_t * tokens_dev, int n, void * stream);
+/* steps 1-4 above: out[n_vocab] = the penalised copy of logits[n_vocab]; out must not alias logits.  One launch. */
+PB200_API int pb200_penalty_apply(const float * logits, int n_vocab, const void * state_dev, float * out, void * stream);
+/* All three only enqueue on stream: no host synchronisation, no allocation, capturable in a CUDA graph. */
 
 /* ---- fused decode launches (what the engine is made of), for graph-level fusion in a host such as the ggml-backend plugin ---- */
 typedef struct pb200_gemv_mat {
@@ -298,6 +333,16 @@ PB200_API int pb200_argmax_seq(pb200_model * m, int seq, int feed_back);
  * parameters -> pb200_sample_device(m, seq), and with feed_back the slot's token.  PB200_ESTATE for a slot without parameters. */
 PB200_API int pb200_sampling_set_seq(pb200_model * m, int seq, const pb200_sampling * p);
 PB200_API int pb200_sample_seq(pb200_model * m, int seq, int feed_back);
+/* logit bias and penalties per slot (pb200_penalty_apply's semantics): pb200_penalties_set_seq configures slot seq and clears its
+ * history (NULL removes them); it allocates the slot's state on first use, so call it outside any capture.  It does not touch the
+ * sampling parameters or the generator.  With penalties set, pb200_sample_seq is apply -> the slot's chain on the penalised row (greedy
+ * for temp <= 0) -> accept of the token: three launches, the last left out when last_n is 0.  pb200_logits_device keeps the raw
+ * logits.  pb200_argmax_seq stays a plain argmax: greedy with penalties is pb200_sample_seq with temp <= 0.  pb200_sampler_accept_seq
+ * accepts n host tokens into the slot's history (the prompt, as llama-cli accepts it); PB200_ESTATE for a slot without penalties.
+ * pb200_kv_clear and pb200_kv_seq_shift leave the history alone, as the reference's sampler is independent of the KV cache.
+ * PB200_ESTATE on a shard without the head. */
+PB200_API int pb200_penalties_set_seq(pb200_model * m, int seq, const pb200_penalties * p);
+PB200_API int pb200_sampler_accept_seq(pb200_model * m, int seq, const int32_t * tokens_host, int n);
 PB200_API int32_t * pb200_token_device(pb200_model * m, int seq);    /* int32[2]: {token, position} of the slot */
 PB200_API int32_t * pb200_sample_device(pb200_model * m, int seq);   /* int32: the slot's last sample (pb200_argmax_seq or pb200_sample_seq) */
 PB200_API float * pb200_logits_device(pb200_model * m);      /* [n_vocab] f32 */

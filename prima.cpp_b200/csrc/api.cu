@@ -286,4 +286,26 @@ int pb200_sample(const float * logits, int n_vocab, const pb200_sampling * p, vo
     return rc;
 }
 
+size_t pb200_penalty_state_bytes(int n_vocab, int last_n, int n_logit_bias) { (void) n_vocab; return penalty_state_bytes(last_n, n_logit_bias); }
+int pb200_penalty_init(void * state_dev, int n_vocab, const pb200_penalties * p, void * stream) {
+    if (!state_dev || n_vocab <= 0 || !penalties_ok(p)) return PB200_EINVAL;
+    uint64_t nl = 0;
+    const int rc = launch_penalty_init(state_dev, n_vocab, *p, (cudaStream_t) stream, nl);
+    g_launches += nl;
+    return rc;
+}
+int pb200_penalty_accept(void * state_dev, const int32_t * tokens_dev, int n, void * stream) {
+    if (!state_dev || n < 0 || (n > 0 && !tokens_dev)) return PB200_EINVAL;
+    if (n == 0) return 0;
+    const int rc = launch_penalty_accept(state_dev, tokens_dev, n, (cudaStream_t) stream, false);
+    if (rc == 0) g_launches++;
+    return rc;
+}
+int pb200_penalty_apply(const float * logits, int n_vocab, const void * state_dev, float * out, void * stream) {
+    if (!logits || n_vocab <= 0 || !state_dev || !out || out == logits) return PB200_EINVAL;
+    const int rc = launch_penalize(logits, n_vocab, state_dev, out, (cudaStream_t) stream, false);
+    if (rc == 0) g_launches++;
+    return rc;
+}
+
 }  // extern "C"

@@ -88,6 +88,16 @@ struct pb200_model {
     uint8_t * sampler_state = nullptr;  // [n_seq] mt19937 states of pb200_sample_seq, sampler_state_bytes() apart
     std::vector<pb200_sampling> sampling;   // per slot, valid where sampling_set
     std::vector<char> sampling_set;
+    struct Penalty {                    // logit bias + penalties of one slot (pb200_penalties_set_seq)
+        void * state = nullptr;         // penalty_state_bytes(last_n, n_bias) device bytes, grown on demand
+        size_t bytes = 0;
+        int32_t last_n = 0;             // clamped to >= 0
+        bool set = false;
+    };
+    std::vector<Penalty> pen;
+    float * pen_logits = nullptr;       // [n_vocab] the penalised row the chain reads (one for all slots: they share the stream)
+    int32_t * pen_tok = nullptr;        // staging of pb200_sampler_accept_seq
+    size_t pen_tok_n = 0;
     uint64_t launches_per_step = 0;
     int64_t weight_bytes = 0;
     std::vector<void *> allocs;
@@ -239,6 +249,9 @@ void pb200_model_free(pb200_model * m) {
     for (cudaGraphExec_t ge : m->graph_exec) if (ge) cudaGraphExecDestroy(ge);
     for (void * p : m->allocs) cudaFree(p);
     for (void * p : m->pf.allocs) cudaFree(p);
+    for (auto & p : m->pen) if (p.state) cudaFree(p.state);
+    if (m->pen_logits) cudaFree(m->pen_logits);
+    if (m->pen_tok) cudaFree(m->pen_tok);
     if (m->tokpos_host) cudaFreeHost(m->tokpos_host);
     if (m->logits_host) cudaFreeHost(m->logits_host);
     cudaStreamDestroy(m->stream);
@@ -499,6 +512,7 @@ int pb200_model_finalize(pb200_model * m) {
     if (m->with_head) CK(m->alloc((void **) &m->sampler_state, sampler_state_bytes() * (size_t) m->n_seq));
     m->sampling.assign((size_t) m->n_seq, pb200_sampling{});
     m->sampling_set.assign((size_t) m->n_seq, 0);
+    m->pen.assign((size_t) m->n_seq, pb200_model::Penalty{});
     CK(cudaMallocHost((void **) &m->tokpos_host, 16));
     if (m->with_head) CK(cudaMallocHost((void **) &m->logits_host, (size_t) hp.n_vocab * 4));
     rope_params_init(m->rp, hp.head_dim, hp.rope_mode, hp.n_ctx_orig, hp.rope_freq_base, hp.rope_freq_scale, 0.0f, 1.0f, 32.0f, 1.0f);
@@ -866,9 +880,66 @@ int pb200_sample_seq(pb200_model * m, int seq, int feed_back) {
     if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
     if (!m->sampling_set[seq]) return PB200_ESTATE;
     cudaSetDevice(m->device);
+    const pb200_model::Penalty & pen = m->pen[seq];
+    const int n = (int) m->hp.n_vocab;
+    const float * row = m->logits;
+    if (pen.set) {                      // logit bias + penalties on a copy of the row, then the unchanged chain on that copy
+        CK(launch_penalize(m->logits, n, pen.state, m->pen_logits, m->stream, true));
+        g_launches++;
+        row = m->pen_logits;
+    }
+    CK(launch_sample(row, n, m->sampling[seq], m->sampler_state + sampler_state_bytes() * (size_t) seq, m->sample_dev + seq,
+                     feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr, m->stream, true));
     g_launches++;
-    return launch_sample((const float *) m->logits, (int) m->hp.n_vocab, m->sampling[seq], m->sampler_state + sampler_state_bytes() * (size_t) seq,
-                         m->sample_dev + seq, feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr, m->stream, true);
+    if (pen.set && pen.last_n > 0) {    // gpt_sampler_accept: the token joins the slot's history
+        CK(launch_penalty_accept(pen.state, m->sample_dev + seq, 1, m->stream, true));
+        g_launches++;
+    }
+    return 0;
+}
+// logit bias + penalties of the slot: state allocated (or grown) here, configuration uploaded and history cleared on the model stream
+int pb200_penalties_set_seq(pb200_model * m, int seq, const pb200_penalties * p) {
+    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
+    if (seq < 0 || seq >= m->n_seq || (p && !penalties_ok(p))) return PB200_EINVAL;
+    pb200_model::Penalty & pen = m->pen[seq];
+    if (!p) { pen.set = false; return 0; }
+    cudaSetDevice(m->device);
+    if (!m->pen_logits) CK(cudaMalloc((void **) &m->pen_logits, (size_t) m->hp.n_vocab * 4));
+    const size_t bytes = penalty_state_bytes(p->last_n, p->n_logit_bias);
+    if (bytes > pen.bytes) {
+        if (pen.state) { CK(cudaStreamSynchronize(m->stream)); CK(cudaFree(pen.state)); pen.state = nullptr; pen.bytes = 0; pen.set = false; }
+        CK(cudaMalloc(&pen.state, bytes));
+        pen.bytes = bytes;
+    }
+    uint64_t nl = 0;
+    const int rc = launch_penalty_init(pen.state, (int) m->hp.n_vocab, *p, m->stream, nl);
+    g_launches += nl;
+    if (rc) return rc;
+    pen.last_n = std::max(p->last_n, 0);
+    pen.set = true;
+    return 0;
+}
+// llama-cli accepts the prompt into the sampler (examples/main/main.cpp:720): the last last_n host tokens go to the slot's history
+int pb200_sampler_accept_seq(pb200_model * m, int seq, const int32_t * tokens_host, int n) {
+    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
+    if (seq < 0 || seq >= m->n_seq || n < 0 || (n > 0 && !tokens_host)) return PB200_EINVAL;
+    const pb200_model::Penalty & pen = m->pen[seq];
+    if (!pen.set) return PB200_ESTATE;
+    const int k = std::min(n, pen.last_n);
+    if (k == 0) return 0;
+    cudaSetDevice(m->device);
+    if ((size_t) k > m->pen_tok_n) {
+        CK(cudaStreamSynchronize(m->stream));
+        if (m->pen_tok) { CK(cudaFree(m->pen_tok)); m->pen_tok = nullptr; m->pen_tok_n = 0; }
+        CK(cudaMalloc((void **) &m->pen_tok, (size_t) k * 4));
+        m->pen_tok_n = (size_t) k;
+    }
+    // from pageable memory the copy returns once the tokens are staged, so the caller may reuse its array; stream order keeps the
+    // staging buffer until the accept has read it
+    CK(cudaMemcpyAsync(m->pen_tok, tokens_host + (n - k), (size_t) k * 4, cudaMemcpyHostToDevice, m->stream));
+    CK(launch_penalty_accept(pen.state, m->pen_tok, k, m->stream, false));
+    g_launches++;
+    return 0;
 }
 int32_t * pb200_token_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->tokpos_dev + 4 * seq : nullptr; }
 int32_t * pb200_sample_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->sample_dev + seq : nullptr; }

@@ -196,6 +196,15 @@ size_t sampler_state_bytes();
 bool sampling_params_ok(const pb200_sampling * p);   // finite, top_p in (0, 1], min_p in [0, 1), min_keep >= 0
 int launch_sampler_seed(void * state, uint32_t seed, cudaStream_t stream);
 int launch_sample(const float * x, int n, const pb200_sampling & p, void * state, int32_t * out, int32_t * out2, cudaStream_t stream, bool pdl);
+// logit bias + penalties (sample.cu): state = header, bias list, history ring of penalty_state_bytes(last_n, n_bias) device bytes.
+// launch_penalty_init enqueues max(1, ceil(n_bias / 256)) launches (the list travels in their arguments) and adds them to nlaunch;
+// launch_penalize writes the penalised copy of x[n] into out (k_penalize, one launch); launch_penalty_accept pushes tokens[n] (device)
+// into the history (one launch; nothing happens on the device when last_n is 0).
+size_t penalty_state_bytes(int last_n, int n_bias);
+bool penalties_ok(const pb200_penalties * p);   // repeat finite and > 0, freq / present finite, no NaN bias, a list where n_logit_bias > 0
+int launch_penalty_init(void * state, int n_vocab, const pb200_penalties & p, cudaStream_t stream, uint64_t & nlaunch);
+int launch_penalize(const float * x, int n, const void * state, float * out, cudaStream_t stream, bool pdl);
+int launch_penalty_accept(void * state, const int32_t * tokens, int n, cudaStream_t stream, bool pdl);
 
 // element-wise helpers for the plugin
 int launch_binary(int op /*0 add, 1 mul*/, const float * a, const float * b, float * y, int64_t n, int64_t nb /*b broadcast period*/, cudaStream_t stream);

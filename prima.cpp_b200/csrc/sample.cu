@@ -15,6 +15,7 @@
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 #include <cstdint>
 
@@ -331,7 +332,153 @@ __global__ void k_sampler_seed(MtState * st, uint32_t seed) {   // std::mt19937(
 
 FuncAttrCache sample_attr;
 
+// ---- logit bias and repeat / frequency / presence penalties (llama_sampler_init_logit_bias, :1568-1645, and
+// llama_sampler_init_penalties, :1373-1566): the two samplers gpt_sampler_init puts in front of every chain.  They write a penalised
+// copy of the logits row that the chain above (or k_argmax) then reads like any other row.
+// Device state: PenHdr, the bias list (n_bias entries), the history ring (last_n int32).
+struct PenHdr {
+    int32_t last_n;          // ring capacity, >= 0; 0: accept does nothing
+    int32_t n_bias;
+    int32_t eos;             // -1: no EOS step (ignore_eos off, or no EOS id in [0, n_vocab))
+    int32_t nl;              // -1: the newline is penalised like any other token
+    int32_t active;          // 0: the early exit (last_n 0, or repeat 1 / freq 0 / present 0): bias and EOS only
+    float repeat, freq, present;
+    int32_t count, pos;      // tokens in the ring (min(accepted, last_n)) and the next slot to write
+    int32_t pad_[6];
+};
+static_assert(sizeof(PenHdr) == 64, "PenHdr");
+constexpr int PEN_CHUNK = 256;        // bias entries per init launch, passed by value
+constexpr int PEN_SLICE = 4096;       // vocabulary ids per CTA of k_penalize
+constexpr int PEN_NT = 512;
+struct BiasChunk { pb200_logit_bias e[PEN_CHUNK]; };
+
+__device__ __forceinline__ const pb200_logit_bias * pen_bias(const PenHdr * h) { return (const pb200_logit_bias *) (h + 1); }
+__device__ __forceinline__ int32_t * pen_ring(const PenHdr * h, int n_bias) { return (int32_t *) ((const pb200_logit_bias *) (h + 1) + n_bias); }
+
+// a fresh penalties sampler: header (first chunk only; count = pos = 0 clears the history) and entries [off, off + cnt) of the bias list
+__global__ void k_penalty_init(PenHdr * st, PenHdr h, BiasChunk c, int off, int cnt) {
+    pb200_logit_bias * b = (pb200_logit_bias *) (st + 1);
+    for (int i = threadIdx.x; i < cnt; i += blockDim.x) b[off + i] = c.e[i];
+    if (off == 0 && threadIdx.x == 0) *st = h;
+}
+
+// out = the penalised copy of x[n].  CTA b owns ids [b * PEN_SLICE, ...): its slice of the row and a count per id in shared memory.
+__global__ void __launch_bounds__(PEN_NT) k_penalize(const float * __restrict__ x, int n, const PenHdr * __restrict__ st, float * __restrict__ out) {
+    __shared__ float s_row[PEN_SLICE];
+    __shared__ int s_cnt[PEN_SLICE];
+    __shared__ float s_bv[32];
+    pdl_trigger();
+    pdl_wait();
+    const PenHdr h = *st;
+    const int lo = blockIdx.x * PEN_SLICE, cnt = min(n - lo, PEN_SLICE);
+    for (int i = threadIdx.x; i < cnt; i += PEN_NT) { s_row[i] = x[lo + i]; s_cnt[i] = 0; }
+    __syncthreads();
+    // 1. bias, one rounded add per entry in list order: warp 0 takes 32 entries at a time; the lowest lane of each group of equal
+    //    ids in this slice adds the group's biases in lane (= list) order.  Ids outside [0, n) fall in no slice.
+    if (threadIdx.x < 32) {
+        const int lane = threadIdx.x;
+        const pb200_logit_bias * b = pen_bias(st);
+        for (int j0 = 0; j0 < h.n_bias; j0 += 32) {
+            int t = -1;
+            float v = 0.f;
+            if (j0 + lane < h.n_bias) { t = b[j0 + lane].token; v = b[j0 + lane].bias; }
+            const bool mine = t >= lo && t < lo + cnt;
+            const unsigned grp = __match_any_sync(~0u, mine ? t : -1);
+            s_bv[lane] = v;
+            __syncwarp();
+            if (mine && __ffs(grp) - 1 == lane) {
+                float acc = s_row[t - lo];
+                for (unsigned g = grp; g; g &= g - 1) acc = __fadd_rn(acc, s_bv[__ffs(g) - 1]);
+                s_row[t - lo] = acc;
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    // 2. ignore_eos
+    if (threadIdx.x == 0 && h.eos >= lo && h.eos < lo + cnt) s_row[h.eos - lo] = -INFINITY;
+    // 3. early exit: bias and EOS only
+    if (h.active) {
+        // 5. counts of the ids of this slice among the last min(last_n, accepted) tokens (the ring holds exactly those)
+        const int32_t * ring = pen_ring(st, h.n_bias);
+        for (int i = threadIdx.x; i < h.count; i += PEN_NT) {
+            const int t = ring[i];
+            if (t >= lo && t < lo + cnt) atomicAdd(&s_cnt[t - lo], 1);
+        }
+        __syncthreads();
+        // 4. + 6. the newline keeps the logit it had before this step: it is simply not penalised
+        for (int i = threadIdx.x; i < cnt; i += PEN_NT) {
+            const int c = s_cnt[i];
+            if (c > 0 && lo + i != h.nl) {
+                float l = s_row[i];
+                l = l <= 0.f ? __fmul_rn(l, h.repeat) : __fdiv_rn(l, h.repeat);
+                s_row[i] = __fsub_rn(l, __fadd_rn(__fmul_rn((float) c, h.freq), __fmul_rn(1.0f, h.present)));
+            }
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < cnt; i += PEN_NT) out[lo + i] = s_row[i];
+}
+
+// llama_sampler_accept for n tokens: only the last last_n reach the ring
+__global__ void k_penalty_accept(PenHdr * st, const int32_t * __restrict__ tok, int n) {
+    pdl_trigger();
+    pdl_wait();
+    const int L = st->last_n;
+    if (L <= 0) return;
+    int32_t * ring = pen_ring(st, st->n_bias);
+    const int m = min(n, L), pos = st->pos, count = st->count;
+    for (int i = threadIdx.x; i < m; i += blockDim.x) ring[(pos + i) % L] = tok[n - m + i];
+    __syncthreads();
+    if (threadIdx.x == 0) { st->pos = (pos + m) % L; st->count = min(count + m, L); }
+}
+
 }  // namespace
+
+size_t penalty_state_bytes(int last_n, int n_bias) {
+    return (sizeof(PenHdr) + (size_t) std::max(n_bias, 0) * sizeof(pb200_logit_bias) + (size_t) std::max(last_n, 0) * 4 + 255) / 256 * 256;
+}
+
+bool penalties_ok(const pb200_penalties * p) {
+    if (!p) return false;
+    if (!std::isfinite(p->repeat) || !(p->repeat > 0.f) || !std::isfinite(p->freq) || !std::isfinite(p->present)) return false;
+    if (p->n_logit_bias < 0 || (p->n_logit_bias > 0 && !p->logit_bias)) return false;
+    for (int i = 0; i < p->n_logit_bias; i++)
+        if (std::isnan(p->logit_bias[i].bias)) return false;
+    return true;
+}
+
+int launch_penalty_init(void * state, int n_vocab, const pb200_penalties & p, cudaStream_t stream, uint64_t & nlaunch) {
+    PenHdr h{};
+    h.last_n = std::max(p.last_n, 0);
+    h.n_bias = p.n_logit_bias;
+    h.eos = p.ignore_eos && p.eos_token >= 0 && p.eos_token < n_vocab ? p.eos_token : -1;
+    h.nl = !p.penalize_nl && p.nl_token >= 0 && p.nl_token < n_vocab ? p.nl_token : -1;
+    h.active = h.last_n != 0 && !(p.repeat == 1.f && p.freq == 0.f && p.present == 0.f);
+    h.repeat = p.repeat; h.freq = p.freq; h.present = p.present;
+    int off = 0;
+    do {
+        const int cnt = std::min(PEN_CHUNK, p.n_logit_bias - off);
+        BiasChunk c;
+        for (int i = 0; i < cnt; i++) c.e[i] = p.logit_bias[off + i];
+        k_penalty_init<<<1, PEN_CHUNK, 0, stream>>>((PenHdr *) state, h, c, off, cnt);
+        nlaunch++;
+        const cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return (int) e;
+        off += cnt;
+    } while (off < p.n_logit_bias);
+    return 0;
+}
+
+int launch_penalize(const float * x, int n, const void * state, float * out, cudaStream_t stream, bool pdl) {
+    LaunchCfg lc(dim3((n + PEN_SLICE - 1) / PEN_SLICE), dim3(PEN_NT), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_penalize, x, n, (const PenHdr *) state, out);
+}
+
+int launch_penalty_accept(void * state, const int32_t * tokens, int n, cudaStream_t stream, bool pdl) {
+    LaunchCfg lc(dim3(1), dim3(256), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_penalty_accept, (PenHdr *) state, tokens, n);
+}
 
 size_t sampler_state_bytes() { return (sizeof(MtState) + 255) / 256 * 256; }
 

@@ -45,6 +45,29 @@ def sampling(top_k: int = 40, top_p: float = 0.95, min_p: float = 0.05, temp: fl
     return Sampling(int(top_k), float(top_p), float(min_p), float(temp), int(min_keep), int(seed) & 0xFFFFFFFF)
 
 
+class LogitBias(C.Structure):
+    """pb200_logit_bias (llama_logit_bias)."""
+    _fields_ = [("token", C.c_int32), ("bias", C.c_float)]
+
+
+class Penalties(C.Structure):
+    """pb200_penalties: logit bias, ignore_eos and the repeat / frequency / presence penalties over the last last_n accepted tokens."""
+    _fields_ = [("last_n", C.c_int32), ("repeat", C.c_float), ("freq", C.c_float), ("present", C.c_float), ("penalize_nl", C.c_int32),
+                ("ignore_eos", C.c_int32), ("nl_token", C.c_int32), ("eos_token", C.c_int32), ("n_logit_bias", C.c_int32),
+                ("logit_bias", C.POINTER(LogitBias))]
+
+
+def penalties(last_n: int = 64, repeat: float = 1.0, freq: float = 0.0, present: float = 0.0, penalize_nl: bool = False,
+              ignore_eos: bool = False, nl_token: int = -1, eos_token: int = -1, logit_bias=()) -> Penalties:
+    """Defaults of llama-cli (common/common.h:118-126): last_n 64, every penalty off, the newline not penalised.  logit_bias: pairs
+    (token, bias).  The vocabulary's newline / EOS ids are the caller's to pass (-1: none).  The returned structure keeps its list alive."""
+    arr = (LogitBias * max(len(logit_bias), 1))(*[LogitBias(int(t), float(b)) for t, b in logit_bias])
+    p = Penalties(int(last_n), float(repeat), float(freq), float(present), int(bool(penalize_nl)), int(bool(ignore_eos)), int(nl_token),
+                  int(eos_token), len(logit_bias), C.cast(arr, C.POINTER(LogitBias)))
+    p._keep = arr
+    return p
+
+
 class Pb200Error(RuntimeError):
     pass
 
@@ -130,6 +153,13 @@ class Lib:
         c.pb200_sample.argtypes = [vp, C.c_int, C.POINTER(Sampling), vp, vp, vp]
         c.pb200_sampling_set_seq.argtypes = [vp, C.c_int, C.POINTER(Sampling)]
         c.pb200_sample_seq.argtypes = [vp, C.c_int, C.c_int]
+        c.pb200_penalty_state_bytes.restype = C.c_size_t
+        c.pb200_penalty_state_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        c.pb200_penalty_init.argtypes = [vp, C.c_int, C.POINTER(Penalties), vp]
+        c.pb200_penalty_accept.argtypes = [vp, vp, C.c_int, vp]
+        c.pb200_penalty_apply.argtypes = [vp, C.c_int, vp, vp, vp]
+        c.pb200_penalties_set_seq.argtypes = [vp, C.c_int, C.POINTER(Penalties)]
+        c.pb200_sampler_accept_seq.argtypes = [vp, C.c_int, vp, C.c_int]
 
     @classmethod
     def get(cls) -> "Lib":
@@ -152,6 +182,22 @@ class Lib:
         """pb200_sample: one token from n_vocab device logits into the int32 at token_ptr (enqueued on stream)."""
         self.check(self.c.pb200_sample(C.c_void_p(logits_ptr), n_vocab, C.byref(p), C.c_void_p(state_ptr), C.c_void_p(token_ptr), C.c_void_p(stream)),
                    "sample")
+
+    def penalty_state_bytes(self, n_vocab: int, p: Penalties) -> int:
+        return self.c.pb200_penalty_state_bytes(n_vocab, p.last_n, p.n_logit_bias)
+
+    def penalty_init(self, state_ptr: int, n_vocab: int, p: Penalties, stream: int = 0) -> None:
+        """A fresh penalties sampler in device memory of penalty_state_bytes(): configuration uploaded, history cleared."""
+        self.check(self.c.pb200_penalty_init(C.c_void_p(state_ptr), n_vocab, C.byref(p), C.c_void_p(stream)), "penalty_init")
+
+    def penalty_accept(self, state_ptr: int, tokens_ptr: int, n: int, stream: int = 0) -> None:
+        """llama_sampler_accept for n int32 device tokens at tokens_ptr."""
+        self.check(self.c.pb200_penalty_accept(C.c_void_p(state_ptr), C.c_void_p(tokens_ptr), n, C.c_void_p(stream)), "penalty_accept")
+
+    def penalty_apply(self, logits_ptr: int, n_vocab: int, state_ptr: int, out_ptr: int, stream: int = 0) -> None:
+        """out = the row with logit bias and penalties applied (a copy; out must not alias logits)."""
+        self.check(self.c.pb200_penalty_apply(C.c_void_p(logits_ptr), n_vocab, C.c_void_p(state_ptr), C.c_void_p(out_ptr), C.c_void_p(stream)),
+                   "penalty_apply")
 
 
 class Model:
@@ -297,6 +343,19 @@ class Model:
     def sample_seq(self, seq: int, feed_back: bool = False) -> None:
         """argmax_seq with the slot's sampling parameters: the token goes to sample_ptr(seq) (and with feed_back to the slot)."""
         self.lib.check(self.lib.c.pb200_sample_seq(self.h, seq, int(feed_back)), "sample_seq")
+
+    def set_penalties(self, seq: int, p: Penalties | None = None, **kw) -> None:
+        """Logit bias and penalties of slot seq (a Penalties, or penalties()'s keywords); clears its history.  None without keywords
+        removes them.  Sampling parameters and generator are left alone."""
+        if p is None and kw:
+            p = penalties(**kw)
+        self.lib.check(self.lib.c.pb200_penalties_set_seq(self.h, seq, C.byref(p) if p is not None else None), "penalties_set_seq")
+
+    def accept(self, seq: int, tokens) -> None:
+        """Host tokens into slot seq's penalty history (the prompt, as llama-cli accepts it)."""
+        import numpy as np
+        t = np.ascontiguousarray(tokens, dtype=np.int32)
+        self.lib.check(self.lib.c.pb200_sampler_accept_seq(self.h, seq, t.ctypes.data_as(C.c_void_p), int(t.size)), "sampler_accept_seq")
 
     def token_ptr(self, seq: int) -> int:
         return self.lib.c.pb200_token_device(self.h, seq)
