@@ -60,7 +60,52 @@ struct Layer {
 struct ActBuf {
     ActQ q{};
     void * base = nullptr;
-    int64_t K = 0;
+};
+
+// Device scratch that only grows.  grow() waits for the stream before it frees the old block, which kernels in flight may still read,
+// so it must not run during stream capture; the engine captures only in pb200_model_finalize, which grows nothing.
+struct DevBuf {
+    void * p = nullptr;
+    size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf &) = delete;
+    DevBuf & operator=(const DevBuf &) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
+    int grow(size_t need, cudaStream_t st) {
+        if (need <= bytes) return 0;
+        if (p) {
+            CK(cudaStreamSynchronize(st));
+            CK(cudaFree(p));
+            p = nullptr;
+            bytes = 0;
+        }
+        CK(cudaMalloc(&p, need));
+        bytes = need;
+        return 0;
+    }
+};
+
+struct Penalty {                    // logit bias + penalties of one slot (pb200_penalties_set_seq)
+    DevBuf state;                   // penalty_state_bytes(last_n, n_bias) device bytes
+    int32_t last_n = 0;             // clamped to >= 0
+    bool set = false;
+};
+
+// One sequence slot: an independent sequence with its own KV cache, token and position (the pipeline keeps one per stage in flight).
+// The device words point into the model's per-slot arrays, whose layouts hosts see: pb200_token_device, pb200_sample_device and
+// pb200_kv_device.
+struct Slot {
+    int32_t * tokpos = nullptr;         // {token, pos}, 16 bytes per slot
+    int32_t * sample = nullptr;         // the slot's last sample (pb200_argmax_seq / pb200_sample_seq)
+    uint8_t * rng = nullptr;            // mt19937 state of pb200_sample_seq (shards with the head)
+    __half *k = nullptr, *v = nullptr;  // the slot's [layer][n_ctx][n_head_kv * head_dim] block of the K and V caches
+    size_t layer_elems = 0;             // n_ctx * n_head_kv * head_dim
+    pb200_sampling sampling{};          // valid where sampling_set
+    bool sampling_set = false;
+    Penalty pen;
+    cudaGraphExec_t graph = nullptr;    // the captured step (NULL: direct launches)
+    __half * kc(int layer) const { return k + layer * layer_elems; }   // layer: index within this shard
+    __half * vc(int layer) const { return v + layer * layer_elems; }
 };
 
 }  // namespace
@@ -73,42 +118,29 @@ struct pb200_model {
     Tensor tok_embd, output;
     float *output_norm = nullptr, *rope_ff = nullptr;
     std::vector<Layer> layers;   // index il - l0
-    __half *kcache = nullptr, *vcache = nullptr;
+    __half *kcache = nullptr, *vcache = nullptr;   // [n_seq][layer][n_ctx][n_head_kv * head_dim] each
+    size_t kv_bytes = 0;                           // of each
     float *x_in = nullptr, *x_a = nullptr, *x_b = nullptr, *q = nullptr, *k = nullptr, *v = nullptr, *att = nullptr, *g = nullptr, *u = nullptr,
           *xn = nullptr, *x_out = nullptr, *logits = nullptr;
     ActBuf actE, actQD, actF;
     unsigned int * gbar = nullptr;     // grid-barrier state of the distributed GEMV prologues (2 words, self-resetting)
-    int32_t * tokpos_dev = nullptr;    // [0] token, [1] pos
     int32_t * tokpos_host = nullptr;   // pinned
     float * logits_host = nullptr;     // pinned
     RopeParams rp{};
-    int n_seq = 1;                      // independent sequences with their own KV cache / token / position (the pipeline keeps one per stage in flight)
-    std::vector<cudaGraphExec_t> graph_exec;   // one captured step per sequence slot
-    int32_t * sample_dev = nullptr;     // [n_seq] token of the slot's last sample (pb200_argmax_seq / pb200_sample_seq)
-    uint8_t * sampler_state = nullptr;  // [n_seq] mt19937 states of pb200_sample_seq, sampler_state_bytes() apart
-    std::vector<pb200_sampling> sampling;   // per slot, valid where sampling_set
-    std::vector<char> sampling_set;
-    struct Penalty {                    // logit bias + penalties of one slot (pb200_penalties_set_seq)
-        void * state = nullptr;         // penalty_state_bytes(last_n, n_bias) device bytes, grown on demand
-        size_t bytes = 0;
-        int32_t last_n = 0;             // clamped to >= 0
-        bool set = false;
-    };
-    std::vector<Penalty> pen;
-    float * pen_logits = nullptr;       // [n_vocab] the penalised row the chain reads (one for all slots: they share the stream)
-    int32_t * pen_tok = nullptr;        // staging of pb200_sampler_accept_seq
-    size_t pen_tok_n = 0;
+    int n_seq = 1;
+    std::vector<Slot> slots;           // [n_seq], from finalize on
+    DevBuf pen_logits;                 // [n_vocab] the penalised row the chain reads (one for all slots: they share the stream)
+    DevBuf pen_tok;                    // staging of pb200_sampler_accept_seq
     uint64_t launches_per_step = 0;
     int64_t weight_bytes = 0;
     std::vector<void *> allocs;
     bool profiling = false;
-    // prompt-processing (prefill) scratch, grown on demand
-    struct Prefill {
+    struct Prefill {                   // prompt-processing scratch for up to T tokens: one block, grown on demand
         int T = 0;
+        DevBuf mem;
         float *x0 = nullptr, *x1 = nullptr, *xn = nullptr, *q = nullptr, *k = nullptr, *v = nullptr, *att = nullptr, *g = nullptr, *u = nullptr;
         void * ws = nullptr;
         int32_t *tok = nullptr, *pos = nullptr;
-        std::vector<void *> allocs;
     } pf;
     std::vector<cudaEvent_t> prof_ev;
     std::vector<int64_t> prof_bytes;
@@ -122,6 +154,29 @@ struct pb200_model {
         return 0;
     }
 };
+
+// Argument checks of the entry points.  ready: a NULL or unfinalized model, or a shard without the head where the call needs the logits,
+// returns `unready` (PB200_ESTATE; the host copies pb200_get_hidden / pb200_set_hidden / pb200_debug_read answer PB200_EINVAL); ready_seq
+// then returns PB200_EINVAL for a seq outside [0, n_seq).  building: the calls that fill an unfinalized model.  Each makes the model's
+// device current when its checks pass.
+static int ready(pb200_model * m, bool head = false, int unready = PB200_ESTATE) {
+    if (!m || !m->finalized || (head && !m->with_head)) return unready;
+    cudaSetDevice(m->device);
+    return 0;
+}
+static int ready_seq(pb200_model * m, int seq, bool head = false) {
+    CK(ready(m, head));
+    return seq < 0 || seq >= m->n_seq ? PB200_EINVAL : 0;
+}
+static int building(pb200_model * m) {
+    if (!m) return PB200_EINVAL;
+    if (m->finalized) return PB200_ESTATE;
+    cudaSetDevice(m->device);
+    return 0;
+}
+static bool tokpos_ok(const pb200_model * m, int32_t token, int32_t pos) {
+    return pos >= 0 && pos < m->hp.n_ctx && token >= 0 && token < m->hp.n_vocab;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // synthetic raw blocks generated on the device (bench without a checkpoint): valid bit patterns, weight std ~ 1/sqrt(K)
@@ -190,36 +245,43 @@ static int fallback_type(int t, int64_t k) {   // src/llama.cpp:19516-19551
     return T_Q8_0;   // Q6_K
 }
 
-static Tensor * find_tensor(pb200_model * m, const std::string & name, bool & is_f32, float *** f32slot, int64_t & n_f32) {
-    is_f32 = false;
+// Where a GGUF tensor name goes on this shard.
+struct Found {
+    enum Kind { UNKNOWN, SKIPPED, QUANT, F32 } kind = UNKNOWN;   // SKIPPED: another stage's tensor, or a per-layer one the engine does not use
+    Tensor * t = nullptr;       // QUANT, with its N and K set
+    float ** f32 = nullptr;     // F32: where the vector's device address is kept
+    int64_t n = 0;              // F32: its length
+};
+static Found find_tensor(pb200_model * m, const std::string & name) {
     const pb200_hparams & hp = m->hp;
     const int64_t E = hp.n_embd, QD = (int64_t) hp.n_head * hp.head_dim, EK = (int64_t) hp.n_head_kv * hp.head_dim, F = hp.n_ff;
-    auto T = [&](Tensor & t, int64_t N, int64_t K) { t.N = N; t.K = K; return &t; };
-    if (name == "token_embd.weight") return m->with_embd ? T(m->tok_embd, hp.n_vocab, E) : nullptr;
-    if (name == "output.weight") return m->with_head ? T(m->output, hp.n_vocab, E) : nullptr;
-    if (name == "output_norm.weight") { is_f32 = true; *f32slot = m->with_head ? &m->output_norm : nullptr; n_f32 = E; return nullptr; }
-    if (name == "rope_freqs.weight") { is_f32 = true; *f32slot = &m->rope_ff; n_f32 = hp.head_dim / 2; return nullptr; }
+    auto quant = [](Tensor & t, int64_t N, int64_t K) { t.N = N; t.K = K; Found f; f.kind = Found::QUANT; f.t = &t; return f; };
+    auto f32 = [](float *& p, int64_t n) { Found f; f.kind = Found::F32; f.f32 = &p; f.n = n; return f; };
+    Found skipped;
+    skipped.kind = Found::SKIPPED;
+    if (name == "token_embd.weight") return m->with_embd ? quant(m->tok_embd, hp.n_vocab, E) : skipped;
+    if (name == "output.weight") return m->with_head ? quant(m->output, hp.n_vocab, E) : skipped;
+    if (name == "output_norm.weight") return m->with_head ? f32(m->output_norm, E) : skipped;
+    if (name == "rope_freqs.weight") return f32(m->rope_ff, hp.head_dim / 2);
+    if (name.rfind("blk.", 0) != 0) return Found{};
     int il = -1;
     char what[64] = {0};
-    if (sscanf(name.c_str(), "blk.%d.%63s", &il, what) != 2) return nullptr;
-    if (il < m->l0 || il >= m->l1) { is_f32 = true; *f32slot = nullptr; return nullptr; }
+    if (sscanf(name.c_str(), "blk.%d.%63s", &il, what) != 2 || il < m->l0 || il >= m->l1) return skipped;
     Layer & L = m->layers[il - m->l0];
     const std::string w(what);
-    if (w == "attn_q.weight") return T(L.wq, QD, E);
-    if (w == "attn_k.weight") return T(L.wk, EK, E);
-    if (w == "attn_v.weight") return T(L.wv, EK, E);
-    if (w == "attn_output.weight") return T(L.wo, E, QD);
-    if (w == "ffn_gate.weight") return T(L.gate, F, E);
-    if (w == "ffn_up.weight") return T(L.up, F, E);
-    if (w == "ffn_down.weight") return T(L.down, E, F);
-    is_f32 = true;
-    if (w == "attn_norm.weight") { *f32slot = &L.attn_norm; n_f32 = E; }
-    else if (w == "ffn_norm.weight") { *f32slot = &L.ffn_norm; n_f32 = E; }
-    else if (w == "attn_q.bias") { *f32slot = &L.bq; n_f32 = QD; }
-    else if (w == "attn_k.bias") { *f32slot = &L.bk; n_f32 = EK; }
-    else if (w == "attn_v.bias") { *f32slot = &L.bv; n_f32 = EK; }
-    else { is_f32 = false; }
-    return nullptr;
+    if (w == "attn_q.weight") return quant(L.wq, QD, E);
+    if (w == "attn_k.weight") return quant(L.wk, EK, E);
+    if (w == "attn_v.weight") return quant(L.wv, EK, E);
+    if (w == "attn_output.weight") return quant(L.wo, E, QD);
+    if (w == "ffn_gate.weight") return quant(L.gate, F, E);
+    if (w == "ffn_up.weight") return quant(L.up, F, E);
+    if (w == "ffn_down.weight") return quant(L.down, E, F);
+    if (w == "attn_norm.weight") return f32(L.attn_norm, E);
+    if (w == "ffn_norm.weight") return f32(L.ffn_norm, E);
+    if (w == "attn_q.bias") return f32(L.bq, QD);
+    if (w == "attn_k.bias") return f32(L.bk, EK);
+    if (w == "attn_v.bias") return f32(L.bv, EK);
+    return skipped;
 }
 
 extern "C" {
@@ -246,16 +308,13 @@ void pb200_model_free(pb200_model * m) {
     if (!m) return;
     cudaSetDevice(m->device);
     cudaStreamSynchronize(m->stream);
-    for (cudaGraphExec_t ge : m->graph_exec) if (ge) cudaGraphExecDestroy(ge);
+    for (Slot & s : m->slots) if (s.graph) cudaGraphExecDestroy(s.graph);
     for (void * p : m->allocs) cudaFree(p);
-    for (void * p : m->pf.allocs) cudaFree(p);
-    for (auto & p : m->pen) if (p.state) cudaFree(p.state);
-    if (m->pen_logits) cudaFree(m->pen_logits);
-    if (m->pen_tok) cudaFree(m->pen_tok);
+    for (cudaEvent_t e : m->prof_ev) cudaEventDestroy(e);
     if (m->tokpos_host) cudaFreeHost(m->tokpos_host);
     if (m->logits_host) cudaFreeHost(m->logits_host);
     cudaStreamDestroy(m->stream);
-    delete m;
+    delete m;   // the grow-only buffers free themselves
 }
 
 // Reserves the device memory of one tensor of this shard and returns its address (NULL with rc 0: the tensor lives on another stage).
@@ -263,32 +322,25 @@ void pb200_model_free(pb200_model * m) {
 int pb200_model_tensor_alloc(pb200_model * m, const char * name, int type, size_t nbytes, void ** dev_ptr) {
     if (!m || !name || !dev_ptr) return PB200_EINVAL;
     *dev_ptr = nullptr;
-    if (m->finalized) return PB200_ESTATE;
-    cudaSetDevice(m->device);
-    bool is_f32 = false;
-    float ** slot = nullptr;
-    int64_t n_f32 = 0;
-    Tensor * t = find_tensor(m, name, is_f32, &slot, n_f32);
-    if (is_f32) {
-        if (!slot) return 0;   // tensor belongs to another pipeline stage: ignore
-        if (type != T_F32 || nbytes != (size_t) n_f32 * 4) return PB200_EINVAL;
-        CK(m->alloc((void **) slot, nbytes));
-        *dev_ptr = *slot;
+    CK(building(m));
+    const Found f = find_tensor(m, name);
+    if (f.kind == Found::SKIPPED) return 0;
+    if (f.kind == Found::UNKNOWN) return PB200_EINVAL;
+    if (f.kind == Found::F32) {
+        if (type != T_F32 || nbytes != (size_t) f.n * 4) return PB200_EINVAL;
+        CK(m->alloc((void **) f.f32, nbytes));
+        *dev_ptr = *f.f32;
         return 0;
     }
-    if (!t) {
-        const std::string s(name);
-        if (s == "token_embd.weight" || s == "output.weight" || s.rfind("blk.", 0) == 0) return 0;   // other stage
-        return PB200_EINVAL;
-    }
+    Tensor & t = *f.t;
     if (!is_quant_type(type)) return PB200_ENOTSUP;
-    if (t->K % block_elems(type) != 0) return PB200_EINVAL;
-    const size_t need = (size_t) (row_bytes(type, t->K) * t->N);
+    if (t.K % block_elems(type) != 0) return PB200_EINVAL;
+    const size_t need = (size_t) (row_bytes(type, t.K) * t.N);
     if (nbytes != need) return PB200_EINVAL;
-    t->type = type;
-    t->bytes = need;
-    CK(m->alloc(&t->data, need + 16));
-    *dev_ptr = t->data;
+    t.type = type;
+    t.bytes = need;
+    CK(m->alloc(&t.data, need + 16));
+    *dev_ptr = t.data;
     return 0;
 }
 
@@ -301,9 +353,7 @@ int pb200_model_set_tensor(pb200_model * m, const char * name, int type, const v
 }
 
 int pb200_model_synth(pb200_model * m, int ftype, uint64_t seed) {
-    if (!m) return PB200_EINVAL;
-    if (m->finalized) return PB200_ESTATE;
-    cudaSetDevice(m->device);
+    CK(building(m));
     const pb200_hparams & hp = m->hp;
     const int def = ftype == 0 ? T_Q4_K : ftype == 2 ? T_Q4_0 : T_Q5_K;
     const bool kq = ftype != 2;   // Q4_0 (no imatrix): every matrix and the embedding Q4_0, only the head Q6_K (src/llama.cpp:19296-19460)
@@ -382,8 +432,14 @@ static int enqueue_step(pb200_model * m, int seq, uint64_t * nlaunch) {
     cudaStream_t st = m->stream;
     uint64_t n = 0;
     cudaEvent_t ev = nullptr;   // profiling: start event of the next GEMV group
-    const int32_t * tok_dev = m->tokpos_dev + 4 * seq, * pos_dev = m->tokpos_dev + 4 * seq + 1;
-    const size_t nl_ = m->layers.size();
+    // one GEMV group between its profiling events
+    auto gemv = [&](const GemvDesc * d, int nmat, int K, const ActQ & act, const GemvPrologue & pro, int64_t bytes, bool pdl, const char * what) -> int {
+        CK(prof_begin(m, bytes, ev));
+        CK(launch_gemv(d, nmat, K, act, pro, st, pdl, n, ev)); CK(dbg_sync(st, what));
+        return prof_end(m);
+    };
+    const Slot & s = m->slots[seq];
+    const int32_t * tok_dev = s.tokpos, * pos_dev = s.tokpos + 1;
     float * x = m->x_in;
     if (m->with_embd) {
         CK(launch_get_rows(m->tok_embd.data, m->tok_embd.type, E, tok_dev, 1, m->x_a, st, true)); n++; CK(dbg_sync(st, "get_rows"));
@@ -393,59 +449,38 @@ static int enqueue_step(pb200_model * m, int seq, uint64_t * nlaunch) {
     // three rotating hidden-state buffers so that a residual source is never overwritten by its consumer
     float * bufs[3] = {m->x_a, m->x_b, m->xn};
     for (int il = m->l0; il < m->l1; il++) {
-        Layer & L = m->layers[il - m->l0];
-        __half * kc = m->kcache + ((size_t) seq * nl_ + (size_t) (il - m->l0)) * hp.n_ctx * EK;
-        __half * vc = m->vcache + ((size_t) seq * nl_ + (size_t) (il - m->l0)) * hp.n_ctx * EK;
+        const int li = il - m->l0;
+        Layer & L = m->layers[li];
         float * x1 = nullptr, * x2 = nullptr;
         for (int i = 0; i < 3 && (!x1 || !x2); i++)
             if (bufs[i] != x) { if (!x1) x1 = bufs[i]; else x2 = bufs[i]; }
         if (il + 1 == m->l1) x2 = m->x_out;   // the last layer writes hidden_out in place (a copy node would break the PDL chain)
         // --- attention block ---
-        {
-            GemvDesc d[3] = {{L.wq.data, m->q, L.bq, nullptr, L.wq.type, QD},
-                             {L.wk.data, m->k, L.bk, nullptr, L.wk.type, EK},
-                             {L.wv.data, m->v, L.bv, nullptr, L.wv.type, EK}};
-            const GemvPrologue pro{PRO_RMSNORM, x, L.attn_norm, hp.rms_eps, m->gbar, m->g};   // g: scratch
-            CK(prof_begin(m, tbytes(L.wq) + tbytes(L.wk) + tbytes(L.wv), ev));
-            CK(launch_gemv(d, 3, E, m->actE.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv qkv"));
-            CK(prof_end(m));
-        }
+        const GemvDesc qkv[3] = {{L.wq.data, m->q, L.bq, nullptr, L.wq.type, QD},
+                                 {L.wk.data, m->k, L.bk, nullptr, L.wk.type, EK},
+                                 {L.wv.data, m->v, L.bv, nullptr, L.wv.type, EK}};
+        CK(gemv(qkv, 3, E, m->actE.q, GemvPrologue{PRO_RMSNORM, x, L.attn_norm, hp.rms_eps, m->gbar, m->g},   // g: scratch
+                tbytes(L.wq) + tbytes(L.wk) + tbytes(L.wv), true, "gemv qkv"));
         bool att_quantized = false;   // the attention kernel also wrote wo's activation
-        CK(launch_attn_step(m->q, m->k, m->v, kc, vc, m->att, m->actQD.q, act_mode_for(L.wo.type), H, HK, D, pos_dev, hp.n_ctx, m->rp, m->rope_ff,
-                            kq_scale, st, true, att_quantized)); n++; CK(dbg_sync(st, "attn"));
-        {
-            GemvDesc d1 = {L.wo.data, x1, nullptr, x, L.wo.type, E};   // ffn_inp = wo.att + inpSA
-            const GemvPrologue pro = att_quantized ? GemvPrologue{} : GemvPrologue{PRO_QUANTIZE, m->att};
-            CK(prof_begin(m, tbytes(L.wo), ev));
-            CK(launch_gemv(&d1, 1, QD, m->actQD.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv wo"));
-            CK(prof_end(m));
-        }
+        CK(launch_attn_step(m->q, m->k, m->v, s.kc(li), s.vc(li), m->att, m->actQD.q, act_mode_for(L.wo.type), H, HK, D, pos_dev, hp.n_ctx, m->rp,
+                            m->rope_ff, kq_scale, st, true, att_quantized)); n++; CK(dbg_sync(st, "attn"));
+        const GemvDesc wo = {L.wo.data, x1, nullptr, x, L.wo.type, E};   // ffn_inp = wo.att + inpSA
+        CK(gemv(&wo, 1, QD, m->actQD.q, att_quantized ? GemvPrologue{} : GemvPrologue{PRO_QUANTIZE, m->att}, tbytes(L.wo), true, "gemv wo"));
         // --- FFN block ---
-        {
-            GemvDesc d[2] = {{L.gate.data, m->g, nullptr, nullptr, L.gate.type, F}, {L.up.data, m->u, nullptr, nullptr, L.up.type, F}};
-            const GemvPrologue pro{PRO_RMSNORM, x1, L.ffn_norm, hp.rms_eps, m->gbar, m->att};   // att: scratch
-            CK(prof_begin(m, tbytes(L.gate) + tbytes(L.up), ev));
-            CK(launch_gemv(d, 2, E, m->actE.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv gate|up"));
-            CK(prof_end(m));
-        }
-        {
-            GemvDesc d1 = {L.down.data, x2, nullptr, x1, L.down.type, E};   // l_out = down.act + ffn_inp
-            const GemvPrologue pro{PRO_SILU_MUL, m->g, m->u, 0.f, m->gbar};
-            CK(prof_begin(m, tbytes(L.down), ev));
-            CK(launch_gemv(&d1, 1, F, m->actF.q, pro, st, true, n, ev)); CK(dbg_sync(st, "gemv down"));
-            CK(prof_end(m));
-        }
+        const GemvDesc gu[2] = {{L.gate.data, m->g, nullptr, nullptr, L.gate.type, F}, {L.up.data, m->u, nullptr, nullptr, L.up.type, F}};
+        CK(gemv(gu, 2, E, m->actE.q, GemvPrologue{PRO_RMSNORM, x1, L.ffn_norm, hp.rms_eps, m->gbar, m->att},   // att: scratch
+                tbytes(L.gate) + tbytes(L.up), true, "gemv gate|up"));
+        const GemvDesc down = {L.down.data, x2, nullptr, x1, L.down.type, E};   // l_out = down.act + ffn_inp
+        CK(gemv(&down, 1, F, m->actF.q, GemvPrologue{PRO_SILU_MUL, m->g, m->u, 0.f, m->gbar}, tbytes(L.down), true, "gemv down"));
         x = x2;
     }
     // hidden_out has a stable address for the next pipeline stage / tests (a stage without layers forwards its input)
     if (x != m->x_out) { CK(cudaMemcpyAsync(m->x_out, x, (size_t) E * 4, cudaMemcpyDeviceToDevice, st)); }
     if (m->with_head) {
-        GemvDesc d1 = {m->output.data, m->logits, nullptr, nullptr, m->output.type, hp.n_vocab};
-        const GemvPrologue pro{PRO_RMSNORM, m->x_out, m->output_norm, hp.rms_eps, m->gbar};
+        const GemvDesc head = {m->output.data, m->logits, nullptr, nullptr, m->output.type, hp.n_vocab};
         const bool head_pdl = m->l1 > m->l0;   // a stage without layers starts with a copy node: no programmatic edge
-        CK(prof_begin(m, tbytes(m->output), ev));
-        CK(launch_gemv(&d1, 1, E, m->actE.q, pro, st, head_pdl, n, ev));
-        CK(prof_end(m));
+        CK(gemv(&head, 1, E, m->actE.q, GemvPrologue{PRO_RMSNORM, m->x_out, m->output_norm, hp.rms_eps, m->gbar}, tbytes(m->output), head_pdl,
+                "gemv head"));
     }
     if (nlaunch) *nlaunch = n;
     return 0;
@@ -472,13 +507,13 @@ int pb200_model_finalize(pb200_model * m) {
         wb += E * 4;
     }
     m->weight_bytes = wb;
-    const size_t nl = m->layers.size();
-    const size_t kvb = (size_t) m->n_seq * nl * (size_t) hp.n_ctx * EK * sizeof(__half);
+    const size_t nl = m->layers.size(), layer_elems = (size_t) hp.n_ctx * EK;
+    m->kv_bytes = (size_t) m->n_seq * nl * layer_elems * sizeof(__half);
     if (nl) {
-        CK(m->alloc((void **) &m->kcache, kvb));
-        CK(m->alloc((void **) &m->vcache, kvb));
-        CK(cudaMemset(m->kcache, 0, kvb));
-        CK(cudaMemset(m->vcache, 0, kvb));
+        CK(m->alloc((void **) &m->kcache, m->kv_bytes));
+        CK(m->alloc((void **) &m->vcache, m->kv_bytes));
+        CK(cudaMemset(m->kcache, 0, m->kv_bytes));
+        CK(cudaMemset(m->vcache, 0, m->kv_bytes));
     }
     const int64_t big = std::max<int64_t>(std::max<int64_t>(F, QD), E);
     CK(m->alloc((void **) &m->x_in, E * 4));
@@ -494,7 +529,6 @@ int pb200_model_finalize(pb200_model * m) {
     CK(m->alloc((void **) &m->u, big * 4));
     if (m->with_head) CK(m->alloc((void **) &m->logits, (size_t) hp.n_vocab * 4));
     auto mk = [&](ActBuf & a, int64_t K) -> int {
-        a.K = K;
         CK(m->alloc(&a.base, act_ws_bytes(K)));
         CK(cudaMemset(a.base, 0, act_ws_bytes(K)));
         a.q = act_from_ws(a.base, K);
@@ -505,14 +539,23 @@ int pb200_model_finalize(pb200_model * m) {
     CK(mk(m->actF, F));
     CK(m->alloc((void **) &m->gbar, 16));
     CK(cudaMemset(m->gbar, 0, 16));
-    CK(m->alloc((void **) &m->tokpos_dev, 16 * (size_t) m->n_seq));
-    CK(cudaMemset(m->tokpos_dev, 0, 16 * (size_t) m->n_seq));
-    CK(m->alloc((void **) &m->sample_dev, 4 * (size_t) m->n_seq));
-    CK(cudaMemset(m->sample_dev, 0, 4 * (size_t) m->n_seq));
-    if (m->with_head) CK(m->alloc((void **) &m->sampler_state, sampler_state_bytes() * (size_t) m->n_seq));
-    m->sampling.assign((size_t) m->n_seq, pb200_sampling{});
-    m->sampling_set.assign((size_t) m->n_seq, 0);
-    m->pen.assign((size_t) m->n_seq, pb200_model::Penalty{});
+    int32_t * tokpos = nullptr, * sample = nullptr;
+    uint8_t * rng = nullptr;
+    CK(m->alloc((void **) &tokpos, 16 * (size_t) m->n_seq));
+    CK(cudaMemset(tokpos, 0, 16 * (size_t) m->n_seq));
+    CK(m->alloc((void **) &sample, 4 * (size_t) m->n_seq));
+    CK(cudaMemset(sample, 0, 4 * (size_t) m->n_seq));
+    if (m->with_head) CK(m->alloc((void **) &rng, sampler_state_bytes() * (size_t) m->n_seq));
+    m->slots = std::vector<Slot>((size_t) m->n_seq);
+    for (int sq = 0; sq < m->n_seq; sq++) {
+        Slot & s = m->slots[sq];
+        s.tokpos = tokpos + 4 * sq;
+        s.sample = sample + sq;
+        s.rng = rng ? rng + sampler_state_bytes() * (size_t) sq : nullptr;
+        s.k = m->kcache + (size_t) sq * nl * layer_elems;
+        s.v = m->vcache + (size_t) sq * nl * layer_elems;
+        s.layer_elems = layer_elems;
+    }
     CK(cudaMallocHost((void **) &m->tokpos_host, 16));
     if (m->with_head) CK(cudaMallocHost((void **) &m->logits_host, (size_t) hp.n_vocab * 4));
     rope_params_init(m->rp, hp.head_dim, hp.rope_mode, hp.n_ctx_orig, hp.rope_freq_base, hp.rope_freq_scale, 0.0f, 1.0f, 32.0f, 1.0f);
@@ -521,17 +564,17 @@ int pb200_model_finalize(pb200_model * m) {
     // warm-up (sets kernel attributes outside of capture), then capture the whole token as one graph per sequence slot
     CK(enqueue_step(m, 0, &m->launches_per_step));
     CK(cudaStreamSynchronize(m->stream));
-    if (nl) { CK(cudaMemset(m->kcache, 0, kvb)); CK(cudaMemset(m->vcache, 0, kvb)); }
-    m->graph_exec.assign((size_t) m->n_seq, nullptr);
+    if (nl) { CK(cudaMemset(m->kcache, 0, m->kv_bytes)); CK(cudaMemset(m->vcache, 0, m->kv_bytes)); }
     for (int sq = 0; sq < m->n_seq; sq++) {
+        Slot & s = m->slots[sq];
         cudaGraph_t graph = nullptr;
         cudaError_t e = cudaStreamBeginCapture(m->stream, cudaStreamCaptureModeThreadLocal);
         if (e != cudaSuccess) break;
         int rc = enqueue_step(m, sq, nullptr);
         e = cudaStreamEndCapture(m->stream, &graph);
         if (rc == 0 && e == cudaSuccess && graph) {
-            e = cudaGraphInstantiate(&m->graph_exec[sq], graph, 0);
-            if (e != cudaSuccess) m->graph_exec[sq] = nullptr;
+            e = cudaGraphInstantiate(&s.graph, graph, 0);
+            if (e != cudaSuccess) s.graph = nullptr;
         }
         if (graph) cudaGraphDestroy(graph);
     }
@@ -544,20 +587,18 @@ int64_t pb200_model_weight_bytes(const pb200_model * m) { return m ? m->weight_b
 
 int pb200_model_tensor_device(pb200_model * m, const char * name, const void ** dev_ptr, size_t * nbytes, int * type) {
     if (!m || !name || !dev_ptr || !nbytes) return PB200_EINVAL;
-    bool is_f32 = false;
-    float ** slot = nullptr;
-    int64_t n_f32 = 0;
-    Tensor * t = find_tensor(m, name, is_f32, &slot, n_f32);
-    if (is_f32) {
-        if (!slot || !*slot) return PB200_ESTATE;
-        *dev_ptr = *slot; *nbytes = (size_t) n_f32 * 4;
+    const Found f = find_tensor(m, name);
+    if (f.kind == Found::F32 && *f.f32) {
+        *dev_ptr = *f.f32; *nbytes = (size_t) f.n * 4;
         if (type) *type = T_F32;
         return 0;
     }
-    if (!t || !t->data) return PB200_ESTATE;
-    *dev_ptr = t->data; *nbytes = t->bytes;
-    if (type) *type = t->type;
-    return 0;
+    if (f.kind == Found::QUANT && f.t->data) {
+        *dev_ptr = f.t->data; *nbytes = f.t->bytes;
+        if (type) *type = f.t->type;
+        return 0;
+    }
+    return PB200_ESTATE;
 }
 
 }  // extern "C"
@@ -569,23 +610,19 @@ int pb200_model_tensor_device(pb200_model * m, const char * name, const void ** 
 static int pf_reserve(pb200_model * m, int T) {
     pb200_model::Prefill & P = m->pf;
     if (T <= P.T) return 0;
-    CK(cudaStreamSynchronize(m->stream));
-    for (void * p : P.allocs) cudaFree(p);
-    P.allocs.clear();
-    P.T = 0;
     const pb200_hparams & hp = m->hp;
     const size_t E = hp.n_embd, QD = (size_t) hp.n_head * hp.head_dim, EK = (size_t) hp.n_head_kv * hp.head_dim, F = hp.n_ff;
-    auto grab = [&](void ** p, size_t bytes) -> int {
-        cudaError_t e = cudaMalloc(p, (bytes + 255) / 256 * 256);
-        if (e != cudaSuccess) return (int) e;
-        P.allocs.push_back(*p);
-        return 0;
-    };
-    CK(grab((void **) &P.x0, T * E * 4)); CK(grab((void **) &P.x1, T * E * 4)); CK(grab((void **) &P.xn, T * std::max(E, QD) * 4));
-    CK(grab((void **) &P.q, T * QD * 4)); CK(grab((void **) &P.k, T * EK * 4)); CK(grab((void **) &P.v, T * EK * 4));
-    CK(grab((void **) &P.att, T * QD * 4)); CK(grab((void **) &P.g, T * F * 4)); CK(grab((void **) &P.u, T * F * 4));
-    CK(grab(&P.ws, mmq_workspace_bytes((int64_t) std::max(std::max(E, QD), F), T) + 256));
-    CK(grab((void **) &P.tok, (size_t) T * 4)); CK(grab((void **) &P.pos, (size_t) T * 4));
+    void ** part[] = {(void **) &P.x0, (void **) &P.x1, (void **) &P.xn, (void **) &P.q, (void **) &P.k, (void **) &P.v, (void **) &P.att,
+                      (void **) &P.g, (void **) &P.u, &P.ws, (void **) &P.tok, (void **) &P.pos};
+    const size_t bytes[] = {T * E * 4, T * E * 4, T * std::max(E, QD) * 4, T * QD * 4, T * EK * 4, T * EK * 4, T * QD * 4, T * F * 4, T * F * 4,
+                            mmq_workspace_bytes((int64_t) std::max(std::max(E, QD), F), T) + 256, (size_t) T * 4, (size_t) T * 4};
+    auto padded = [](size_t b) { return (b + 255) / 256 * 256; };
+    size_t total = 0;
+    for (size_t b : bytes) total += padded(b);
+    P.T = 0;
+    CK(P.mem.grow(total, m->stream));
+    char * p = (char *) P.mem.p;
+    for (int i = 0; i < 12; i++) { *part[i] = p; p += padded(bytes[i]); }
     P.T = T;
     return 0;
 }
@@ -620,7 +657,7 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
 static const int PB200_N_UBATCH = 512;   // the reference's default n_ubatch (common/common.h): longer prompts go through in slices
 
 extern "C" int pb200_prefill(pb200_model * m, const int32_t * tokens_host, int32_t T, int32_t pos0, float * logits_host) {
-    if (!m || !m->finalized) return PB200_ESTATE;
+    CK(ready(m));
     if (!tokens_host || T <= 0 || pos0 < 0 || pos0 + T > m->hp.n_ctx) return PB200_EINVAL;
     if (!m->with_embd || m->l0 != 0) return PB200_ENOTSUP;   // whole prompts start at the embedding; pipeline shards: pb200_prefill_stage
     for (int32_t done = 0; done < T; done += PB200_N_UBATCH) {
@@ -635,7 +672,7 @@ extern "C" int pb200_prefill(pb200_model * m, const int32_t * tokens_host, int32
 // previous stage's hidden states [n_tokens][n_embd] f32 in device memory (left untouched); the result stays in pb200_prefill_hidden_device.
 extern "C" int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host,
                                    int32_t synchronize) {
-    if (!m || !m->finalized) return PB200_ESTATE;
+    CK(ready(m));
     if (T <= 0 || T > PB200_N_UBATCH || pos0 < 0 || pos0 + T > m->hp.n_ctx) return PB200_EINVAL;
     if (m->with_embd ? !tokens_host : !hidden_in_dev) return PB200_EINVAL;
     if (logits_host && !synchronize) return PB200_EINVAL;   // host logits are read back at the synchronisation point
@@ -643,17 +680,14 @@ extern "C" int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host,
 }
 extern "C" float * pb200_prefill_hidden_device(pb200_model * m) { return (m && m->finalized) ? m->pf.x0 : nullptr; }
 
+// the callers have checked the model, T, pos0 and which input is given; prompts go to slot 0
 static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host, bool sync) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (T <= 0 || pos0 < 0 || pos0 + T > m->hp.n_ctx) return PB200_EINVAL;
-    if (m->with_embd) {
-        if (!tokens_host) return PB200_EINVAL;
+    if (m->with_embd)
         for (int t = 0; t < T; t++)
             if (tokens_host[t] < 0 || tokens_host[t] >= m->hp.n_vocab) return PB200_EINVAL;
-    } else if (!hidden_in_dev) return PB200_EINVAL;
-    cudaSetDevice(m->device);
     CK(pf_reserve(m, T));
     pb200_model::Prefill & P = m->pf;
+    const Slot & s0 = m->slots[0];
     const pb200_hparams & hp = m->hp;
     const int E = hp.n_embd, H = hp.n_head, HK = hp.n_head_kv, D = hp.head_dim, F = hp.n_ff;
     const int QD = H * D, EK = HK * D;
@@ -670,23 +704,19 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
     const float kq_scale = 1.0f / sqrtf((float) D);
     float * x = P.x0, * y = P.x1;
     for (int il = m->l0; il < m->l1; il++) {
-        Layer & L = m->layers[il - m->l0];
-        __half * kc = m->kcache + (size_t) (il - m->l0) * hp.n_ctx * EK;
-        __half * vc = m->vcache + (size_t) (il - m->l0) * hp.n_ctx * EK;
+        const int li = il - m->l0;
+        Layer & L = m->layers[li];
+        __half * kc = s0.kc(li), * vc = s0.vc(li);
+        // Each block's producer (rms_norm * norm weight, silu(g) * u) rides in the activation pass of the block's first mat-mul when the
+        // block takes the tensor-core path with k-quants (later mat-muls reuse its image); otherwise a kernel runs it first.
         // --- attention block ---
-        // rms_norm * attn_norm rides in the activation pass of q (k and v reuse its image) when all three take the tensor-core path
         const bool qkv_fused = pf_tc(L.wq, T) && pf_tc(L.wk, T) && pf_tc(L.wv, T) && is_kquant(L.wq.type) && is_kquant(L.wk.type) && is_kquant(L.wv.type);
-        if (qkv_fused) {
-            MmqPre pre; pre.kind = PRO_RMSNORM; pre.aux = L.attn_norm; pre.eps = hp.rms_eps;
-            CK(pf_matmul(m, L.wq, x, T, P.q, L.bq, nullptr, n, nullptr, &pre));
-            CK(pf_matmul(m, L.wk, x, T, P.k, L.bk, nullptr, n, &L.wq));
-            CK(pf_matmul(m, L.wv, x, T, P.v, L.bv, nullptr, n, &L.wk));
-        } else {
-            CK(launch_rms_norm(x, P.xn, E, T, hp.rms_eps, st, L.attn_norm)); n++;
-            CK(pf_matmul(m, L.wq, P.xn, T, P.q, L.bq, nullptr, n));
-            CK(pf_matmul(m, L.wk, P.xn, T, P.k, L.bk, nullptr, n, &L.wq));
-            CK(pf_matmul(m, L.wv, P.xn, T, P.v, L.bv, nullptr, n, &L.wk));
-        }
+        const MmqPre attn_norm{PRO_RMSNORM, L.attn_norm, 0, hp.rms_eps};
+        if (!qkv_fused) { CK(launch_rms_norm(x, P.xn, E, T, hp.rms_eps, st, L.attn_norm)); n++; }
+        const float * xa = qkv_fused ? x : P.xn;
+        CK(pf_matmul(m, L.wq, xa, T, P.q, L.bq, nullptr, n, nullptr, qkv_fused ? &attn_norm : nullptr));
+        CK(pf_matmul(m, L.wk, xa, T, P.k, L.bk, nullptr, n, &L.wq));
+        CK(pf_matmul(m, L.wv, xa, T, P.v, L.bv, nullptr, n, &L.wk));
         CK(launch_rope(P.q, P.q, T, H, D, QD, D, P.pos, m->rp, m->rope_ff, st)); n++;
         CK(launch_rope(P.k, P.k, T, HK, D, EK, D, P.pos, m->rp, m->rope_ff, st)); n++;
         CK(launch_cpy_f32_f16(P.k, kc + (size_t) pos0 * EK, (int64_t) T * EK, st)); n++;
@@ -694,22 +724,16 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
         CK(launch_attn_batch(P.q, kc, vc, P.att, H, HK, D, P.pos, T, pos0 + T, kq_scale, st)); n++;
         CK(pf_matmul(m, L.wo, P.att, T, y, nullptr, x, n));                  // ffn_inp = wo.att + inpSA (residual in the epilogue)
         // --- FFN block ---
-        if (pf_tc(L.gate, T) && pf_tc(L.up, T) && is_kquant(L.gate.type) && is_kquant(L.up.type)) {
-            MmqPre pre; pre.kind = PRO_RMSNORM; pre.aux = L.ffn_norm; pre.eps = hp.rms_eps;
-            CK(pf_matmul(m, L.gate, y, T, P.g, nullptr, nullptr, n, nullptr, &pre));
-            CK(pf_matmul(m, L.up, y, T, P.u, nullptr, nullptr, n, &L.gate));
-        } else {
-            CK(launch_rms_norm(y, P.xn, E, T, hp.rms_eps, st, L.ffn_norm)); n++;
-            CK(pf_matmul(m, L.gate, P.xn, T, P.g, nullptr, nullptr, n));
-            CK(pf_matmul(m, L.up, P.xn, T, P.u, nullptr, nullptr, n, &L.gate));
-        }
-        if (pf_tc(L.down, T) && is_kquant(L.down.type)) {                     // silu(g) * u inside ffn_down's activation pass
-            MmqPre pre; pre.kind = PRO_SILU_MUL; pre.aux = P.u; pre.ld_aux = F;
-            CK(pf_matmul(m, L.down, P.g, T, x, nullptr, y, n, nullptr, &pre));   // l_out = down.act + ffn_inp   (x is free: y holds ffn_inp)
-        } else {
-            CK(launch_silu_mul(P.g, P.u, P.g, (int64_t) T * F, st)); n++;
-            CK(pf_matmul(m, L.down, P.g, T, x, nullptr, y, n));
-        }
+        const bool gu_fused = pf_tc(L.gate, T) && pf_tc(L.up, T) && is_kquant(L.gate.type) && is_kquant(L.up.type);
+        const MmqPre ffn_norm{PRO_RMSNORM, L.ffn_norm, 0, hp.rms_eps};
+        if (!gu_fused) { CK(launch_rms_norm(y, P.xn, E, T, hp.rms_eps, st, L.ffn_norm)); n++; }
+        const float * xf = gu_fused ? y : P.xn;
+        CK(pf_matmul(m, L.gate, xf, T, P.g, nullptr, nullptr, n, nullptr, gu_fused ? &ffn_norm : nullptr));
+        CK(pf_matmul(m, L.up, xf, T, P.u, nullptr, nullptr, n, &L.gate));
+        const bool down_fused = pf_tc(L.down, T) && is_kquant(L.down.type);
+        const MmqPre silu_mul{PRO_SILU_MUL, P.u, F};
+        if (!down_fused) { CK(launch_silu_mul(P.g, P.u, P.g, (int64_t) T * F, st)); n++; }
+        CK(pf_matmul(m, L.down, P.g, T, x, nullptr, y, n, nullptr, down_fused ? &silu_mul : nullptr));   // l_out = down.act + ffn_inp (x is free: y holds ffn_inp)
     }
     // hidden state of the last token -> the decode path's output head
     CK(cudaMemcpyAsync(m->x_out, x + (size_t) (T - 1) * E, (size_t) E * 4, cudaMemcpyDeviceToDevice, st));
@@ -728,10 +752,8 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
 
 extern "C" {
 int pb200_kv_clear(pb200_model * m) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    cudaSetDevice(m->device);
-    const size_t kvb = (size_t) m->n_seq * m->layers.size() * (size_t) m->hp.n_ctx * m->hp.n_head_kv * m->hp.head_dim * sizeof(__half);
-    if (kvb) { CK(cudaMemsetAsync(m->kcache, 0, kvb, m->stream)); CK(cudaMemsetAsync(m->vcache, 0, kvb, m->stream)); }
+    CK(ready(m));
+    if (m->kv_bytes) { CK(cudaMemsetAsync(m->kcache, 0, m->kv_bytes, m->stream)); CK(cudaMemsetAsync(m->vcache, 0, m->kv_bytes, m->stream)); }
     return (int) cudaStreamSynchronize(m->stream);
 }
 
@@ -740,21 +762,19 @@ int pb200_kv_clear(pb200_model * m) {
 // per-slot graphs read the position from device memory, so they stay valid.
 int pb200_kv_seq_shift(pb200_model * m, int seq, int32_t p0, int32_t p1, int32_t delta) {
     if (delta >= 0 || (int64_t) p0 + delta < 0 || p0 >= p1) return PB200_EINVAL;   // checked before the model: no CUDA call needed
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq || p1 > m->hp.n_ctx) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    const pb200_hparams & hp = m->hp;
-    const size_t nl = m->layers.size(), slot = (size_t) seq * nl * (size_t) hp.n_ctx * hp.n_head_kv * hp.head_dim;
+    CK(ready_seq(m, seq));
+    if (p1 > m->hp.n_ctx) return PB200_EINVAL;
+    const Slot & s = m->slots[seq];
     g_launches++;
-    return launch_kv_shift(m->kcache ? m->kcache + slot : nullptr, m->vcache ? m->vcache + slot : nullptr, (int) nl, hp.n_head_kv, hp.n_ctx, p0, p1,
-                           delta, m->rp, m->rope_ff, m->tokpos_dev + 4 * seq, m->stream);
+    return launch_kv_shift(s.k, s.v, (int) m->layers.size(), m->hp.n_head_kv, m->hp.n_ctx, p0, p1, delta, m->rp, m->rope_ff, s.tokpos, m->stream);
 }
 void * pb200_kv_device(pb200_model * m, int v) { return (m && m->finalized) ? (void *) (v ? m->vcache : m->kcache) : nullptr; }
 
-static int step(pb200_model * m, int seq = 0) {
-    if (m->use_graph && (size_t) seq < m->graph_exec.size() && m->graph_exec[seq]) {
+static int step(pb200_model * m, int seq) {
+    const Slot & s = m->slots[seq];
+    if (m->use_graph && s.graph) {
         g_launches += m->launches_per_step;
-        return (int) cudaGraphLaunch(m->graph_exec[seq], m->stream);
+        return (int) cudaGraphLaunch(s.graph, m->stream);
     }
     uint64_t n = 0;
     int rc = enqueue_step(m, seq, &n);
@@ -790,23 +810,13 @@ extern "C++" int pb::launch_argmax(const float * x, int n, int32_t * out, int32_
 }
 __global__ void k_advance_pos(int32_t * tp) { pdl_trigger(); pdl_wait(); tp[1] += 1; }
 
-int pb200_decode_async(pb200_model * m, int32_t token, int32_t pos) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (pos < 0 || pos >= m->hp.n_ctx || token < 0 || token >= m->hp.n_vocab) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->tokpos_dev, token, pos);   // by-value kernel args: no host buffer to keep alive
-    CK(cudaGetLastError());
-    return step(m);
-}
-
 int pb200_decode(pb200_model * m, int32_t token, int32_t pos, float * logits_host) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (pos < 0 || pos >= m->hp.n_ctx || token < 0 || token >= m->hp.n_vocab) return PB200_EINVAL;
-    cudaSetDevice(m->device);
+    CK(ready(m));
+    if (!tokpos_ok(m, token, pos)) return PB200_EINVAL;
     m->tokpos_host[0] = token;
     m->tokpos_host[1] = pos;
-    CK(cudaMemcpyAsync(m->tokpos_dev, m->tokpos_host, 8, cudaMemcpyHostToDevice, m->stream));
-    CK(step(m));
+    CK(cudaMemcpyAsync(m->slots[0].tokpos, m->tokpos_host, 8, cudaMemcpyHostToDevice, m->stream));
+    CK(step(m, 0));
     if (m->with_head && logits_host) {
         CK(cudaMemcpyAsync(m->logits_host, m->logits, (size_t) m->hp.n_vocab * 4, cudaMemcpyDeviceToHost, m->stream));
         CK(cudaStreamSynchronize(m->stream));
@@ -820,99 +830,84 @@ int pb200_decode(pb200_model * m, int32_t token, int32_t pos, float * logits_hos
 
 // ---- several sequences in flight (prima's ring keeps every stage busy with a different token, src/llama.cpp:17825-18029, 18299-18387) ----
 int pb200_model_set_n_seq(pb200_model * m, int n_seq) {
-    if (!m || n_seq < 1 || n_seq > 64) return PB200_EINVAL;
-    if (m->finalized) return PB200_ESTATE;
+    if (n_seq < 1 || n_seq > 64) return PB200_EINVAL;
+    CK(building(m));
     m->n_seq = n_seq;
     return 0;
 }
 int pb200_decode_seq_async(pb200_model * m, int seq, int32_t token, int32_t pos) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq || pos < 0 || pos >= m->hp.n_ctx || token < 0 || token >= m->hp.n_vocab) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->tokpos_dev + 4 * seq, token, pos);
+    CK(ready_seq(m, seq));
+    if (!tokpos_ok(m, token, pos)) return PB200_EINVAL;
+    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->slots[seq].tokpos, token, pos);   // by-value kernel args: no host buffer to keep alive
     CK(cudaGetLastError());
     return step(m, seq);
 }
+int pb200_decode_async(pb200_model * m, int32_t token, int32_t pos) { return pb200_decode_seq_async(m, 0, token, pos); }
 // token and position of the slot are ALREADY in device memory (pb200_token_device: written by the previous stage's hand-off or by
 // pb200_argmax_seq); nothing crosses the host.  advance_pos: bump the slot's position afterwards for its next step.
 int pb200_step_seq_dev(pb200_model * m, int seq, int advance_pos) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
-    cudaSetDevice(m->device);
+    CK(ready_seq(m, seq));
     CK(step(m, seq));
     if (advance_pos) {
-        k_advance_pos<<<1, 1, 0, m->stream>>>(m->tokpos_dev + 4 * seq);
+        k_advance_pos<<<1, 1, 0, m->stream>>>(m->slots[seq].tokpos);
         g_launches++;
         CK(cudaGetLastError());
     }
     return 0;
 }
 int pb200_set_tokpos_seq(pb200_model * m, int seq, int32_t token, int32_t pos) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->tokpos_dev + 4 * seq, token, pos);
+    CK(ready_seq(m, seq));
+    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->slots[seq].tokpos, token, pos);
     return (int) cudaGetLastError();
 }
-// greedy token of the slot's logits -> sample_dev[seq] (and, when this shard also holds the embedding, straight into the slot's token)
+// greedy token of the slot's logits -> the slot's sample word (and, when this shard also holds the embedding, straight into its token)
 int pb200_argmax_seq(pb200_model * m, int seq, int feed_back) {
-    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    LaunchCfg lc(dim3(1), dim3(1024), 0, m->stream, true);
+    CK(ready_seq(m, seq, true));
+    const Slot & s = m->slots[seq];
     g_launches++;
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_argmax, (const float *) m->logits, (int) m->hp.n_vocab, m->sample_dev + seq,
-                                    (int32_t *) (feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr));
+    return launch_argmax(m->logits, (int) m->hp.n_vocab, s.sample, feed_back && m->with_embd ? s.tokpos : nullptr, m->stream, true);
 }
 // seeded sampling of the slot (sample.cu): parameters checked and the slot's generator seeded here, on the model stream
 int pb200_sampling_set_seq(pb200_model * m, int seq, const pb200_sampling * p) {
-    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq || !sampling_params_ok(p)) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    CK(launch_sampler_seed(m->sampler_state + sampler_state_bytes() * (size_t) seq, p->seed, m->stream));
-    m->sampling[seq] = *p;
-    m->sampling_set[seq] = 1;
+    CK(ready_seq(m, seq, true));
+    if (!sampling_params_ok(p)) return PB200_EINVAL;
+    Slot & s = m->slots[seq];
+    CK(launch_sampler_seed(s.rng, p->seed, m->stream));
+    s.sampling = *p;
+    s.sampling_set = true;
     return 0;
 }
-// like pb200_argmax_seq with the slot's sampling parameters: -> sample_dev[seq] (and with feed_back the slot's token)
+// like pb200_argmax_seq with the slot's sampling parameters (and logit bias + penalties when the slot has them)
 int pb200_sample_seq(pb200_model * m, int seq, int feed_back) {
-    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq) return PB200_EINVAL;
-    if (!m->sampling_set[seq]) return PB200_ESTATE;
-    cudaSetDevice(m->device);
-    const pb200_model::Penalty & pen = m->pen[seq];
+    CK(ready_seq(m, seq, true));
+    const Slot & s = m->slots[seq];
+    if (!s.sampling_set) return PB200_ESTATE;
     const int n = (int) m->hp.n_vocab;
     const float * row = m->logits;
-    if (pen.set) {                      // logit bias + penalties on a copy of the row, then the unchanged chain on that copy
-        CK(launch_penalize(m->logits, n, pen.state, m->pen_logits, m->stream, true));
+    if (s.pen.set) {                    // logit bias + penalties on a copy of the row, then the unchanged chain on that copy
+        CK(launch_penalize(m->logits, n, s.pen.state.p, (float *) m->pen_logits.p, m->stream, true));
         g_launches++;
-        row = m->pen_logits;
+        row = (const float *) m->pen_logits.p;
     }
-    CK(launch_sample(row, n, m->sampling[seq], m->sampler_state + sampler_state_bytes() * (size_t) seq, m->sample_dev + seq,
-                     feed_back && m->with_embd ? m->tokpos_dev + 4 * seq : nullptr, m->stream, true));
+    CK(launch_sample(row, n, s.sampling, s.rng, s.sample, feed_back && m->with_embd ? s.tokpos : nullptr, m->stream, true));
     g_launches++;
-    if (pen.set && pen.last_n > 0) {    // gpt_sampler_accept: the token joins the slot's history
-        CK(launch_penalty_accept(pen.state, m->sample_dev + seq, 1, m->stream, true));
+    if (s.pen.set && s.pen.last_n > 0) {   // gpt_sampler_accept: the token joins the slot's history
+        CK(launch_penalty_accept(s.pen.state.p, s.sample, 1, m->stream, true));
         g_launches++;
     }
     return 0;
 }
 // logit bias + penalties of the slot: state allocated (or grown) here, configuration uploaded and history cleared on the model stream
 int pb200_penalties_set_seq(pb200_model * m, int seq, const pb200_penalties * p) {
-    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq || (p && !penalties_ok(p))) return PB200_EINVAL;
-    pb200_model::Penalty & pen = m->pen[seq];
-    if (!p) { pen.set = false; return 0; }
-    cudaSetDevice(m->device);
-    if (!m->pen_logits) CK(cudaMalloc((void **) &m->pen_logits, (size_t) m->hp.n_vocab * 4));
-    const size_t bytes = penalty_state_bytes(p->last_n, p->n_logit_bias);
-    if (bytes > pen.bytes) {
-        if (pen.state) { CK(cudaStreamSynchronize(m->stream)); CK(cudaFree(pen.state)); pen.state = nullptr; pen.bytes = 0; pen.set = false; }
-        CK(cudaMalloc(&pen.state, bytes));
-        pen.bytes = bytes;
-    }
+    CK(ready_seq(m, seq, true));
+    if (p && !penalties_ok(p)) return PB200_EINVAL;
+    Penalty & pen = m->slots[seq].pen;
+    pen.set = false;                    // until the new configuration is in place
+    if (!p) return 0;
+    CK(m->pen_logits.grow((size_t) m->hp.n_vocab * 4, m->stream));
+    CK(pen.state.grow(penalty_state_bytes(p->last_n, p->n_logit_bias), m->stream));
     uint64_t nl = 0;
-    const int rc = launch_penalty_init(pen.state, (int) m->hp.n_vocab, *p, m->stream, nl);
+    const int rc = launch_penalty_init(pen.state.p, (int) m->hp.n_vocab, *p, m->stream, nl);
     g_launches += nl;
     if (rc) return rc;
     pen.last_n = std::max(p->last_n, 0);
@@ -921,28 +916,22 @@ int pb200_penalties_set_seq(pb200_model * m, int seq, const pb200_penalties * p)
 }
 // llama-cli accepts the prompt into the sampler (examples/main/main.cpp:720): the last last_n host tokens go to the slot's history
 int pb200_sampler_accept_seq(pb200_model * m, int seq, const int32_t * tokens_host, int n) {
-    if (!m || !m->finalized || !m->with_head) return PB200_ESTATE;
-    if (seq < 0 || seq >= m->n_seq || n < 0 || (n > 0 && !tokens_host)) return PB200_EINVAL;
-    const pb200_model::Penalty & pen = m->pen[seq];
+    CK(ready_seq(m, seq, true));
+    if (n < 0 || (n > 0 && !tokens_host)) return PB200_EINVAL;
+    const Penalty & pen = m->slots[seq].pen;
     if (!pen.set) return PB200_ESTATE;
     const int k = std::min(n, pen.last_n);
     if (k == 0) return 0;
-    cudaSetDevice(m->device);
-    if ((size_t) k > m->pen_tok_n) {
-        CK(cudaStreamSynchronize(m->stream));
-        if (m->pen_tok) { CK(cudaFree(m->pen_tok)); m->pen_tok = nullptr; m->pen_tok_n = 0; }
-        CK(cudaMalloc((void **) &m->pen_tok, (size_t) k * 4));
-        m->pen_tok_n = (size_t) k;
-    }
+    CK(m->pen_tok.grow((size_t) k * 4, m->stream));
     // from pageable memory the copy returns once the tokens are staged, so the caller may reuse its array; stream order keeps the
     // staging buffer until the accept has read it
-    CK(cudaMemcpyAsync(m->pen_tok, tokens_host + (n - k), (size_t) k * 4, cudaMemcpyHostToDevice, m->stream));
-    CK(launch_penalty_accept(pen.state, m->pen_tok, k, m->stream, false));
+    CK(cudaMemcpyAsync(m->pen_tok.p, tokens_host + (n - k), (size_t) k * 4, cudaMemcpyHostToDevice, m->stream));
+    CK(launch_penalty_accept(pen.state.p, (const int32_t *) m->pen_tok.p, k, m->stream, false));
     g_launches++;
     return 0;
 }
-int32_t * pb200_token_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->tokpos_dev + 4 * seq : nullptr; }
-int32_t * pb200_sample_device(pb200_model * m, int seq) { return (m && seq >= 0 && seq < m->n_seq) ? m->sample_dev + seq : nullptr; }
+int32_t * pb200_token_device(pb200_model * m, int seq) { return (m && seq >= 0 && (size_t) seq < m->slots.size()) ? m->slots[seq].tokpos : nullptr; }
+int32_t * pb200_sample_device(pb200_model * m, int seq) { return (m && seq >= 0 && (size_t) seq < m->slots.size()) ? m->slots[seq].sample : nullptr; }
 
 int pb200_synchronize(pb200_model * m) {
     if (!m) return PB200_EINVAL;
@@ -955,30 +944,32 @@ float * pb200_hidden_in_device(pb200_model * m) { return m ? m->x_in : nullptr; 
 float * pb200_hidden_out_device(pb200_model * m) { return m ? m->x_out : nullptr; }
 void * pb200_stream(pb200_model * m) { return m ? (void *) m->stream : nullptr; }
 int pb200_get_hidden(pb200_model * m, float * hidden_host) {
-    if (!m || !m->finalized || !hidden_host) return PB200_EINVAL;
-    cudaSetDevice(m->device);
+    if (!hidden_host) return PB200_EINVAL;
+    CK(ready(m, false, PB200_EINVAL));
     CK(cudaStreamSynchronize(m->stream));
     return (int) cudaMemcpy(hidden_host, m->x_out, (size_t) m->hp.n_embd * 4, cudaMemcpyDeviceToHost);
 }
 int pb200_profile_step(pb200_model * m, int32_t token, int32_t pos, double * gemv_ms, int64_t * gemv_bytes, int32_t * gemv_launches, double * step_ms) {
-    if (!m || !m->finalized) return PB200_ESTATE;
-    if (pos < 0 || pos >= m->hp.n_ctx || token < 0 || token >= m->hp.n_vocab) return PB200_EINVAL;
-    cudaSetDevice(m->device);
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->tokpos_dev, token, pos);
+    CK(ready(m));
+    if (!tokpos_ok(m, token, pos)) return PB200_EINVAL;
+    struct Event {                      // released on every return
+        cudaEvent_t e = nullptr;
+        ~Event() { if (e) cudaEventDestroy(e); }
+    } e0, e1;
+    CK(cudaEventCreate(&e0.e)); CK(cudaEventCreate(&e1.e));
+    k_set_tokpos<<<1, 1, 0, m->stream>>>(m->slots[0].tokpos, token, pos);
+    CK(cudaEventRecord(e0.e, m->stream));
     m->profiling = true;
     m->prof_n = 0;
-    CK(cudaEventRecord(e0, m->stream));
     uint64_t n = 0;
     int rc = enqueue_step(m, 0, &n);
     m->profiling = false;
     if (rc) return rc;
     g_launches += n;
-    CK(cudaEventRecord(e1, m->stream));
+    CK(cudaEventRecord(e1.e, m->stream));
     CK(cudaStreamSynchronize(m->stream));
     float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, e0, e1));
+    CK(cudaEventElapsedTime(&ms, e0.e, e1.e));
     if (step_ms) *step_ms = ms;
     double tot = 0; int64_t by = 0;
     for (size_t i = 0; i < m->prof_n; i++) {
@@ -989,19 +980,18 @@ int pb200_profile_step(pb200_model * m, int32_t token, int32_t pos, double * gem
     if (gemv_ms) *gemv_ms = tot;
     if (gemv_bytes) *gemv_bytes = by;
     if (gemv_launches) *gemv_launches = (int32_t) m->prof_n;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
     return 0;
 }
 int pb200_set_hidden(pb200_model * m, const float * hidden_host) {
-    if (!m || !m->finalized || !hidden_host) return PB200_EINVAL;
-    cudaSetDevice(m->device);
+    if (!hidden_host) return PB200_EINVAL;
+    CK(ready(m, false, PB200_EINVAL));
     CK(cudaStreamSynchronize(m->stream));
     return (int) cudaMemcpy(m->x_in, hidden_host, (size_t) m->hp.n_embd * 4, cudaMemcpyHostToDevice);
 }
 // debugging / white-box tests: copy a named internal activation buffer of the LAST step to the host
 int pb200_debug_read(pb200_model * m, const char * name, float * host, int64_t n) {
-    if (!m || !m->finalized || !name || !host) return PB200_EINVAL;
-    cudaSetDevice(m->device);
+    if (!name || !host) return PB200_EINVAL;
+    CK(ready(m, false, PB200_EINVAL));
     CK(cudaStreamSynchronize(m->stream));
     const std::string s(name);
     const float * p = s == "q" ? m->q : s == "k" ? m->k : s == "v" ? m->v : s == "att" ? m->att : s == "g" ? m->g : s == "u" ? m->u :
