@@ -16,6 +16,7 @@
  *   pb200_rope_f16          the same on f16 rows (rope.cu:200-262); CPU ggml.c:14269-14380
  *   pb200_kv_seq_shift      llama_kv_cache_seq_rm + seq_add (src/llama.cpp:4378-4427) and the K-shift graph of build_k_shift
  *                           (:10665-10719) that llama_kv_cache_update_internal runs at the next decode (:19102-19134)
+ *   pb200_kv_seq_cp         llama_kv_cache_seq_cp (src/llama.cpp:4308-4350, 22646-22651)
  *   pb200_soft_max          ggml_cuda_op_soft_max softmax.cu:170-206; CPU ggml.c:13783-13880
  *   pb200_attn_decode       FA-off attention chain: ggml_cuda_mul_mat_batched_cublas x2 + soft_max + cont,
  *                           ggml-cuda.cu:1737-1881; graph src/llama.cpp:10032-10165
@@ -288,6 +289,20 @@ PB200_API int pb200_prefill(pb200_model * m, const int32_t * tokens_host, int32_
  * synchronize != 0.  K/V rows pos0 .. pos0+n_tokens-1 of this shard's layers are written like pb200_prefill writes them. */
 PB200_API int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t n_tokens, int32_t pos0,
                                   float * logits_host, int32_t synchronize);
+/* The same two calls on sequence slot seq (the reference's server processes each slot's prompt into that slot's sequence,
+ * examples/server/server.cpp); pb200_prefill and pb200_prefill_stage are their seq = 0 forms and launch exactly the same kernels.
+ *   - seq outside [0, n_seq): PB200_EINVAL, checked right after the model (NULL / unfinalized: PB200_ESTATE).  Every other argument rule
+ *     and its code are those of the seq = 0 form, in the same order (a shard without the embedding: PB200_ENOTSUP from pb200_prefill_seq).
+ *   - Only slot seq's cells pos0 .. pos0+n_tokens-1 of this shard's layers are written; every other slot's cache, {token, position} and
+ *     sample words stay bit-identical.  The slot's own {token, position} words are not touched either.
+ *   - The last prompt token's logits land in pb200_logits_device(m) (and logits_host), so pb200_argmax_seq / pb200_sample_seq(seq, feed_back)
+ *     pick the first generated token on the device.  The host sets the slot's position: pb200_set_tokpos_seq(seq, any, pos0 + n_tokens)
+ *     first, then the argmax / sample with feed_back overwrites the token word only.
+ *   - The prefill scratch, the hidden states of pb200_prefill_hidden_device, hidden_out and the logits are shared by all slots.  That is
+ *     safe because every call of the engine is ordered on the model stream; a host that reads them must do so before the next call. */
+PB200_API int pb200_prefill_seq(pb200_model * m, int seq, const int32_t * tokens_host, int32_t n_tokens, int32_t pos0, float * logits_host);
+PB200_API int pb200_prefill_stage_seq(pb200_model * m, int seq, const int32_t * tokens_host, const float * hidden_in_dev, int32_t n_tokens, int32_t pos0,
+                                      float * logits_host, int32_t synchronize);
 PB200_API float * pb200_prefill_hidden_device(pb200_model * m);
 PB200_API int pb200_kv_clear(pb200_model * m);
 /* prima's context shift on this shard's cache for slot seq (what llama-cli does when the context fills, examples/main/main.cpp:578-608):
@@ -307,6 +322,17 @@ PB200_API int pb200_kv_clear(pb200_model * m);
  *     per-slot CUDA graphs stay valid (they read the position from device memory).
  *   - One launch enqueued on the model stream, no host synchronisation; call it outside any stream capture, like pb200_sampling_set_seq. */
 PB200_API int pb200_kv_seq_shift(pb200_model * m, int seq, int32_t p0, int32_t p1, int32_t delta);
+/* llama_kv_cache_seq_cp(seq_src, seq_dst, p0, p1) (src/llama.cpp:4308-4350): cells [p0, p1) of every layer of this shard, K and V, copied bit
+ * for bit from slot seq_src to slot seq_dst — a shared system prompt prefilled once and forked to every slot (examples/server/server.cpp,
+ * examples/parallel/parallel.cpp).  The reference's conventions: p0 < 0 means 0, p1 < 0 means n_ctx, p1 > n_ctx is clamped to n_ctx.
+ *   - seq_src == seq_dst and an empty range are no-ops that return 0; a shard without layers has nothing to copy and returns 0.
+ *   - A slot outside [0, n_seq): PB200_EINVAL; NULL / unfinalized model: PB200_ESTATE.  Any pipeline shard, with or without embedding / head.
+ *   - Neither slot's {token, position} words, sampling state or penalty history change: the host sets seq_dst's position
+ *     (pb200_set_tokpos_seq) or prefills its suffix next (pb200_prefill_seq at pos0 = p1).
+ *   - Two 2-D copies on the model stream (one per cache: one contiguous run per layer), no kernel, no host synchronisation.
+ * llama_kv_cache_seq_rm(seq, p, -1) needs no call here: the engine keeps cell == position and attention reads only cells [0, pos], so the
+ * next prefill or decode at p overwrites the cells from p on before anything reads them. */
+PB200_API int pb200_kv_seq_cp(pb200_model * m, int seq_src, int seq_dst, int32_t p0, int32_t p1);
 /* device address of the f16 K (v == 0) or V (v != 0) cache of this shard: [n_seq][layer_end - layer_begin][n_ctx][n_head_kv * head_dim]
  * (white-box tests and hosts that inspect the cache; NULL before finalize or on a shard without layers) */
 PB200_API void * pb200_kv_device(pb200_model * m, int v);

@@ -653,41 +653,51 @@ __global__ void k_iota_pos(int32_t * pos, int pos0, int T) {
     if (i < T) pos[i] = pos0 + i;
 }
 
-static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host, bool sync);
+static int prefill_ubatch(pb200_model * m, int seq, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host,
+                          bool sync);
 static const int PB200_N_UBATCH = 512;   // the reference's default n_ubatch (common/common.h): longer prompts go through in slices
 
-extern "C" int pb200_prefill(pb200_model * m, const int32_t * tokens_host, int32_t T, int32_t pos0, float * logits_host) {
-    CK(ready(m));
+extern "C" int pb200_prefill_seq(pb200_model * m, int seq, const int32_t * tokens_host, int32_t T, int32_t pos0, float * logits_host) {
+    CK(ready_seq(m, seq));
     if (!tokens_host || T <= 0 || pos0 < 0 || pos0 + T > m->hp.n_ctx) return PB200_EINVAL;
     if (!m->with_embd || m->l0 != 0) return PB200_ENOTSUP;   // whole prompts start at the embedding; pipeline shards: pb200_prefill_stage
     for (int32_t done = 0; done < T; done += PB200_N_UBATCH) {
         const int32_t n = std::min<int32_t>(PB200_N_UBATCH, T - done);
-        const int rc = prefill_ubatch(m, tokens_host + done, nullptr, n, pos0 + done, done + n == T ? logits_host : nullptr, true);
+        const int rc = prefill_ubatch(m, seq, tokens_host + done, nullptr, n, pos0 + done, done + n == T ? logits_host : nullptr, true);
         if (rc) return rc;
     }
     return 0;
 }
+extern "C" int pb200_prefill(pb200_model * m, const int32_t * tokens_host, int32_t T, int32_t pos0, float * logits_host) {
+    return pb200_prefill_seq(m, 0, tokens_host, T, pos0, logits_host);
+}
 // One ubatch (<= 512 tokens) through THIS shard's layers: prima's layer windows during prompt processing (src/llama.cpp:17825-18029: every
 // rank runs its window of the sub-graph on the ubatch and ships the hidden states on).  The first stage takes token ids, the others the
 // previous stage's hidden states [n_tokens][n_embd] f32 in device memory (left untouched); the result stays in pb200_prefill_hidden_device.
-extern "C" int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host,
-                                   int32_t synchronize) {
-    CK(ready(m));
+extern "C" int pb200_prefill_stage_seq(pb200_model * m, int seq, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0,
+                                       float * logits_host, int32_t synchronize) {
+    CK(ready_seq(m, seq));
     if (T <= 0 || T > PB200_N_UBATCH || pos0 < 0 || pos0 + T > m->hp.n_ctx) return PB200_EINVAL;
     if (m->with_embd ? !tokens_host : !hidden_in_dev) return PB200_EINVAL;
     if (logits_host && !synchronize) return PB200_EINVAL;   // host logits are read back at the synchronisation point
-    return prefill_ubatch(m, tokens_host, hidden_in_dev, T, pos0, logits_host, synchronize != 0);
+    return prefill_ubatch(m, seq, tokens_host, hidden_in_dev, T, pos0, logits_host, synchronize != 0);
+}
+extern "C" int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host,
+                                   int32_t synchronize) {
+    return pb200_prefill_stage_seq(m, 0, tokens_host, hidden_in_dev, T, pos0, logits_host, synchronize);
 }
 extern "C" float * pb200_prefill_hidden_device(pb200_model * m) { return (m && m->finalized) ? m->pf.x0 : nullptr; }
 
-// the callers have checked the model, T, pos0 and which input is given; prompts go to slot 0
-static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host, bool sync) {
+// the callers have checked the model, seq, T, pos0 and which input is given; the prompt's K/V rows go to slot seq.  The scratch, x_out and
+// the logits are shared by all slots: every call is ordered on the model stream.
+static int prefill_ubatch(pb200_model * m, int seq, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host,
+                          bool sync) {
     if (m->with_embd)
         for (int t = 0; t < T; t++)
             if (tokens_host[t] < 0 || tokens_host[t] >= m->hp.n_vocab) return PB200_EINVAL;
     CK(pf_reserve(m, T));
     pb200_model::Prefill & P = m->pf;
-    const Slot & s0 = m->slots[0];
+    const Slot & s = m->slots[seq];
     const pb200_hparams & hp = m->hp;
     const int E = hp.n_embd, H = hp.n_head, HK = hp.n_head_kv, D = hp.head_dim, F = hp.n_ff;
     const int QD = H * D, EK = HK * D;
@@ -706,7 +716,7 @@ static int prefill_ubatch(pb200_model * m, const int32_t * tokens_host, const fl
     for (int il = m->l0; il < m->l1; il++) {
         const int li = il - m->l0;
         Layer & L = m->layers[li];
-        __half * kc = s0.kc(li), * vc = s0.vc(li);
+        __half * kc = s.kc(li), * vc = s.vc(li);
         // Each block's producer (rms_norm * norm weight, silu(g) * u) rides in the activation pass of the block's first mat-mul when the
         // block takes the tensor-core path with k-quants (later mat-muls reuse its image); otherwise a kernel runs it first.
         // --- attention block ---
@@ -767,6 +777,22 @@ int pb200_kv_seq_shift(pb200_model * m, int seq, int32_t p0, int32_t p1, int32_t
     const Slot & s = m->slots[seq];
     g_launches++;
     return launch_kv_shift(s.k, s.v, (int) m->layers.size(), m->hp.n_head_kv, m->hp.n_ctx, p0, p1, delta, m->rp, m->rope_ff, s.tokpos, m->stream);
+}
+// llama_kv_cache_seq_cp (src/llama.cpp:4308-4350): cells [p0, p1) of every layer of this shard from slot src to slot dst.  In the slot layout
+// [n_seq][layer][n_ctx][row] the range is one contiguous run per layer at the pitch of one layer's block: one 2-D copy each for K and V on
+// the model stream, no kernel, no host synchronisation.
+int pb200_kv_seq_cp(pb200_model * m, int seq_src, int seq_dst, int32_t p0, int32_t p1) {
+    CK(ready_seq(m, seq_src));
+    CK(ready_seq(m, seq_dst));
+    const int32_t n_ctx = m->hp.n_ctx;
+    if (p0 < 0) p0 = 0;
+    if (p1 < 0 || p1 > n_ctx) p1 = n_ctx;
+    if (seq_src == seq_dst || p0 >= p1 || m->layers.empty()) return 0;
+    const Slot & s = m->slots[seq_src], & d = m->slots[seq_dst];
+    const size_t row = (size_t) m->hp.n_head_kv * m->hp.head_dim * sizeof(__half), pitch = s.layer_elems * sizeof(__half);
+    const size_t off = (size_t) p0 * row, width = (size_t) (p1 - p0) * row, nl = m->layers.size();
+    CK(cudaMemcpy2DAsync((char *) d.k + off, pitch, (const char *) s.k + off, pitch, width, nl, cudaMemcpyDeviceToDevice, m->stream));
+    return (int) cudaMemcpy2DAsync((char *) d.v + off, pitch, (const char *) s.v + off, pitch, width, nl, cudaMemcpyDeviceToDevice, m->stream);
 }
 void * pb200_kv_device(pb200_model * m, int v) { return (m && m->finalized) ? (void *) (v ? m->vcache : m->kcache) : nullptr; }
 

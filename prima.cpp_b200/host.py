@@ -123,6 +123,9 @@ class Lib:
         c.pb200_decode.argtypes = [vp, i32, i32, vp]
         c.pb200_prefill.argtypes = [vp, vp, i32, i32, vp]
         c.pb200_prefill_stage.argtypes = [vp, vp, vp, i32, i32, vp, i32]
+        c.pb200_prefill_seq.argtypes = [vp, C.c_int, vp, i32, i32, vp]
+        c.pb200_prefill_stage_seq.argtypes = [vp, C.c_int, vp, vp, i32, i32, vp, i32]
+        c.pb200_kv_seq_cp.argtypes = [vp, C.c_int, C.c_int, i32, i32]
         c.pb200_gguf_probe.argtypes = [C.c_char_p, C.POINTER(HParams), C.POINTER(i32), C.POINTER(i64), C.c_char_p]
         c.pb200_model_load_gguf.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp), C.POINTER(C.c_double), C.POINTER(i64)]
         c.pb200_model_tensor_alloc.argtypes = [vp, C.c_char_p, C.c_int, C.c_size_t, C.POINTER(vp)]
@@ -255,6 +258,11 @@ class Model:
         n_discard = (n_past - n_keep) // 2, kv_shift(seq, n_keep + n_discard, n_past, -n_discard)."""
         self.lib.check(self.lib.c.pb200_kv_seq_shift(self.h, seq, int(p0), int(p1), int(delta)), "kv_seq_shift")
 
+    def kv_copy(self, src: int, dst: int, p0: int = -1, p1: int = -1) -> None:
+        """llama_kv_cache_seq_cp (pb200_kv_seq_cp): cells [p0, p1) of every layer of this shard from slot src to slot dst, bit for bit
+        (p0 < 0: 0, p1 < 0: n_ctx).  Enqueued on the model stream; positions, sampling and penalties of both slots are left alone."""
+        self.lib.check(self.lib.c.pb200_kv_seq_cp(self.h, int(src), int(dst), int(p0), int(p1)), "kv_seq_cp")
+
     def kv_ptr(self, v: bool = False) -> int:
         """Device address of the f16 K (or V) cache: [n_seq][layers of this shard][n_ctx][n_head_kv * 128]."""
         return self.lib.c.pb200_kv_device(self.h, int(v)) or 0
@@ -264,25 +272,28 @@ class Model:
         self.lib.check(self.lib.c.pb200_decode(self.h, token, pos, ptr), "decode")
         return logits_out
 
-    def prefill(self, tokens, pos0: int = 0, logits_out=None):
-        """Prompt processing: all tokens as one batch (tensor-core mat-muls); returns the last token's logits."""
+    def prefill(self, tokens, pos0: int = 0, logits_out=None, seq: int = 0):
+        """Prompt processing into slot seq: all tokens as one batch (tensor-core mat-muls); returns the last token's logits.  The slot's
+        {token, position} words are left alone (set_tokpos_seq, then argmax_seq / sample_seq with feed_back, start its decoding)."""
         import numpy as np
         toks = np.ascontiguousarray(tokens, dtype=np.int32)
         out = logits_out if logits_out is not None else np.empty(self.hp.n_vocab, dtype=np.float32)
-        self.lib.check(self.lib.c.pb200_prefill(self.h, toks.ctypes.data_as(C.c_void_p), int(toks.size), int(pos0), out.ctypes.data_as(C.c_void_p)),
-                       "prefill")
+        self.lib.check(self.lib.c.pb200_prefill_seq(self.h, int(seq), toks.ctypes.data_as(C.c_void_p), int(toks.size), int(pos0),
+                                                    out.ctypes.data_as(C.c_void_p)), "prefill")
         return out
 
-    def prefill_stage(self, tokens, hidden_in_ptr: int | None, n_tokens: int, pos0: int, logits_out=None, synchronize: bool = False) -> int:
-        """One ubatch through this shard (pb200_prefill_stage); returns the device pointer of the stage's output hidden states."""
+    def prefill_stage(self, tokens, hidden_in_ptr: int | None, n_tokens: int, pos0: int, logits_out=None, synchronize: bool = False,
+                      seq: int = 0) -> int:
+        """One ubatch through this shard into slot seq (pb200_prefill_stage_seq); returns the device pointer of the stage's output hidden
+        states."""
         import numpy as np
         tp = None
         if tokens is not None:
             self._pf_toks = np.ascontiguousarray(tokens, dtype=np.int32)   # kept alive until the (possibly asynchronous) copy has run
             tp = self._pf_toks.ctypes.data_as(C.c_void_p)
         lp = None if logits_out is None else logits_out.ctypes.data_as(C.c_void_p)
-        self.lib.check(self.lib.c.pb200_prefill_stage(self.h, tp, C.c_void_p(hidden_in_ptr) if hidden_in_ptr else None, int(n_tokens), int(pos0), lp,
-                                                      1 if synchronize else 0), "prefill_stage")
+        self.lib.check(self.lib.c.pb200_prefill_stage_seq(self.h, int(seq), tp, C.c_void_p(hidden_in_ptr) if hidden_in_ptr else None, int(n_tokens),
+                                                          int(pos0), lp, 1 if synchronize else 0), "prefill_stage")
         return self.lib.c.pb200_prefill_hidden_device(self.h)
 
     def decode_async(self, token: int, pos: int) -> None:

@@ -95,8 +95,10 @@ class RingRunner:
     The stage object provides: hidden_in / hidden_out (tensors aliasing the engine's buffers), token_in(seq) / token_out(seq)
     (int32[1] tensors: where a returned token lands on stage 0 / where the last stage leaves its sample), begin(seq, token, pos)
     (stage 0: first token of a sequence; other stages: position only) and run(seq) (one step of the slot, sampling included on the
-    last stage), and kv_shift(seq, p0, p1, delta) where shift() is used.  The same class drives CPU tensors over gloo in
-    tests/test_pipeline_gloo.py."""
+    last stage), and kv_shift(seq, p0, p1, delta) where shift() is used.  prefill() also needs prefill_stage(..., seq=) and hidden_buf
+    (as PrefillPipeline drives them) and, on the last stage, sample(seq) (the first token of the slot's logits -> token_out(seq)); copy()
+    needs kv_copy(src, dst, p0, p1).  The same class drives CPU tensors over gloo in tests/test_pipeline_gloo.py and
+    tests/test_ring_prompts_gloo.py."""
 
     def __init__(self, stage, rank: int, world: int, dist, stream=None):
         if world < 2 or dist is None:
@@ -106,6 +108,7 @@ class RingRunner:
         self.t = 0
         self.runs: dict[int, int] = {}                          # runs of each sequence on this rank so far
         self.shifts: dict[int, list[tuple[int, int, int, int]]] = {}
+        self.copies: dict[int, list[tuple[int, int, int, int]]] = {}   # dst -> (at_step, src, p0, p1)
 
     def shift(self, seq: int, at_step: int, p0: int, p1: int, delta: int) -> None:
         """Context shift of sequence seq (prima forwards llama_kv_cache_seq_rm / seq_add down the ring, src/llama.cpp:17946, 18345):
@@ -116,6 +119,40 @@ class RingRunner:
         if at_step < self.runs.get(seq, 0):
             raise ValueError(f"sequence {seq} has already run {self.runs.get(seq, 0)} steps on rank {self.rank}")
         self.shifts.setdefault(seq, []).append((at_step, p0, p1, delta))
+
+    def copy(self, src: int, dst: int, at_step: int, p0: int = -1, p1: int = -1) -> None:
+        """KV copy between sequences (prima's kv_seq_cp ring command, src/llama.cpp:17955): every rank applies
+        stage.kv_copy(src, dst, p0, p1) immediately before its own run number at_step (0-based) of dst, like shift().  Every rank runs the
+        sequences in the same order, so at that point src has also run the same number of steps on every rank.  Call it with the same
+        arguments on every rank, before that run; positions are the caller's (the copy moves none)."""
+        if at_step < self.runs.get(dst, 0):
+            raise ValueError(f"sequence {dst} has already run {self.runs.get(dst, 0)} steps on rank {self.rank}")
+        self.copies.setdefault(dst, []).append((at_step, src, p0, p1))
+
+    def prefill(self, prompts, ubatch: int = 512) -> None:
+        """Starts every sequence from a prompt: call it on every rank with the same prompts (one token list per sequence, world of them)
+        before the first slots(), which then runs without first_tokens.  For each sequence s in turn the prompt goes through the stages in
+        micro-batches into slot s (PrefillPipeline), the last stage samples the first token into token_out(s) (stage.sample(s)) and sends it
+        to stage 0's token_in(s), and every stage sets the slot's position to len(prompts[s]) (begin(s, 0, len)).  On stage 0 the begin is
+        ordered before the receive, so the received token overwrites the placeholder.  One send / recv pair per stage boundary and
+        micro-batch, then one from the last stage to stage 0: each pair's sender finishes its part first, so the exchange cannot
+        deadlock."""
+        if self.t != 0:
+            raise ValueError("prefill() starts the sequences: call it before the first slots()")
+        if len(prompts) != self.world or not all(len(p) for p in prompts):
+            raise ValueError(f"need one non-empty prompt per sequence ({self.world})")
+        st, d, r, N = self.stage, self.dist, self.rank, self.world
+        pipe = PrefillPipeline(st, r, N, d, ubatch=ubatch)
+        with _entered(self.stream):
+            for s, prompt in enumerate(prompts):
+                n = len(prompt)
+                pipe.run(prompt, n, 0, seq=s)
+                st.begin(s, 0, n)
+                if r == N - 1:
+                    st.sample(s)
+                    d.send(st.token_out(s), dst=0)
+                elif r == 0:
+                    d.recv(st.token_in(s), src=N - 1)
 
     def slots(self, n: int, first_tokens=None) -> None:
         """Runs time slots self.t .. self.t + n - 1 (the same n on every rank).  first_tokens[s] = (token, pos) seeds sequence s."""
@@ -150,6 +187,9 @@ class RingRunner:
                 for sh in [s for s in self.shifts.get(sq, ()) if s[0] == done]:
                     st.kv_shift(sq, *sh[1:])
                     self.shifts[sq].remove(sh)
+                for cp in [c for c in self.copies.get(sq, ()) if c[0] == done]:
+                    st.kv_copy(cp[1], sq, *cp[2:])
+                    self.copies[sq].remove(cp)
                 st.run(sq)
                 self.runs[sq] = done + 1
             self.t += 1
@@ -170,9 +210,12 @@ class PrefillPipeline:
             raise ValueError("PrefillPipeline needs world >= 2 and torch.distributed")
         self.stage, self.rank, self.world, self.dist, self.ubatch, self.stream = stage, rank, world, dist, ubatch, stream
 
-    def run(self, tokens, n_tokens: int, pos0: int = 0):
-        """tokens: the prompt's token ids (read on rank 0 only).  Returns the last micro-batch's output of this stage."""
+    def run(self, tokens, n_tokens: int, pos0: int = 0, seq: int = 0):
+        """tokens: the prompt's token ids (read on rank 0 only).  seq: the sequence slot the prompt goes to; it is passed to the stage's
+        prefill_stage as the keyword seq only when it is not 0, so a stage that only serves slot 0 keeps its four-argument method.  Returns
+        the last micro-batch's output of this stage."""
         st, d, r = self.stage, self.dist, self.rank
+        kw = {"seq": seq} if seq else {}
         out = None
         with _entered(self.stream):
             for j0 in range(0, n_tokens, self.ubatch):
@@ -181,7 +224,7 @@ class PrefillPipeline:
                 if r > 0:
                     hin = st.hidden_buf[:n]
                     d.recv(hin, src=r - 1)
-                out = st.prefill_stage(tokens[j0:j0 + n] if r == 0 else None, hin, n, pos0 + j0)
+                out = st.prefill_stage(tokens[j0:j0 + n] if r == 0 else None, hin, n, pos0 + j0, **kw)
                 if r < self.world - 1:
                     d.send(out, dst=r + 1)
         return out
