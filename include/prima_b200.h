@@ -196,6 +196,19 @@ PB200_API int pb200_penalty_accept(void * state_dev, const int32_t * tokens_dev,
 PB200_API int pb200_penalty_apply(const float * logits, int n_vocab, const void * state_dev, float * out, void * stream);
 /* All three only enqueue on stream: no host synchronisation, no allocation, capturable in a CUDA graph. */
 
+/* ---- scoring of prompt logits: llama-perplexity's log_softmax per scored position (examples/perplexity/perplexity.cpp:106-116, 155-188).
+ * For each row r of logits[n_rows][n_vocab] (device) and tok = targets_dev[r]:
+ *   top   = the first index of the row's maximum max;
+ *   sum   = the sum over the row of expf(l - max), each term the accurate f32 expf of an f32 difference, accumulated in double (in another
+ *           order than the reference's serial loop: a double-rounding difference only);
+ *   nll   = max + log(sum) - logit[tok] in double (the reference's -log_softmax), logit = logits[tok], prob = expf(logit - max) / (float) sum.
+ * A target outside [0, n_vocab) leaves the row unscored: nll, logit and prob are 0, top is still written.  Rows must hold at least one
+ * finite logit; -inf entries are allowed, and a -inf target gives nll = +inf, prob = 0.  One launch of n_rows CTAs (n_vocab up to at least
+ * 262 144), enqueue-only: no host synchronisation, no allocation. */
+typedef struct pb200_token_score { double nll; float logit, prob; int32_t top, _pad; } pb200_token_score;   /* 24 bytes */
+PB200_API int pb200_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets_dev, pb200_token_score * out_dev,
+                                 void * stream);
+
 /* ---- fused decode launches (what the engine is made of), for graph-level fusion in a host such as the ggml-backend plugin ---- */
 typedef struct pb200_gemv_mat {
     int32_t type;          /* k-quant type of W (Q4_K / Q5_K / Q6_K) */
@@ -304,6 +317,21 @@ PB200_API int pb200_prefill_seq(pb200_model * m, int seq, const int32_t * tokens
 PB200_API int pb200_prefill_stage_seq(pb200_model * m, int seq, const int32_t * tokens_host, const float * hidden_in_dev, int32_t n_tokens, int32_t pos0,
                                       float * logits_host, int32_t synchronize);
 PB200_API float * pb200_prefill_hidden_device(pb200_model * m);
+/* Logits of any rows of the last prompt ubatch — the reference's batch.logits[i] flags, which become inp_out_ids and select the rows that
+ * reach output_norm and the head (src/llama.cpp:10831-10835, 11120-11125); llama-perplexity sets them for every scored position
+ * (examples/perplexity/perplexity.cpp:475-687).  Rows [row0, row0 + n_rows) of the hidden states the last pb200_prefill* call left at
+ * pb200_prefill_hidden_device(m) (its last ubatch, at most 512 rows, whatever the slot) go through output_norm and output into a grow-only
+ * device buffer [n_rows][n_vocab]: with a k-quant head and n_rows >= 8 one tensor-core mat-mul with the rms-norm fused into its activation
+ * pass (pb200_mul_mat_q's numerics), otherwise the rms-norm kernel and then the mat-mul's own fallbacks (another mmq type, or the decode GEMV
+ * row by row below 8 rows).
+ *   - targets_host (optional, n_rows ids): also scores the rows with pb200_token_scores; a negative target leaves its row unscored.
+ *   - logits_host (optional) receives [n_rows][n_vocab] f32, scores_host (optional, needs targets_host) n_rows scores.  The call
+ *     synchronises the model stream; a watchdog abort returns PB200_EABORTED like pb200_prefill.
+ *   - NULL or unfinalized model, or a shard without the head: PB200_ESTATE.  PB200_EINVAL: no prefill yet on this model, row0 < 0,
+ *     n_rows <= 0 or row0 + n_rows past the last ubatch, both outputs NULL, scores_host without targets_host, a target >= n_vocab.
+ *   - Writes nothing that decode or prefill reads: not hidden_out, pb200_logits_device, the KV cache or any slot's words. */
+PB200_API int pb200_prompt_head(pb200_model * m, int32_t row0, int32_t n_rows, const int32_t * targets_host, float * logits_host,
+                                pb200_token_score * scores_host);
 PB200_API int pb200_kv_clear(pb200_model * m);
 /* prima's context shift on this shard's cache for slot seq (what llama-cli does when the context fills, examples/main/main.cpp:578-608):
  *   llama_kv_cache_seq_rm(seq, p0 + delta, p0) + llama_kv_cache_seq_add(seq, p0, p1, delta)

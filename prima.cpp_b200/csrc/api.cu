@@ -308,4 +308,11 @@ int pb200_penalty_apply(const float * logits, int n_vocab, const void * state_de
     return rc;
 }
 
+int pb200_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets_dev, pb200_token_score * out_dev, void * stream) {
+    if (!logits || !targets_dev || !out_dev || n_rows <= 0 || n_rows > INT32_MAX || n_vocab <= 0) return PB200_EINVAL;
+    const int rc = launch_token_scores(logits, n_rows, n_vocab, targets_dev, out_dev, (cudaStream_t) stream);
+    if (rc == 0) g_launches++;
+    return rc;
+}
+
 }  // extern "C"

@@ -131,12 +131,14 @@ struct pb200_model {
     std::vector<Slot> slots;           // [n_seq], from finalize on
     DevBuf pen_logits;                 // [n_vocab] the penalised row the chain reads (one for all slots: they share the stream)
     DevBuf pen_tok;                    // staging of pb200_sampler_accept_seq
+    DevBuf head;                       // pb200_prompt_head: logits [n_rows][n_vocab] | targets [n_rows] | scores [n_rows]
     uint64_t launches_per_step = 0;
     int64_t weight_bytes = 0;
     std::vector<void *> allocs;
     bool profiling = false;
     struct Prefill {                   // prompt-processing scratch for up to T tokens: one block, grown on demand
         int T = 0;
+        int rows = 0;                  // tokens of the last ubatch, whose hidden states x0 holds (0: no prefill yet)
         DevBuf mem;
         float *x0 = nullptr, *x1 = nullptr, *xn = nullptr, *q = nullptr, *k = nullptr, *v = nullptr, *att = nullptr, *g = nullptr, *u = nullptr;
         void * ws = nullptr;
@@ -688,6 +690,44 @@ extern "C" int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host,
 }
 extern "C" float * pb200_prefill_hidden_device(pb200_model * m) { return (m && m->finalized) ? m->pf.x0 : nullptr; }
 
+// The head over rows [row0, row0 + n_rows) of the last ubatch (the reference's inp_out_ids rows, src/llama.cpp:11120-11125): output_norm
+// rides in the tensor-core mat-mul's activation pass like q|k|v's attn_norm, or runs first where pf_matmul takes a fallback.  Reads x0,
+// writes only the head buffer and the prefill scratch (xn, ws, actF), which every prefill and decode rewrites before reading.
+extern "C" int pb200_prompt_head(pb200_model * m, int32_t row0, int32_t n_rows, const int32_t * targets_host, float * logits_host,
+                                 pb200_token_score * scores_host) {
+    CK(ready(m, true));
+    pb200_model::Prefill & P = m->pf;
+    if (P.rows == 0 || row0 < 0 || n_rows <= 0 || row0 > P.rows - n_rows) return PB200_EINVAL;
+    if ((!logits_host && !scores_host) || (scores_host && !targets_host)) return PB200_EINVAL;
+    const pb200_hparams & hp = m->hp;
+    const int E = hp.n_embd, V = hp.n_vocab;
+    if (targets_host)
+        for (int32_t i = 0; i < n_rows; i++)
+            if (targets_host[i] >= V) return PB200_EINVAL;
+    cudaStream_t st = m->stream;
+    const size_t lg_bytes = ((size_t) n_rows * V * 4 + 255) / 256 * 256, tg_bytes = ((size_t) n_rows * 4 + 255) / 256 * 256;
+    CK(m->head.grow(lg_bytes + tg_bytes + (size_t) n_rows * sizeof(pb200_token_score), st));
+    float * lg = (float *) m->head.p;
+    int32_t * tg = (int32_t *) ((char *) m->head.p + lg_bytes);
+    pb200_token_score * sc = (pb200_token_score *) ((char *) m->head.p + lg_bytes + tg_bytes);
+    uint64_t n = 0;
+    const float * x = P.x0 + (size_t) row0 * E;
+    const bool fused = pf_tc(m->output, n_rows) && is_kquant(m->output.type);
+    const MmqPre output_norm{PRO_RMSNORM, m->output_norm, 0, hp.rms_eps};
+    if (!fused) { CK(launch_rms_norm(x, P.xn, E, n_rows, hp.rms_eps, st, m->output_norm)); n++; }
+    CK(pf_matmul(m, m->output, fused ? x : P.xn, n_rows, lg, nullptr, nullptr, n, nullptr, fused ? &output_norm : nullptr));
+    if (targets_host) {
+        // from pageable memory the copy returns once the ids are staged; stream order keeps them until the scores have read them
+        CK(cudaMemcpyAsync(tg, targets_host, (size_t) n_rows * 4, cudaMemcpyHostToDevice, st));
+        CK(launch_token_scores(lg, n_rows, V, tg, sc, st)); n++;
+    }
+    g_launches += n;
+    if (logits_host) CK(cudaMemcpyAsync(logits_host, lg, (size_t) n_rows * V * 4, cudaMemcpyDeviceToHost, st));
+    if (scores_host) CK(cudaMemcpyAsync(scores_host, sc, (size_t) n_rows * sizeof(pb200_token_score), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return check_clear_abort() ? PB200_EABORTED : 0;   // a kernel's wait watchdog gave up: these rows are invalid (flag re-armed)
+}
+
 // the callers have checked the model, seq, T, pos0 and which input is given; the prompt's K/V rows go to slot seq.  The scratch, x_out and
 // the logits are shared by all slots: every call is ordered on the model stream.
 static int prefill_ubatch(pb200_model * m, int seq, const int32_t * tokens_host, const float * hidden_in_dev, int32_t T, int32_t pos0, float * logits_host,
@@ -751,6 +791,7 @@ static int prefill_ubatch(pb200_model * m, int seq, const int32_t * tokens_host,
         GemvDesc d1 = {m->output.data, m->logits, nullptr, nullptr, m->output.type, hp.n_vocab};
         CK(launch_gemv(&d1, 1, E, m->actE.q, GemvPrologue{PRO_RMSNORM, m->x_out, m->output_norm, hp.rms_eps}, st, false, n));
     }
+    P.rows = T;
     g_launches += n;
     if (!sync) return 0;
     if (m->with_head && logits_host) CK(cudaMemcpyAsync(m->logits_host, m->logits, (size_t) hp.n_vocab * 4, cudaMemcpyDeviceToHost, st));

@@ -205,6 +205,9 @@ bool penalties_ok(const pb200_penalties * p);   // repeat finite and > 0, freq /
 int launch_penalty_init(void * state, int n_vocab, const pb200_penalties & p, cudaStream_t stream, uint64_t & nlaunch);
 int launch_penalize(const float * x, int n, const void * state, float * out, cudaStream_t stream, bool pdl);
 int launch_penalty_accept(void * state, const int32_t * tokens, int n, cudaStream_t stream, bool pdl);
+// per-row scores of logits[n_rows][n_vocab] against targets[n_rows] (device) -> out[n_rows] (sample.cu, k_token_scores): one launch of
+// n_rows CTAs (n_rows <= INT32_MAX)
+int launch_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets, pb200_token_score * out, cudaStream_t stream);
 
 // element-wise helpers for the plugin
 int launch_binary(int op /*0 add, 1 mul*/, const float * a, const float * b, float * y, int64_t n, int64_t nb /*b broadcast period*/, cudaStream_t stream);

@@ -433,7 +433,64 @@ __global__ void k_penalty_accept(PenHdr * st, const int32_t * __restrict__ tok, 
     if (threadIdx.x == 0) { st->pos = (pos + m) % L; st->count = min(count + m, L); }
 }
 
+// ---- scoring of prompt logits: llama-perplexity's log_softmax (examples/perplexity/perplexity.cpp:106-116), one CTA per row ----
+constexpr int TS_NT = 512;
+
+__global__ void __launch_bounds__(TS_NT) k_token_scores(const float * __restrict__ logits, int n_vocab, const int32_t * __restrict__ targets,
+                                                         pb200_token_score * __restrict__ out) {
+    __shared__ float s_max[TS_NT / 32];
+    __shared__ int s_top[TS_NT / 32];
+    __shared__ double s_sum[TS_NT / 32];
+    const int64_t r = blockIdx.x;
+    const float * x = logits + r * n_vocab;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    // max and the first index of the maximum (ascending i per thread, strict '>': the first occurrence; -inf and NaN never win)
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) {
+        const float v = x[i];
+        if (v > best) { best = v; bi = i; }
+    }
+    warp_argmax(best, bi);
+    if (lane == 0) { s_max[warp] = best; s_top[warp] = bi; }
+    __syncthreads();
+    if (warp == 0) {
+        best = lane < TS_NT / 32 ? s_max[lane] : -INFINITY;
+        bi = lane < TS_NT / 32 ? s_top[lane] : 0x7fffffff;
+        warp_argmax(best, bi);
+        if (lane == 0) { s_max[0] = best; s_top[0] = bi; }   // every lane has read its slot: warp_argmax's shuffles order them
+    }
+    __syncthreads();
+    const float mx = s_max[0];
+    // sum of expf(l - max): each term the accurate f32 expf of an f32 difference, as the reference computes it, summed in double
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) s += (double) expf(x[i] - mx);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) s_sum[warp] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double sum = 0.0;
+        for (int w = 0; w < TS_NT / 32; w++) sum += s_sum[w];
+        pb200_token_score o{};
+        o.top = s_top[0];
+        const int tok = targets[r];
+        if (tok >= 0 && tok < n_vocab) {               // otherwise the row is not scored: nll, logit and prob stay 0
+            const float l = x[tok];
+            o.logit = l;
+            o.nll = (double) mx + log(sum) - (double) l;
+            o.prob = __fdiv_rn(expf(l - mx), (float) sum);
+        }
+        out[r] = o;
+    }
+}
+
 }  // namespace
+
+int launch_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets, pb200_token_score * out, cudaStream_t stream) {
+    k_token_scores<<<(unsigned) n_rows, TS_NT, 0, stream>>>(logits, n_vocab, targets, out);
+    return (int) cudaGetLastError();
+}
 
 size_t penalty_state_bytes(int last_n, int n_bias) {
     return (sizeof(PenHdr) + (size_t) std::max(n_bias, 0) * sizeof(pb200_logit_bias) + (size_t) std::max(last_n, 0) * 4 + 255) / 256 * 256;

@@ -68,6 +68,12 @@ def penalties(last_n: int = 64, repeat: float = 1.0, freq: float = 0.0, present:
     return p
 
 
+class TokenScore(C.Structure):
+    """pb200_token_score: llama-perplexity's log_softmax of one scored position (nll = -log p(target), the target's logit and
+    probability, the first index of the row's maximum)."""
+    _fields_ = [("nll", C.c_double), ("logit", C.c_float), ("prob", C.c_float), ("top", C.c_int32), ("_pad", C.c_int32)]
+
+
 class Pb200Error(RuntimeError):
     pass
 
@@ -163,6 +169,8 @@ class Lib:
         c.pb200_penalty_apply.argtypes = [vp, C.c_int, vp, vp, vp]
         c.pb200_penalties_set_seq.argtypes = [vp, C.c_int, C.POINTER(Penalties)]
         c.pb200_sampler_accept_seq.argtypes = [vp, C.c_int, vp, C.c_int]
+        c.pb200_token_scores.argtypes = [vp, i64, C.c_int, vp, vp, vp]
+        c.pb200_prompt_head.argtypes = [vp, i32, i32, vp, vp, vp]
 
     @classmethod
     def get(cls) -> "Lib":
@@ -201,6 +209,11 @@ class Lib:
         """out = the row with logit bias and penalties applied (a copy; out must not alias logits)."""
         self.check(self.c.pb200_penalty_apply(C.c_void_p(logits_ptr), n_vocab, C.c_void_p(state_ptr), C.c_void_p(out_ptr), C.c_void_p(stream)),
                    "penalty_apply")
+
+    def token_scores(self, logits_ptr: int, n_rows: int, n_vocab: int, targets_ptr: int, out_ptr: int, stream: int = 0) -> None:
+        """pb200_token_scores: one TokenScore per row of the device logits [n_rows][n_vocab] against the int32 device targets (enqueued)."""
+        self.check(self.c.pb200_token_scores(C.c_void_p(logits_ptr), n_rows, n_vocab, C.c_void_p(targets_ptr), C.c_void_p(out_ptr),
+                                             C.c_void_p(stream)), "token_scores")
 
 
 class Model:
@@ -295,6 +308,23 @@ class Model:
         self.lib.check(self.lib.c.pb200_prefill_stage_seq(self.h, int(seq), tp, C.c_void_p(hidden_in_ptr) if hidden_in_ptr else None, int(n_tokens),
                                                           int(pos0), lp, 1 if synchronize else 0), "prefill_stage")
         return self.lib.c.pb200_prefill_hidden_device(self.h)
+
+    def prompt_head(self, row0: int, n: int, targets=None, logits: bool = True):
+        """pb200_prompt_head: rows [row0, row0 + n) of the last prompt ubatch through output_norm and the head.  Returns (logits [n][n_vocab]
+        f32 or None, scores or None): with targets (n ids; negative: unscored) a numpy array of TokenScore records (fields nll, logit,
+        prob, top)."""
+        import numpy as np
+        lg = np.empty((n, self.hp.n_vocab), dtype=np.float32) if logits else None
+        tg = sc = None
+        if targets is not None:
+            tg = np.ascontiguousarray(targets, dtype=np.int32)
+            if tg.shape != (n,):
+                raise ValueError(f"need {n} targets, got shape {tg.shape}")
+            sc = np.zeros(n, dtype=np.dtype(TokenScore))
+        def p(a):
+            return None if a is None else a.ctypes.data_as(C.c_void_p)
+        self.lib.check(self.lib.c.pb200_prompt_head(self.h, int(row0), int(n), p(tg), p(lg), p(sc)), "prompt_head")
+        return lg, sc
 
     def decode_async(self, token: int, pos: int) -> None:
         self.lib.check(self.lib.c.pb200_decode_async(self.h, token, pos), "decode_async")

@@ -210,9 +210,11 @@ class PrefillPipeline:
             raise ValueError("PrefillPipeline needs world >= 2 and torch.distributed")
         self.stage, self.rank, self.world, self.dist, self.ubatch, self.stream = stage, rank, world, dist, ubatch, stream
 
-    def run(self, tokens, n_tokens: int, pos0: int = 0, seq: int = 0):
+    def run(self, tokens, n_tokens: int, pos0: int = 0, seq: int = 0, outputs=None):
         """tokens: the prompt's token ids (read on rank 0 only).  seq: the sequence slot the prompt goes to; it is passed to the stage's
-        prefill_stage as the keyword seq only when it is not 0, so a stage that only serves slot 0 keeps its four-argument method.  Returns
+        prefill_stage as the keyword seq only when it is not 0, so a stage that only serves slot 0 keeps its four-argument method.
+        outputs(j0, n): called on the last rank only, right after micro-batch [j0, j0 + n)'s prefill_stage and before the next one, while
+        the stage's output hidden states still hold that micro-batch (Model.prompt_head reads them: the logits of any of its rows).  Returns
         the last micro-batch's output of this stage."""
         st, d, r = self.stage, self.dist, self.rank
         kw = {"seq": seq} if seq else {}
@@ -225,6 +227,8 @@ class PrefillPipeline:
                     hin = st.hidden_buf[:n]
                     d.recv(hin, src=r - 1)
                 out = st.prefill_stage(tokens[j0:j0 + n] if r == 0 else None, hin, n, pos0 + j0, **kw)
+                if outputs is not None and r == self.world - 1:
+                    outputs(j0, n)
                 if r < self.world - 1:
                     d.send(out, dst=r + 1)
         return out
