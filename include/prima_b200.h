@@ -209,6 +209,33 @@ typedef struct pb200_token_score { double nll; float logit, prob; int32_t top, _
 PB200_API int pb200_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets_dev, pb200_token_score * out_dev,
                                  void * stream);
 
+/* ---- KL-divergence against a base model: llama-perplexity --kl-divergence-base FILE / --kl-divergence (examples/perplexity/perplexity.cpp).
+ * Record: what the reference's writer log_softmax(n_vocab, logits, uint16_t *, tok) (:118-153) stores per scored position in the base
+ * file, nv = pb200_logprob_record_u16s(n_vocab) = 2*((n_vocab+1)/2) + 4 uint16:
+ *   { f32 scale, f32 min_log_prob, uint16 q[n_vocab], uint16 0 when n_vocab is odd }, a log-probability being scale * q + min_log_prob.
+ * pb200_logprobs_u16 writes row r's record at records_dev + r * nv (4-byte aligned), in the reference's order and roundings (no contraction):
+ *   min_logit = max(min, max - 16);  sum = the double sum of expf(l - max) (pb200_token_scores' sum);  lse = (float) log(sum);
+ *   min_log_prob = min_logit - max - lse;  scale = (max - min_logit) / 65535.f;
+ *   q[i] = l > min_logit ? nearest_int((1 / scale) * (l - min_logit)) : 0 (the reference's +12582912.f rounding), all 0 when scale == 0;
+ *   nll_dev[r] (optional, needs targets_dev) = max + lse - logit[tok] in float: the value the reference sums in this mode.
+ * For the same f32 row, scale and every q are bit-identical to the reference; min_log_prob and nll may differ in the last bit, as the
+ * double sum runs in another order than the reference's serial loop (and the double log is CUDA's, within 1 ulp).
+ * pb200_kld_scores is the reference's log_softmax(n_vocab, logits, base_log_prob, tok, kld) (:237-296) per row against base record
+ * base_dev + r * nv:
+ *   nll = max + lse - logit[tok], nll_base = -(scale * q[tok] + min_log_prob), p_diff = expf(-nll) - expf(-nll_base) (all float);
+ *   kld = the sum, over the entries whose base log-probability p_log_base = scale * q[i] + min_log_prob is above -16, of the float product
+ *         expf(p_log_base) * (p_log_base - l[i] + max + lse), accumulated in double;
+ *   same_top = the first index of the row's maximum equals the first index of the base's maximum log-probability.
+ * Its float fields may differ from the reference's by a few ulp (CUDA's expf is within 2 ulp of glibc's), kld by about 2^-23 of the sum of
+ * its terms' magnitudes.  In both calls a target outside [0, n_vocab) zeroes what depends on it (nll; nll, nll_base, p_diff).  Rows must
+ * hold at least one finite logit.  One launch of n_rows CTAs each, enqueue-only: no host synchronisation, no allocation. */
+typedef struct pb200_kld_score { double kld; float nll, nll_base, p_diff; int32_t same_top; } pb200_kld_score;   /* 24 bytes */
+PB200_API int pb200_logprob_record_u16s(int n_vocab);   /* nv, or 0 for n_vocab <= 0 */
+PB200_API int pb200_logprobs_u16(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets_dev, uint16_t * records_dev,
+                                 float * nll_dev, void * stream);
+PB200_API int pb200_kld_scores(const float * logits, int64_t n_rows, int n_vocab, const uint16_t * base_dev, const int32_t * targets_dev,
+                               pb200_kld_score * out_dev, void * stream);
+
 /* ---- fused decode launches (what the engine is made of), for graph-level fusion in a host such as the ggml-backend plugin ---- */
 typedef struct pb200_gemv_mat {
     int32_t type;          /* k-quant type of W (Q4_K / Q5_K / Q6_K) */
@@ -332,6 +359,17 @@ PB200_API float * pb200_prefill_hidden_device(pb200_model * m);
  *   - Writes nothing that decode or prefill reads: not hidden_out, pb200_logits_device, the KV cache or any slot's words. */
 PB200_API int pb200_prompt_head(pb200_model * m, int32_t row0, int32_t n_rows, const int32_t * targets_host, float * logits_host,
                                 pb200_token_score * scores_host);
+/* llama-perplexity's two KL-divergence modes on the same rows and the same head computation as pb200_prompt_head (its logits bit for bit),
+ * with targets_host (n_rows ids in [0, n_vocab), required):
+ *   - writer (--kl-divergence-base): records_host receives the rows' n_rows * nv records (pb200_logprobs_u16), nll_host (optional, needs
+ *     records_host) their n_rows float nll;
+ *   - compare (--kl-divergence): base_host holds n_rows * nv base records, kld_host receives n_rows pb200_kld_scores against them.
+ * Either mode or both in one call.  Only the records and the 24-byte scores cross PCIe, never the logits.  Codes in pb200_prompt_head's
+ * order: PB200_ESTATE for a NULL or unfinalized model or a shard without the head; PB200_EINVAL for a bad row range, no output, nll_host
+ * without records_host, base_host without kld_host or the other way round, a missing target or one outside [0, n_vocab).  Synchronises the
+ * model stream (PB200_EABORTED on a watchdog abort) and writes nothing that decode or prefill reads. */
+PB200_API int pb200_prompt_head_kld(pb200_model * m, int32_t row0, int32_t n_rows, const int32_t * targets_host, uint16_t * records_host,
+                                    float * nll_host, const uint16_t * base_host, pb200_kld_score * kld_host);
 PB200_API int pb200_kv_clear(pb200_model * m);
 /* prima's context shift on this shard's cache for slot seq (what llama-cli does when the context fills, examples/main/main.cpp:578-608):
  *   llama_kv_cache_seq_rm(seq, p0 + delta, p0) + llama_kv_cache_seq_add(seq, p0, p1, delta)

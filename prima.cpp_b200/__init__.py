@@ -5,6 +5,6 @@ The product is ``libprima_b200.so`` (CUDA kernels + C++ decode engine, ``include
 This Python package is only the thin ctypes binding used by tests and bench.py; it never falls back to a CPU
 path: importing :mod:`host` raises if the CUDA library is missing.
 """
-from .host import Lib, Model, HParams, Sampling, sampling, Penalties, LogitBias, penalties, Pb200Error, TokenScore, lib_path, build, TYPES  # noqa: F401
+from .host import Lib, Model, HParams, Sampling, sampling, Penalties, LogitBias, penalties, Pb200Error, TokenScore, KldScore, record_u16s, lib_path, build, TYPES  # noqa: F401
 from .pipeline import PipelineRunner, RingRunner, PrefillPipeline, layer_windows  # noqa: F401
 from . import perplexity  # noqa: F401

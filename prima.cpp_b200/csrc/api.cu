@@ -315,4 +315,26 @@ int pb200_token_scores(const float * logits, int64_t n_rows, int n_vocab, const 
     return rc;
 }
 
+int pb200_logprob_record_u16s(int n_vocab) { return n_vocab > 0 && n_vocab <= INT32_MAX - 5 ? 2 * ((n_vocab + 1) / 2) + 4 : 0; }
+
+int pb200_logprobs_u16(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets_dev, uint16_t * records_dev, float * nll_dev,
+                       void * stream) {
+    if (!logits || !records_dev || (nll_dev && !targets_dev) || n_rows <= 0 || n_rows > INT32_MAX || pb200_logprob_record_u16s(n_vocab) == 0 ||
+        ((uintptr_t) records_dev & 3))
+        return PB200_EINVAL;
+    const int rc = launch_logprobs_u16(logits, n_rows, n_vocab, targets_dev, records_dev, nll_dev, (cudaStream_t) stream);
+    if (rc == 0) g_launches++;
+    return rc;
+}
+
+int pb200_kld_scores(const float * logits, int64_t n_rows, int n_vocab, const uint16_t * base_dev, const int32_t * targets_dev,
+                     pb200_kld_score * out_dev, void * stream) {
+    if (!logits || !base_dev || !targets_dev || !out_dev || n_rows <= 0 || n_rows > INT32_MAX || pb200_logprob_record_u16s(n_vocab) == 0 ||
+        ((uintptr_t) base_dev & 3))
+        return PB200_EINVAL;
+    const int rc = launch_kld_scores(logits, n_rows, n_vocab, base_dev, targets_dev, out_dev, (cudaStream_t) stream);
+    if (rc == 0) g_launches++;
+    return rc;
+}
+
 }  // extern "C"

@@ -131,7 +131,7 @@ struct pb200_model {
     std::vector<Slot> slots;           // [n_seq], from finalize on
     DevBuf pen_logits;                 // [n_vocab] the penalised row the chain reads (one for all slots: they share the stream)
     DevBuf pen_tok;                    // staging of pb200_sampler_accept_seq
-    DevBuf head;                       // pb200_prompt_head: logits [n_rows][n_vocab] | targets [n_rows] | scores [n_rows]
+    DevBuf head;                       // pb200_prompt_head(_kld): logits [n_rows][n_vocab] | that call's per-row data (head_rows)
     uint64_t launches_per_step = 0;
     int64_t weight_bytes = 0;
     std::vector<void *> allocs;
@@ -690,32 +690,51 @@ extern "C" int pb200_prefill_stage(pb200_model * m, const int32_t * tokens_host,
 }
 extern "C" float * pb200_prefill_hidden_device(pb200_model * m) { return (m && m->finalized) ? m->pf.x0 : nullptr; }
 
+// Rows [row0, row0 + n_rows) of the last ubatch: PB200_EINVAL when there is no prefill yet or the range leaves it.
+static int head_range(const pb200_model * m, int32_t row0, int32_t n_rows) {
+    const int rows = m->pf.rows;
+    return rows == 0 || row0 < 0 || n_rows <= 0 || row0 > rows - n_rows ? PB200_EINVAL : 0;
+}
+
+static size_t round256(size_t b) { return (b + 255) / 256 * 256; }
+
 // The head over rows [row0, row0 + n_rows) of the last ubatch (the reference's inp_out_ids rows, src/llama.cpp:11120-11125): output_norm
 // rides in the tensor-core mat-mul's activation pass like q|k|v's attn_norm, or runs first where pf_matmul takes a fallback.  Reads x0,
-// writes only the head buffer and the prefill scratch (xn, ws, actF), which every prefill and decode rewrites before reading.
+// writes only the head buffer and the prefill scratch (xn, ws, actF), which every prefill and decode rewrites before reading.  The head
+// buffer grows to the logits [n_rows][n_vocab] (256-byte rounded) and `extra` bytes after them, for the caller's per-row data; lg and ex
+// point at both.  Enqueued on the model stream; n counts the launches.  The caller has checked the model and the rows.
+static int head_rows(pb200_model * m, int32_t row0, int32_t n_rows, size_t extra, float *& lg, char *& ex, uint64_t & n) {
+    pb200_model::Prefill & P = m->pf;
+    const pb200_hparams & hp = m->hp;
+    const int E = hp.n_embd;
+    const size_t lg_bytes = round256((size_t) n_rows * hp.n_vocab * 4);
+    CK(m->head.grow(lg_bytes + extra, m->stream));
+    lg = (float *) m->head.p;
+    ex = (char *) m->head.p + lg_bytes;
+    const float * x = P.x0 + (size_t) row0 * E;
+    const bool fused = pf_tc(m->output, n_rows) && is_kquant(m->output.type);
+    const MmqPre output_norm{PRO_RMSNORM, m->output_norm, 0, hp.rms_eps};
+    if (!fused) { CK(launch_rms_norm(x, P.xn, E, n_rows, hp.rms_eps, m->stream, m->output_norm)); n++; }
+    return pf_matmul(m, m->output, fused ? x : P.xn, n_rows, lg, nullptr, nullptr, n, nullptr, fused ? &output_norm : nullptr);
+}
+
 extern "C" int pb200_prompt_head(pb200_model * m, int32_t row0, int32_t n_rows, const int32_t * targets_host, float * logits_host,
                                  pb200_token_score * scores_host) {
     CK(ready(m, true));
-    pb200_model::Prefill & P = m->pf;
-    if (P.rows == 0 || row0 < 0 || n_rows <= 0 || row0 > P.rows - n_rows) return PB200_EINVAL;
+    CK(head_range(m, row0, n_rows));
     if ((!logits_host && !scores_host) || (scores_host && !targets_host)) return PB200_EINVAL;
-    const pb200_hparams & hp = m->hp;
-    const int E = hp.n_embd, V = hp.n_vocab;
+    const int V = m->hp.n_vocab;
     if (targets_host)
         for (int32_t i = 0; i < n_rows; i++)
             if (targets_host[i] >= V) return PB200_EINVAL;
     cudaStream_t st = m->stream;
-    const size_t lg_bytes = ((size_t) n_rows * V * 4 + 255) / 256 * 256, tg_bytes = ((size_t) n_rows * 4 + 255) / 256 * 256;
-    CK(m->head.grow(lg_bytes + tg_bytes + (size_t) n_rows * sizeof(pb200_token_score), st));
-    float * lg = (float *) m->head.p;
-    int32_t * tg = (int32_t *) ((char *) m->head.p + lg_bytes);
-    pb200_token_score * sc = (pb200_token_score *) ((char *) m->head.p + lg_bytes + tg_bytes);
+    const size_t tg_bytes = round256((size_t) n_rows * 4);
+    float * lg;
+    char * ex;
     uint64_t n = 0;
-    const float * x = P.x0 + (size_t) row0 * E;
-    const bool fused = pf_tc(m->output, n_rows) && is_kquant(m->output.type);
-    const MmqPre output_norm{PRO_RMSNORM, m->output_norm, 0, hp.rms_eps};
-    if (!fused) { CK(launch_rms_norm(x, P.xn, E, n_rows, hp.rms_eps, st, m->output_norm)); n++; }
-    CK(pf_matmul(m, m->output, fused ? x : P.xn, n_rows, lg, nullptr, nullptr, n, nullptr, fused ? &output_norm : nullptr));
+    CK(head_rows(m, row0, n_rows, tg_bytes + (size_t) n_rows * sizeof(pb200_token_score), lg, ex, n));
+    int32_t * tg = (int32_t *) ex;
+    pb200_token_score * sc = (pb200_token_score *) (ex + tg_bytes);
     if (targets_host) {
         // from pageable memory the copy returns once the ids are staged; stream order keeps them until the scores have read them
         CK(cudaMemcpyAsync(tg, targets_host, (size_t) n_rows * 4, cudaMemcpyHostToDevice, st));
@@ -726,6 +745,43 @@ extern "C" int pb200_prompt_head(pb200_model * m, int32_t row0, int32_t n_rows, 
     if (scores_host) CK(cudaMemcpyAsync(scores_host, sc, (size_t) n_rows * sizeof(pb200_token_score), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return check_clear_abort() ? PB200_EABORTED : 0;   // a kernel's wait watchdog gave up: these rows are invalid (flag re-armed)
+}
+
+// The same rows' u16 log-probability records (llama-perplexity --kl-divergence-base) and / or their KL-divergence against base records
+// (--kl-divergence), from one head computation.  Only the records and the per-row results cross PCIe.
+extern "C" int pb200_prompt_head_kld(pb200_model * m, int32_t row0, int32_t n_rows, const int32_t * targets_host, uint16_t * records_host,
+                                     float * nll_host, const uint16_t * base_host, pb200_kld_score * kld_host) {
+    CK(ready(m, true));
+    CK(head_range(m, row0, n_rows));
+    if ((!records_host && !kld_host) || (nll_host && !records_host) || (!base_host != !kld_host) || !targets_host) return PB200_EINVAL;
+    const int V = m->hp.n_vocab;
+    for (int32_t i = 0; i < n_rows; i++)
+        if (targets_host[i] < 0 || targets_host[i] >= V) return PB200_EINVAL;
+    cudaStream_t st = m->stream;
+    const size_t rec_bytes = (size_t) n_rows * pb200_logprob_record_u16s(V) * 2;
+    // after the logits: targets | the records written | the base records read | nll | KLD scores, each 256-byte aligned
+    const size_t tg_b = round256((size_t) n_rows * 4), rec_b = records_host ? round256(rec_bytes) : 0, base_b = base_host ? round256(rec_bytes) : 0,
+                 nll_b = nll_host ? round256((size_t) n_rows * 4) : 0, kld_b = kld_host ? (size_t) n_rows * sizeof(pb200_kld_score) : 0;
+    float * lg;
+    char * ex;
+    uint64_t n = 0;
+    CK(head_rows(m, row0, n_rows, tg_b + rec_b + base_b + nll_b + kld_b, lg, ex, n));
+    int32_t * tg = (int32_t *) ex;
+    uint16_t * rec = (uint16_t *) (ex + tg_b);
+    uint16_t * base = (uint16_t *) (ex + tg_b + rec_b);
+    float * nll = nll_host ? (float *) (ex + tg_b + rec_b + base_b) : nullptr;
+    pb200_kld_score * kld = (pb200_kld_score *) (ex + tg_b + rec_b + base_b + nll_b);
+    // from pageable memory the copies return once staged; stream order keeps them until the kernels have read them
+    CK(cudaMemcpyAsync(tg, targets_host, (size_t) n_rows * 4, cudaMemcpyHostToDevice, st));
+    if (base_host) CK(cudaMemcpyAsync(base, base_host, rec_bytes, cudaMemcpyHostToDevice, st));
+    if (records_host) { CK(launch_logprobs_u16(lg, n_rows, V, tg, rec, nll, st)); n++; }
+    if (kld_host) { CK(launch_kld_scores(lg, n_rows, V, base, tg, kld, st)); n++; }
+    g_launches += n;
+    if (records_host) CK(cudaMemcpyAsync(records_host, rec, rec_bytes, cudaMemcpyDeviceToHost, st));
+    if (nll_host) CK(cudaMemcpyAsync(nll_host, nll, (size_t) n_rows * 4, cudaMemcpyDeviceToHost, st));
+    if (kld_host) CK(cudaMemcpyAsync(kld_host, kld, (size_t) n_rows * sizeof(pb200_kld_score), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return check_clear_abort() ? PB200_EABORTED : 0;
 }
 
 // the callers have checked the model, seq, T, pos0 and which input is given; the prompt's K/V rows go to slot seq.  The scratch, x_out and

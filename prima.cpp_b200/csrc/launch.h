@@ -208,6 +208,12 @@ int launch_penalty_accept(void * state, const int32_t * tokens, int n, cudaStrea
 // per-row scores of logits[n_rows][n_vocab] against targets[n_rows] (device) -> out[n_rows] (sample.cu, k_token_scores): one launch of
 // n_rows CTAs (n_rows <= INT32_MAX)
 int launch_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets, pb200_token_score * out, cudaStream_t stream);
+// llama-perplexity's u16 log-probability records of the same rows (sample.cu, k_logprobs_u16; nll optional, targets only read with it),
+// and their KL-divergence against base records (k_kld): one launch of n_rows CTAs each (n_rows <= INT32_MAX, records 4-byte aligned)
+int launch_logprobs_u16(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets, uint16_t * records, float * nll,
+                        cudaStream_t stream);
+int launch_kld_scores(const float * logits, int64_t n_rows, int n_vocab, const uint16_t * base, const int32_t * targets, pb200_kld_score * out,
+                      cudaStream_t stream);
 
 // element-wise helpers for the plugin
 int launch_binary(int op /*0 add, 1 mul*/, const float * a, const float * b, float * y, int64_t n, int64_t nb /*b broadcast period*/, cudaStream_t stream);

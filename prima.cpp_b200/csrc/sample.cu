@@ -436,21 +436,12 @@ __global__ void k_penalty_accept(PenHdr * st, const int32_t * __restrict__ tok, 
 // ---- scoring of prompt logits: llama-perplexity's log_softmax (examples/perplexity/perplexity.cpp:106-116), one CTA per row ----
 constexpr int TS_NT = 512;
 
-__global__ void __launch_bounds__(TS_NT) k_token_scores(const float * __restrict__ logits, int n_vocab, const int32_t * __restrict__ targets,
-                                                         pb200_token_score * __restrict__ out) {
+// The CTA's (max, first index of the maximum) from each thread's (best, bi); every thread gets the winner.  Lanes' candidates come from
+// ascending i per thread with strict '>', so ties go to the lowest index: the reference's first occurrence.
+__device__ __forceinline__ void block_argmax(float & best, int & bi) {
     __shared__ float s_max[TS_NT / 32];
     __shared__ int s_top[TS_NT / 32];
-    __shared__ double s_sum[TS_NT / 32];
-    const int64_t r = blockIdx.x;
-    const float * x = logits + r * n_vocab;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    // max and the first index of the maximum (ascending i per thread, strict '>': the first occurrence; -inf and NaN never win)
-    float best = -INFINITY;
-    int bi = 0x7fffffff;
-    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) {
-        const float v = x[i];
-        if (v > best) { best = v; bi = i; }
-    }
     warp_argmax(best, bi);
     if (lane == 0) { s_max[warp] = best; s_top[warp] = bi; }
     __syncthreads();
@@ -461,10 +452,15 @@ __global__ void __launch_bounds__(TS_NT) k_token_scores(const float * __restrict
         if (lane == 0) { s_max[0] = best; s_top[0] = bi; }   // every lane has read its slot: warp_argmax's shuffles order them
     }
     __syncthreads();
-    const float mx = s_max[0];
-    // sum of expf(l - max): each term the accurate f32 expf of an f32 difference, as the reference computes it, summed in double
-    double s = 0.0;
-    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) s += (double) expf(x[i] - mx);
+    best = s_max[0];
+    bi = s_top[0];
+    __syncthreads();                                       // the slots may be reused by the next call
+}
+
+// The CTA's double sum of each thread's s, in one fixed order (lanes by xor shuffle, then warps in ascending order); every thread gets it.
+__device__ __forceinline__ double block_sum(double s) {
+    __shared__ double s_sum[TS_NT / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
     if (lane == 0) s_sum[warp] = s;
@@ -472,14 +468,152 @@ __global__ void __launch_bounds__(TS_NT) k_token_scores(const float * __restrict
     if (threadIdx.x == 0) {
         double sum = 0.0;
         for (int w = 0; w < TS_NT / 32; w++) sum += s_sum[w];
+        s_sum[0] = sum;
+    }
+    __syncthreads();
+    const double sum = s_sum[0];
+    __syncthreads();
+    return sum;
+}
+
+// What all three of llama-perplexity's log_softmax overloads compute first over a row: the max (with the first index of the maximum, and
+// the min where MIN), then the sum of expf(l - max), each term the accurate f32 expf of an f32 difference as the reference computes it,
+// summed in double.  -inf and NaN never win the max.  One CTA of TS_NT threads per row; every thread gets the result.
+struct RowSoftmax { float mx, mn; int top; double sum; };
+
+template <bool MIN>
+__device__ __forceinline__ RowSoftmax row_softmax(const float * __restrict__ x, int n_vocab) {
+    __shared__ float s_min[TS_NT / 32];
+    RowSoftmax r;
+    float best = -INFINITY, lo = INFINITY;
+    int bi = 0x7fffffff;
+    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) {
+        const float v = x[i];
+        if (v > best) { best = v; bi = i; }
+        if (MIN) lo = fminf(lo, v);
+    }
+    if (MIN) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+        if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = lo;
+    }
+    block_argmax(best, bi);                                // its barriers publish s_min
+    if (MIN) {
+        lo = s_min[0];
+        for (int w = 1; w < TS_NT / 32; w++) lo = fminf(lo, s_min[w]);
+    }
+    r.mx = best; r.top = bi; r.mn = lo;
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) s += (double) expf(x[i] - r.mx);
+    r.sum = block_sum(s);
+    return r;
+}
+
+__global__ void __launch_bounds__(TS_NT) k_token_scores(const float * __restrict__ logits, int n_vocab, const int32_t * __restrict__ targets,
+                                                         pb200_token_score * __restrict__ out) {
+    const int64_t r = blockIdx.x;
+    const float * x = logits + r * n_vocab;
+    const RowSoftmax rs = row_softmax<false>(x, n_vocab);
+    if (threadIdx.x == 0) {
         pb200_token_score o{};
-        o.top = s_top[0];
+        o.top = rs.top;
         const int tok = targets[r];
         if (tok >= 0 && tok < n_vocab) {               // otherwise the row is not scored: nll, logit and prob stay 0
             const float l = x[tok];
             o.logit = l;
-            o.nll = (double) mx + log(sum) - (double) l;
-            o.prob = __fdiv_rn(expf(l - mx), (float) sum);
+            o.nll = (double) rs.mx + log(rs.sum) - (double) l;
+            o.prob = __fdiv_rn(expf(l - rs.mx), (float) rs.sum);
+        }
+        out[r] = o;
+    }
+}
+
+// the reference's nearest_int (examples/perplexity/perplexity.cpp:118-123): round to nearest even through the float adder, valid for
+// |fval| <= 4194303
+__device__ __forceinline__ int nearest_int(float fval) {
+    return (__float_as_int(__fadd_rn(fval, 12582912.f)) & 0x007fffff) - 0x00400000;
+}
+
+// ---- llama-perplexity --kl-divergence-base: log_softmax(n_vocab, logits, uint16_t * log_prob, tok) (perplexity.cpp:125-153) ----
+// Row r becomes record r of nv = 2*((n_vocab+1)/2) + 4 uint16: {f32 scale, f32 min_log_prob}, n_vocab entries, a zero pad entry when
+// n_vocab is odd.  Every product and sum is rounded on its own (no contraction), in the reference's order.
+__global__ void __launch_bounds__(TS_NT) k_logprobs_u16(const float * __restrict__ logits, int n_vocab, const int32_t * __restrict__ targets,
+                                                        uint16_t * __restrict__ records, float * __restrict__ nll) {
+    __shared__ float s_par[2];
+    const int64_t r = blockIdx.x;
+    const float * x = logits + r * n_vocab;
+    const int nv = 2 * ((n_vocab + 1) / 2) + 4;
+    uint16_t * rec = records + r * nv;
+    const RowSoftmax rs = row_softmax<true>(x, n_vocab);
+    if (threadIdx.x == 0) {
+        const float min_logit = fmaxf(rs.mn, __fsub_rn(rs.mx, 16.f));
+        const float lse = (float) log(rs.sum);
+        const float min_log_prob = __fsub_rn(__fsub_rn(min_logit, rs.mx), lse);
+        const float scale = __fdiv_rn(__fsub_rn(rs.mx, min_logit), 65535.f);
+        reinterpret_cast<float *>(rec)[0] = scale;
+        reinterpret_cast<float *>(rec)[1] = min_log_prob;
+        s_par[0] = min_logit;
+        s_par[1] = scale;
+        if (nll) {
+            const int tok = targets[r];
+            nll[r] = (tok >= 0 && tok < n_vocab) ? __fsub_rn(__fadd_rn(rs.mx, lse), x[tok]) : 0.f;
+        }
+    }
+    __syncthreads();
+    const float min_logit = s_par[0], scale = s_par[1];
+    const float inv_scale = scale != 0.f ? __fdiv_rn(1.f, scale) : 0.f;
+    // entries in pairs (one 4-byte store each: the record and its entries start 4-byte aligned); entry n_vocab is the odd row's zero pad
+    uint32_t * e = reinterpret_cast<uint32_t *>(rec + 4);
+    for (int j = threadIdx.x; j < nv / 2 - 2; j += TS_NT) {
+        uint32_t q[2] = {0u, 0u};
+#pragma unroll
+        for (int k = 0; k < 2; k++) {
+            const int i = 2 * j + k;
+            if (scale != 0.f && i < n_vocab) {
+                const float l = x[i];
+                q[k] = l > min_logit ? (uint16_t) nearest_int(__fmul_rn(inv_scale, __fsub_rn(l, min_logit))) : 0u;
+            }
+        }
+        e[j] = q[0] | (q[1] << 16);
+    }
+}
+
+// ---- llama-perplexity --kl-divergence: log_softmax(n_vocab, logits, base_log_prob, tok, kld) (perplexity.cpp:237-296), per row ----
+__global__ void __launch_bounds__(TS_NT) k_kld(const float * __restrict__ logits, int n_vocab, const uint16_t * __restrict__ base,
+                                               const int32_t * __restrict__ targets, pb200_kld_score * __restrict__ out) {
+    const int64_t r = blockIdx.x;
+    const float * x = logits + r * n_vocab;
+    const int nv = 2 * ((n_vocab + 1) / 2) + 4;
+    const uint16_t * rec = base + r * nv;
+    const RowSoftmax rs = row_softmax<false>(x, n_vocab);
+    const float lse = (float) log(rs.sum);
+    const float scale = reinterpret_cast<const float *>(rec)[0], min_log_prob = reinterpret_cast<const float *>(rec)[1];
+    const uint16_t * q = rec + 4;
+    const float max_lse = __fadd_rn(rs.mx, lse);           // max_logit += log_sum_exp
+    // the base's first index of its maximum ('i == 0 || >'), and the KLD terms where the base's log-probability is above -16, each a
+    // float product summed in double
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n_vocab; i += TS_NT) {
+        const float p_log_base = __fadd_rn(__fmul_rn(scale, (float) q[i]), min_log_prob);
+        if (p_log_base > best) { best = p_log_base; bi = i; }
+        if (p_log_base > -16.f)
+            s += (double) __fmul_rn(expf(p_log_base), __fadd_rn(__fsub_rn(p_log_base, x[i]), max_lse));
+    }
+    block_argmax(best, bi);
+    const double kld = block_sum(s);
+    if (threadIdx.x == 0) {
+        pb200_kld_score o{};
+        o.kld = kld;
+        o.same_top = rs.top == bi;
+        const int tok = targets[r];
+        if (tok >= 0 && tok < n_vocab) {               // otherwise nll, nll_base and p_diff stay 0
+            const float nll = __fsub_rn(max_lse, x[tok]);
+            const float nll_base = -__fadd_rn(__fmul_rn(scale, (float) q[tok]), min_log_prob);
+            o.nll = nll;
+            o.nll_base = nll_base;
+            o.p_diff = __fsub_rn(expf(-nll), expf(-nll_base));
         }
         out[r] = o;
     }
@@ -489,6 +623,18 @@ __global__ void __launch_bounds__(TS_NT) k_token_scores(const float * __restrict
 
 int launch_token_scores(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets, pb200_token_score * out, cudaStream_t stream) {
     k_token_scores<<<(unsigned) n_rows, TS_NT, 0, stream>>>(logits, n_vocab, targets, out);
+    return (int) cudaGetLastError();
+}
+
+int launch_logprobs_u16(const float * logits, int64_t n_rows, int n_vocab, const int32_t * targets, uint16_t * records, float * nll,
+                        cudaStream_t stream) {
+    k_logprobs_u16<<<(unsigned) n_rows, TS_NT, 0, stream>>>(logits, n_vocab, targets, records, nll);
+    return (int) cudaGetLastError();
+}
+
+int launch_kld_scores(const float * logits, int64_t n_rows, int n_vocab, const uint16_t * base, const int32_t * targets, pb200_kld_score * out,
+                      cudaStream_t stream) {
+    k_kld<<<(unsigned) n_rows, TS_NT, 0, stream>>>(logits, n_vocab, base, targets, out);
     return (int) cudaGetLastError();
 }
 

@@ -5,6 +5,8 @@ import ctypes as C
 import subprocess
 from pathlib import Path
 
+from .perplexity import record_u16s
+
 PKG = Path(__file__).resolve().parent
 ROOT = PKG.parent
 
@@ -72,6 +74,13 @@ class TokenScore(C.Structure):
     """pb200_token_score: llama-perplexity's log_softmax of one scored position (nll = -log p(target), the target's logit and
     probability, the first index of the row's maximum)."""
     _fields_ = [("nll", C.c_double), ("logit", C.c_float), ("prob", C.c_float), ("top", C.c_int32), ("_pad", C.c_int32)]
+
+
+class KldScore(C.Structure):
+    """pb200_kld_score: llama-perplexity --kl-divergence's log_softmax of one scored position against the base model's record: the KL
+    divergence from the base, the nll of the target under this model and under the base, p(target) - p_base(target), and whether both
+    rows' first index of the maximum agree."""
+    _fields_ = [("kld", C.c_double), ("nll", C.c_float), ("nll_base", C.c_float), ("p_diff", C.c_float), ("same_top", C.c_int32)]
 
 
 class Pb200Error(RuntimeError):
@@ -171,6 +180,10 @@ class Lib:
         c.pb200_sampler_accept_seq.argtypes = [vp, C.c_int, vp, C.c_int]
         c.pb200_token_scores.argtypes = [vp, i64, C.c_int, vp, vp, vp]
         c.pb200_prompt_head.argtypes = [vp, i32, i32, vp, vp, vp]
+        c.pb200_logprob_record_u16s.argtypes = [C.c_int]
+        c.pb200_logprobs_u16.argtypes = [vp, i64, C.c_int, vp, vp, vp, vp]
+        c.pb200_kld_scores.argtypes = [vp, i64, C.c_int, vp, vp, vp, vp]
+        c.pb200_prompt_head_kld.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp]
 
     @classmethod
     def get(cls) -> "Lib":
@@ -214,6 +227,17 @@ class Lib:
         """pb200_token_scores: one TokenScore per row of the device logits [n_rows][n_vocab] against the int32 device targets (enqueued)."""
         self.check(self.c.pb200_token_scores(C.c_void_p(logits_ptr), n_rows, n_vocab, C.c_void_p(targets_ptr), C.c_void_p(out_ptr),
                                              C.c_void_p(stream)), "token_scores")
+
+    def logprobs_u16(self, logits_ptr: int, n_rows: int, n_vocab: int, targets_ptr: int, records_ptr: int, nll_ptr: int = 0, stream: int = 0) -> None:
+        """pb200_logprobs_u16: the u16 log-probability record of each row of the device logits (and, with nll_ptr, the f32 nll against the
+        int32 device targets) (enqueued)."""
+        self.check(self.c.pb200_logprobs_u16(C.c_void_p(logits_ptr), n_rows, n_vocab, C.c_void_p(targets_ptr or None), C.c_void_p(records_ptr),
+                                             C.c_void_p(nll_ptr or None), C.c_void_p(stream)), "logprobs_u16")
+
+    def kld_scores(self, logits_ptr: int, n_rows: int, n_vocab: int, base_ptr: int, targets_ptr: int, out_ptr: int, stream: int = 0) -> None:
+        """pb200_kld_scores: one KldScore per row of the device logits against the device base records and int32 targets (enqueued)."""
+        self.check(self.c.pb200_kld_scores(C.c_void_p(logits_ptr), n_rows, n_vocab, C.c_void_p(base_ptr), C.c_void_p(targets_ptr),
+                                           C.c_void_p(out_ptr), C.c_void_p(stream)), "kld_scores")
 
 
 class Model:
@@ -325,6 +349,29 @@ class Model:
             return None if a is None else a.ctypes.data_as(C.c_void_p)
         self.lib.check(self.lib.c.pb200_prompt_head(self.h, int(row0), int(n), p(tg), p(lg), p(sc)), "prompt_head")
         return lg, sc
+
+    def prompt_head_kld(self, row0: int, n: int, targets, records: bool = False, base=None):
+        """pb200_prompt_head_kld: the same rows and head as prompt_head, in llama-perplexity's KL-divergence modes.  targets: n ids in
+        [0, n_vocab).  records=True (writer mode) returns the rows' u16 log-probability records [n][record_u16s(n_vocab)] and their f32 nll;
+        base (compare mode, [n][record_u16s(n_vocab)] uint16) returns a numpy array of KldScore records.  Returns (records or None, nll or None,
+        kld or None)."""
+        import numpy as np
+        nv = record_u16s(self.hp.n_vocab)
+        tg = np.ascontiguousarray(targets, dtype=np.int32)
+        if tg.shape != (n,):
+            raise ValueError(f"need {n} targets, got shape {tg.shape}")
+        rec = np.empty((n, nv), dtype=np.uint16) if records else None
+        nll = np.empty(n, dtype=np.float32) if records else None
+        kld = bs = None
+        if base is not None:
+            bs = np.ascontiguousarray(base, dtype=np.uint16)
+            if bs.shape != (n, nv):
+                raise ValueError(f"need base records of shape {(n, nv)}, got {bs.shape}")
+            kld = np.zeros(n, dtype=np.dtype(KldScore))
+        def p(a):
+            return None if a is None else a.ctypes.data_as(C.c_void_p)
+        self.lib.check(self.lib.c.pb200_prompt_head_kld(self.h, int(row0), int(n), p(tg), p(rec), p(nll), p(bs), p(kld)), "prompt_head_kld")
+        return rec, nll, kld
 
     def decode_async(self, token: int, pos: int) -> None:
         self.lib.check(self.lib.c.pb200_decode_async(self.h, token, pos), "decode_async")
