@@ -84,14 +84,14 @@ template <int TYPE>
 __device__ __forceinline__ float dot_block(int type, const uint8_t * bp, const ActRegs & r) {
     if (TYPE == T_Q4_K) return dot_q4K(bp, r);
     if (TYPE == T_Q5_K) return dot_q5K(bp, r);
-    if (TYPE == T_Q6_K) return dot_q6K(bp, r);
+    if (TYPE == T_Q6_K) return dot_q6K(bp, r, smem_u32(bp) & 3u);
     if (TYPE == T_Q8_0) return dot_q8_0x8(bp, r);
     if (TYPE == T_Q5_1) return dot_q5_1x8(bp, r);
     if (TYPE == T_Q4_0) return dot_q4_0x8(bp, r);
     if (TYPE == T_Q4_1) return dot_q4_1x8(bp, r);
     if (TYPE == T_Q5_0) return dot_q5_0x8(bp, r);
     if (type == T_Q4_K) return dot_q4K(bp, r);
-    if (type == T_Q6_K) return dot_q6K(bp, r);
+    if (type == T_Q6_K) return dot_q6K(bp, r, smem_u32(bp) & 3u);
     return dot_q5K(bp, r);
 }
 
@@ -417,39 +417,48 @@ __global__ void __launch_bounds__(GEMV_THREADS, GEMV_CTAS_PER_SM) k_gemv_kquant(
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Generic fallback: one warp per row, direct global loads, every supported type (incl. the 32-element block types
-// Q8_0 / Q5_1 / Q5_0 that Qwen2.5-72B's ffn_down falls back to, src/llama.cpp:19516-19551, and Q4_0 / Q4_1), any K.
-// Follows ggml_vec_dot_q8_0_q8_0 (ggml-quants.c:5518) and ggml_vec_dot_q5_1_q8_1 (:5144).
+// Generic fallback: one warp per row, direct global loads, every supported type, any K.  It runs what the ring does not take: rows
+// longer than 29 696 elements, 32-element block type rows that are not 8-byte multiples, and W that is not 16-byte aligned.
+// Lane l owns blocks l, l + 32, ... of the row.
 __device__ __forceinline__ uint32_t ld_u16x2(const uint8_t * p) {   // 2-B aligned 32-bit read
     const uint16_t * q = reinterpret_cast<const uint16_t *>(p);
     return (uint32_t) q[0] | ((uint32_t) q[1] << 16);
 }
 
-// One Q4_0 / Q4_1 / Q5_0 block (2-byte aligned, global or shared memory) against its q8_0 / q8_1 activation block (av, scale da, sum sa),
-// in the order of the CPU's block loop (ggml_vec_dot_q4_0_q8_0 ggml-quants.c:3921, _q4_1_q8_1 :4502, _q5_0_q8_0 :4789)
-__device__ __forceinline__ float dot_legacy_block(int type, const uint8_t * bp, const int (&av)[8], float da, float sa) {
-    const uint32_t dw = ld_u16x2(bp);
+// acc + one 32-element block (2-byte aligned) against its q8_0 / q8_1 activation block (av, scale da, sum sa), in the order of the
+// CPU's block loop (ggml_vec_dot_q8_0_q8_0 ggml-quants.c:5518, _q5_1_q8_1 :5144, _q4_0_q8_0 :3921, _q4_1_q8_1 :4502, _q5_0_q8_0 :4789).
+// Blocks: [d f16] then Q8_0 32 x i8; Q4_0 16 x 2 nibbles; Q4_1 [m f16] nibbles; Q5_0 [qh u32] nibbles; Q5_1 [m f16][qh u32] nibbles.
+// The roundings are spelled out (Q8_0's product fused into the running sum, the other types' block term rounded before it is added)
+// so that they do not depend on whether the compiler contracts the running sum across the inlined call.
+__device__ __forceinline__ float dot_blk32(int type, const uint8_t * bp, const int (&av)[8], float da, float sa, float acc) {
+    const uint32_t dw = ld_u16x2(bp);   // d, and m of Q4_1 / Q5_1
     const float d = __half2float(__ushort_as_half((unsigned short) (dw & 0xffffu)));
-    const int qoff = type == T_Q4_0 ? 2 : type == T_Q4_1 ? 4 : 6;
-    const uint32_t qh = type == T_Q5_0 ? ld_u16x2(bp + 2) : 0u;
     int sumi = 0;
+    if (type == T_Q8_0) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) sumi = dp4a_ss((int) ld_u16x2(bp + 2 + 4 * i), av[i], sumi);
+        return __fmaf_rn((float) sumi, d * da, acc);
+    }
+    const bool has_m = type == T_Q4_1 || type == T_Q5_1, has_h = type == T_Q5_0 || type == T_Q5_1;
+    const int qhoff = has_m ? 4 : 2, qoff = has_h ? qhoff + 4 : qhoff;
+    const uint32_t qh = has_h ? ld_u16x2(bp + qhoff) : 0u;
 #pragma unroll
     for (int i = 0; i < 4; i++) {
         const uint32_t w = ld_u16x2(bp + qoff + 4 * i);
         uint32_t lo = w & 0x0f0f0f0fu, hi = (w >> 4) & 0x0f0f0f0fu;
-        if (type == T_Q5_0) {   // bit k of a nibble of qh -> bit 4 of byte k (x * 0x00204081 puts bit k at 8k, no carries)
+        if (has_h) {   // bit k of a nibble of qh -> bit 4 of byte k (x * 0x00204081 puts bit k at 8k, no carries)
             lo |= ((((qh >> (4 * i)) & 0xFu) * 0x00204081u) & 0x01010101u) << 4;
             hi |= ((((qh >> (4 * i + 16)) & 0xFu) * 0x00204081u) & 0x01010101u) << 4;
         }
         sumi = dp4a_us(lo, av[i], sumi);
         sumi = dp4a_us(hi, av[4 + i], sumi);
     }
-    if (type == T_Q4_1) return (d * da) * (float) sumi + __half2float(__ushort_as_half((unsigned short) (dw >> 16))) * sa;
+    if (has_m) return __fadd_rn(acc, __fmaf_rn(d * da, (float) sumi, __half2float(__ushort_as_half((unsigned short) (dw >> 16))) * sa));
     int asum = 0;
 #pragma unroll
     for (int i = 0; i < 8; i++) asum = dp4a_ss(0x01010101, av[i], asum);
-    if (type == T_Q4_0) return (float) (sumi - 8 * asum) * d * da;
-    return (d * da) * (float) (sumi - 16 * asum);
+    if (type == T_Q4_0) return __fadd_rn(acc, (float) (sumi - 8 * asum) * d * da);
+    return __fadd_rn(acc, (d * da) * (float) (sumi - 16 * asum));
 }
 
 struct GemvGenericParams {
@@ -470,112 +479,54 @@ __global__ void __launch_bounds__(256) k_gemv_generic(const __grid_constant__ Ge
     if (row >= P.N) return;
     const uint8_t * wrow = P.W + (int64_t) row * P.row_bytes;
     float acc = 0.f;
-    if (P.type == T_Q8_0) {
-        const int nb = P.K / 32;
-        for (int b = lane; b < nb; b += 32) {
-            const uint8_t * bp = wrow + (int64_t) b * BYTES_Q8_0;
-            const float d = __half2float(__ushort_as_half(*reinterpret_cast<const uint16_t *>(bp)));
-            const int4 * a = reinterpret_cast<const int4 *>(P.act.qs + (int64_t) b * 32);
-            const int4 a0 = a[0], a1 = a[1];
-            const int av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            int sumi = 0;
-#pragma unroll
-            for (int i = 0; i < 8; i++) sumi = dp4a_ss((int) ld_u16x2(bp + 2 + 4 * i), av[i], sumi);
-            acc += (float) sumi * (d * P.act.d[b]);
-        }
-    } else if (P.type == T_Q5_1) {
-        const int nb = P.K / 32;
-        for (int b = lane; b < nb; b += 32) {
-            const uint8_t * bp = wrow + (int64_t) b * BYTES_Q5_1;   // 24 B: 8-B aligned rows, 4-B aligned fields
-            const uint32_t dmw = *reinterpret_cast<const uint32_t *>(bp);
-            const float d = __half2float(__ushort_as_half((unsigned short) (dmw & 0xffff)));
-            const float mm = __half2float(__ushort_as_half((unsigned short) (dmw >> 16)));
-            const uint32_t qh = *reinterpret_cast<const uint32_t *>(bp + 4);
-            const int4 * a = reinterpret_cast<const int4 *>(P.act.qs + (int64_t) b * 32);
-            const int4 a0 = a[0], a1 = a[1];
-            const int av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            int sumi = 0;
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const uint32_t w = *reinterpret_cast<const uint32_t *>(bp + 8 + 4 * i);   // qs bytes 4i..4i+3
-                // element j = 4i+k (low nibble) gets bit j of qh; element j+16 (high nibble) gets bit j+16
-                uint32_t hb_lo = 0, hb_hi = 0;
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                    hb_lo |= ((qh >> (4 * i + k)) & 1u) << (8 * k + 4);
-                    hb_hi |= ((qh >> (4 * i + k + 16)) & 1u) << (8 * k + 4);
-                }
-                sumi = dp4a_us((w & 0x0f0f0f0fu) | hb_lo, av[i], sumi);
-                sumi = dp4a_us(((w >> 4) & 0x0f0f0f0fu) | hb_hi, av[4 + i], sumi);
-            }
-            acc += (d * P.act.d[b]) * (float) sumi + mm * P.act.s[b];
-        }
-    } else if (P.type == T_Q4_0 || P.type == T_Q4_1 || P.type == T_Q5_0) {
+    if (is_blk32_type(P.type)) {
         const int nb = P.K / 32, bpb = (int) row_bytes(P.type, 32);
+        const bool act_s = P.type == T_Q4_1 || P.type == T_Q5_1;   // q8_1 activation
         for (int b = lane; b < nb; b += 32) {
             const int4 * a = reinterpret_cast<const int4 *>(P.act.qs + (int64_t) b * 32);
             const int4 a0 = a[0], a1 = a[1];
             const int av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            acc += dot_legacy_block(P.type, wrow + (int64_t) b * bpb, av, P.act.d[b], P.type == T_Q4_1 ? P.act.s[b] : 0.f);
+            acc = dot_blk32(P.type, wrow + (int64_t) b * bpb, av, P.act.d[b], act_s ? P.act.s[b] : 0.f, acc);
         }
     } else {
-        // k-quants without shared-memory staging (used when K > 65 536 or for tiny problems)
         const int nb = P.K / 256;
+        const int bpb = P.type == T_Q4_K ? BYTES_Q4_K : (P.type == T_Q5_K ? BYTES_Q5_K : BYTES_Q6_K);
         for (int b = lane; b < nb; b += 32) {
             ActRegs r;
             load_act_regs(r, P.act, b, true);
             finish_act_regs(r);
-            // stage the block through registers -> local array is avoided by reading global memory directly with the
-            // same dot routines: they only need byte-addressable memory with the block's natural alignment.
-            const int bpb = P.type == T_Q4_K ? BYTES_Q4_K : (P.type == T_Q5_K ? BYTES_Q5_K : BYTES_Q6_K);
+            // the ring's dot routines read the block straight from global memory: dot_q6K at any 2-byte alignment, dot_q4K / dot_q5K
+            // (128-bit loads) only on a 16-byte aligned block
             const uint8_t * bp = wrow + (int64_t) b * bpb;
-            // dot_q6K uses shared-memory addressing for its alignment probe; use the global-memory variant below
-            if (P.type == T_Q4_K && ((uintptr_t) bp & 15) == 0) acc += dot_q4K(bp, r);
+            if (P.type == T_Q6_K) acc += dot_q6K(bp, r, (uint32_t) ((uintptr_t) bp & 3));
+            else if (P.type == T_Q4_K && ((uintptr_t) bp & 15) == 0) acc += dot_q4K(bp, r);
             else if (P.type == T_Q5_K && ((uintptr_t) bp & 15) == 0) acc += dot_q5K(bp, r);
             else {
-                // byte-wise scalar path (rare): dequantize on the fly against int8 activations
+                // Q4_K / Q5_K byte-wise (W not 16-byte aligned): dequantize on the fly against int8 activations
                 const int8_t * a8 = P.act.qs + (int64_t) b * 256;
-                if (P.type == T_Q6_K) {
-                    const float d = __half2float(__ushort_as_half(*reinterpret_cast<const uint16_t *>(bp + 208)));
-                    const int8_t * sc = reinterpret_cast<const int8_t *>(bp + 192);
-                    int sumi = 0;
-                    for (int n = 0; n < 2; n++)
-                        for (int l = 0; l < 32; l++) {
-                            const uint8_t qa = bp[64 * n + l], qb = bp[64 * n + 32 + l], h = bp[128 + 32 * n + l];
-                            const int is = l / 16;
-                            const int q1 = (int) ((qa & 0xF) | (((h >> 0) & 3) << 4)) - 32;
-                            const int q2 = (int) ((qb & 0xF) | (((h >> 2) & 3) << 4)) - 32;
-                            const int q3 = (int) ((qa >> 4) | (((h >> 4) & 3) << 4)) - 32;
-                            const int q4 = (int) ((qb >> 4) | (((h >> 6) & 3) << 4)) - 32;
-                            sumi += sc[8 * n + is + 0] * q1 * a8[128 * n + l] + sc[8 * n + is + 2] * q2 * a8[128 * n + 32 + l] +
-                                    sc[8 * n + is + 4] * q3 * a8[128 * n + 64 + l] + sc[8 * n + is + 6] * q4 * a8[128 * n + 96 + l];
-                        }
-                    acc += (d * r.d) * (float) sumi;
-                } else {
-                    const bool q5 = P.type == T_Q5_K;
-                    const __half2 dm = *reinterpret_cast<const __half2 *>(bp);
-                    const uint8_t * scb = bp + 4;
-                    const uint8_t * qhb = bp + 16;
-                    const uint8_t * qs = bp + (q5 ? 48 : 16);
-                    int sumi = 0, summ = 0;
-                    for (int j = 0; j < 8; j++) {
-                        int sc, mn;
-                        if (j < 4) { sc = scb[j] & 63; mn = scb[j + 4] & 63; }
-                        else { sc = (scb[j + 4] & 0xF) | ((scb[j - 4] >> 6) << 4); mn = (scb[j + 4] >> 4) | ((scb[j] >> 6) << 4); }
-                        int dsum = 0, asum = 0;
-                        for (int l = 0; l < 32; l++) {
-                            const uint8_t byte = qs[32 * (j / 2) + l];
-                            int q = (j & 1) ? (byte >> 4) : (byte & 0xF);
-                            if (q5 && ((qhb[l] >> j) & 1)) q += 16;
-                            const int a = a8[32 * j + l];
-                            dsum += q * a;
-                            asum += a;
-                        }
-                        sumi += sc * dsum;
-                        summ += mn * asum;
+                const bool q5 = P.type == T_Q5_K;
+                const __half2 dm = *reinterpret_cast<const __half2 *>(bp);
+                const uint8_t * scb = bp + 4;
+                const uint8_t * qhb = bp + 16;
+                const uint8_t * qs = bp + (q5 ? 48 : 16);
+                int sumi = 0, summ = 0;
+                for (int j = 0; j < 8; j++) {
+                    int sc, mn;
+                    if (j < 4) { sc = scb[j] & 63; mn = scb[j + 4] & 63; }
+                    else { sc = (scb[j + 4] & 0xF) | ((scb[j - 4] >> 6) << 4); mn = (scb[j + 4] >> 4) | ((scb[j] >> 6) << 4); }
+                    int dsum = 0, asum = 0;
+                    for (int l = 0; l < 32; l++) {
+                        const uint8_t byte = qs[32 * (j / 2) + l];
+                        int q = (j & 1) ? (byte >> 4) : (byte & 0xF);
+                        if (q5 && ((qhb[l] >> j) & 1)) q += 16;
+                        const int a = a8[32 * j + l];
+                        dsum += q * a;
+                        asum += a;
                     }
-                    acc += (__low2float(dm) * r.d) * (float) sumi - (__high2float(dm) * r.d) * (float) summ;
+                    sumi += sc * dsum;
+                    summ += mn * asum;
                 }
+                acc += (__low2float(dm) * r.d) * (float) sumi - (__high2float(dm) * r.d) * (float) summ;
             }
         }
     }
@@ -584,108 +535,6 @@ __global__ void __launch_bounds__(256) k_gemv_generic(const __grid_constant__ Ge
         if (P.bias) acc += P.bias[row];
         if (P.resid) acc += P.resid[row];
         P.y[row] = acc;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Streaming GEMV for the 32-element block types (Q8_0 34 B, Q5_1 24 B per block): Qwen2.5-72B's ffn_down (K = 29 568, not a
-// multiple of 256) falls back to them (src/llama.cpp:19516-19551) and they are a third of that model's bytes.
-// The activation (q8_0 / q8_1) is staged once per CTA in shared memory; every warp streams whole rows through its own 4-deep
-// cp.async ring of 32-block chunks (8-byte pieces, all lanes issue, ~100 KB in flight per SM at 3 CTAs/SM); lane l owns block
-// l of every chunk, i.e. the same blocks and the same per-lane order as k_gemv_generic => bit-identical results.
-constexpr int B32_NST = 4;
-struct GemvB32Params {
-    const uint8_t * W;
-    float * y;
-    const float * bias;
-    const float * resid;
-    int64_t row_bytes;
-    int type, N, K, nb, bpb;
-    ActQ act;
-};
-__global__ void __launch_bounds__(256) k_gemv_blk32(const __grid_constant__ GemvB32Params P) {
-    extern __shared__ __align__(16) uint8_t b32_smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int kp = (P.K + 15) & ~15;
-    int8_t * a_qs = reinterpret_cast<int8_t *>(b32_smem);                        // [K]
-    float * a_d = reinterpret_cast<float *>(b32_smem + kp);                      // [nb]
-    float * a_s = a_d + P.nb;                                                    // [nb]  (q8_1: Q5_1 / Q4_1 only)
-    const int cb = 32 * P.bpb;                                                   // chunk bytes: 1088 / 768
-    uint8_t * ring = b32_smem + ((kp + 8 * P.nb + 15) & ~15) + (size_t) warp * B32_NST * 1088;
-    pdl_trigger();
-    pdl_wait();
-    for (int i = threadIdx.x; i < P.K / 16; i += 256) reinterpret_cast<int4 *>(a_qs)[i] = reinterpret_cast<const int4 *>(P.act.qs)[i];
-    const bool act_s = P.type == T_Q5_1 || P.type == T_Q4_1;
-    for (int i = threadIdx.x; i < P.nb; i += 256) { a_d[i] = P.act.d[i]; if (act_s) a_s[i] = P.act.s[i]; }
-    __syncthreads();
-    const int nchunk = (P.nb + 31) / 32;
-    const int pieces = cb / 8;
-    for (int row = blockIdx.x * 8 + warp; row < P.N; row += gridDim.x * 8) {
-        const uint8_t * wrow = P.W + (int64_t) row * P.row_bytes;
-        auto issue = [&](int c) {
-            if (c < nchunk) {
-                const int64_t off = (int64_t) c * cb;
-                uint8_t * dst = ring + (size_t) (c % B32_NST) * 1088;
-                for (int pc = lane; pc < pieces; pc += 32)
-                    if (off + pc * 8 + 8 <= P.row_bytes)
-                        asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst + pc * 8)), "l"(wrow + off + pc * 8) : "memory");
-            }
-            asm volatile("cp.async.commit_group;" ::: "memory");
-        };
-        for (int c = 0; c < B32_NST - 1; c++) issue(c);
-        float acc = 0.f;
-        for (int c = 0; c < nchunk; c++) {
-            issue(c + B32_NST - 1);
-            asm volatile("cp.async.wait_group %0;" ::"n"(B32_NST - 1) : "memory");
-            __syncwarp();
-            const int b = c * 32 + lane;
-            if (b < P.nb) {
-                const uint8_t * bp = ring + (size_t) (c % B32_NST) * 1088 + lane * P.bpb;
-                const int4 * a = reinterpret_cast<const int4 *>(a_qs + (int64_t) b * 32);
-                const int4 a0 = a[0], a1 = a[1];
-                const int av[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-                int sumi = 0;
-                if (P.type == T_Q8_0) {
-                    // 34-byte blocks are only 2-byte aligned: read the 9 aligned words around the block; qs (offset 2) is either
-                    // word-aligned already (block at 4k+2) or straddles two words (block at 4k): one PRMT per word, selector per lane
-                    const uint32_t * wp = reinterpret_cast<const uint32_t *>(reinterpret_cast<uintptr_t>(bp) & ~(uintptr_t) 3);
-                    const bool odd = (reinterpret_cast<uintptr_t>(bp) & 2) != 0;
-                    const uint32_t sel = odd ? 0x7654u : 0x5432u;
-                    uint32_t w[9];
-#pragma unroll
-                    for (int i = 0; i < 9; i++) w[i] = wp[i];
-                    const float d = __half2float(__ushort_as_half((unsigned short) ((w[0] >> (odd ? 16 : 0)) & 0xffff)));
-#pragma unroll
-                    for (int i = 0; i < 8; i++) sumi = dp4a_ss((int) __byte_perm(w[i], w[i + 1], sel), av[i], sumi);
-                    acc += (float) sumi * (d * a_d[b]);
-                } else if (P.type != T_Q5_1) {
-                    acc += dot_legacy_block(P.type, bp, av, a_d[b], act_s ? a_s[b] : 0.f);
-                } else {
-                    const uint32_t dmw = *reinterpret_cast<const uint32_t *>(bp);
-                    const float d = __half2float(__ushort_as_half((unsigned short) (dmw & 0xffff)));
-                    const float mm = __half2float(__ushort_as_half((unsigned short) (dmw >> 16)));
-                    const uint32_t qh = *reinterpret_cast<const uint32_t *>(bp + 4);
-#pragma unroll
-                    for (int i = 0; i < 4; i++) {
-                        const uint32_t w = *reinterpret_cast<const uint32_t *>(bp + 8 + 4 * i);
-                        // bit k of a nibble of qh -> bit 4 of byte k: x * 0x00204081 puts bit k at 8k (no carries), then << 4
-                        const uint32_t hb_lo = ((((qh >> (4 * i)) & 0xFu) * 0x00204081u) & 0x01010101u) << 4;
-                        const uint32_t hb_hi = ((((qh >> (4 * i + 16)) & 0xFu) * 0x00204081u) & 0x01010101u) << 4;
-                        sumi = dp4a_us((w & 0x0f0f0f0fu) | hb_lo, av[i], sumi);
-                        sumi = dp4a_us(((w >> 4) & 0x0f0f0f0fu) | hb_hi, av[4 + i], sumi);
-                    }
-                    acc += (d * a_d[b]) * (float) sumi + mm * a_s[b];
-                }
-            }
-            __syncwarp();   // the slot is refilled by the next issue()
-        }
-        asm volatile("cp.async.wait_all;" ::: "memory");
-        acc = warp_sum(acc);
-        if (lane == 0) {
-            if (P.bias) acc += P.bias[row];
-            if (P.resid) acc += P.resid[row];
-            P.y[row] = acc;
-        }
     }
 }
 
@@ -771,13 +620,12 @@ bool gemv_fused_prologue_ok(int K) { return K > 0 && K % 256 == 0 && K / 256 <= 
 
 // ring geometry of one launch: rows per tile of each matrix, stage size, depth — everything that must fit 2 CTAs on an SM
 struct GemvPlan { int wpr, nblk_p2, nstage, nstage_init, stage_bytes, smem, owner_only, rel_count, rows[GEMV_MAX_MAT]; };
-static bool is_blk32(int t) { return is_blk32_type(t); }
 // false: the group does not fit the ring kernel
 static bool gemv_plan(const GemvDesc * d, int nmat, int K, GemvPlan & pl) {
     for (int i = 0; i < nmat; i++)
         if ((uintptr_t) d[i].W & 15) return false;    // bulk copies need 16-byte aligned sources
     // k-quants: K a multiple of 256; 32-element block types (one matrix per launch): K a multiple of 32, columns of 8 blocks
-    const bool b32 = nmat == 1 && is_blk32(d[0].type);
+    const bool b32 = nmat == 1 && is_blk32_type(d[0].type);
     if (b32 ? !(K > 0 && K % 32 == 0 && (K + 255) / 256 <= GEMV_ACT_MAX_NBLK) : !gemv_fused_prologue_ok(K)) return false;
     const int nblk = (K + 255) / 256;
     int wpr = 1;
@@ -916,35 +764,6 @@ static int launch_ring(const GemvDesc * d, int nmat, int K, const ActQ & act, co
     return (int) cudaLaunchKernelEx(&lc.cfg, fn, P);
 }
 
-// 32-element block types with 8-byte aligned rows and an activation that fits in shared memory: the per-warp cp.async streaming kernel
-static bool blk32_ok(const GemvDesc & d, int K) {
-    return is_blk32(d.type) && K % 32 == 0 && row_bytes(d.type, K) % 8 == 0 && K <= 131072 && ((uintptr_t) d.W & 7) == 0;
-}
-static int launch_gemv_blk32(const GemvDesc & d, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
-    GemvB32Params P{};
-    P.W = (const uint8_t *) d.W;
-    P.y = d.y;
-    P.bias = d.bias;
-    P.resid = d.resid;
-    P.type = d.type;
-    P.N = d.N;
-    P.K = K;
-    P.nb = K / 32;
-    P.bpb = (int) row_bytes(d.type, 32);
-    P.row_bytes = row_bytes(d.type, K);
-    P.act = act;
-    const int kp = (K + 15) & ~15;
-    const size_t smem = (size_t) ((kp + 8 * P.nb + 15) & ~15) + (size_t) 8 * B32_NST * 1088;
-    static FuncAttrCache attr_cache;
-    {
-        cudaError_t e = ensure_dyn_smem(attr_cache, (const void *) k_gemv_blk32, smem, false);
-        if (e != cudaSuccess) return (int) e;
-    }
-    const int per_sm = (int) std::max<size_t>(1, std::min<size_t>(4, (224 * 1024) / (smem + 1024)));
-    LaunchCfg lc(dim3(std::min((d.N + 7) / 8, sm_count() * per_sm)), dim3(256), smem, stream, pdl);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_gemv_blk32, P);
-}
-
 static int launch_gemv_generic(const GemvDesc & d, int K, const ActQ & act, cudaStream_t stream, bool pdl) {
     GemvGenericParams P{};
     P.W = (const uint8_t *) d.W;
@@ -981,8 +800,7 @@ static int gemv_kernels(const GemvDesc * d, int nmat, int K, const ActQ & act, c
     for (int i = 0; i < nmat; i++) {
         int e;
         // gemv_plan takes a 32-element block type matrix only on its own: each of a group of them still gets the ring when it fits
-        if (is_blk32(d[i].type) && gemv_plan(&d[i], 1, K, pl)) e = launch_ring(&d[i], 1, K, act, pl, GemvPrologue{}, stream, pdl);
-        else if (blk32_ok(d[i], K)) e = launch_gemv_blk32(d[i], K, act, stream, pdl);
+        if (is_blk32_type(d[i].type) && gemv_plan(&d[i], 1, K, pl)) e = launch_ring(&d[i], 1, K, act, pl, GemvPrologue{}, stream, pdl);
         else e = launch_gemv_generic(d[i], K, act, stream, pdl);
         if (e) return e;
         nlaunch++;

@@ -208,11 +208,12 @@ __device__ __forceinline__ float dot_q5K(const uint8_t * blk, const ActRegs & r)
     return d * (float) sumi - dmin * (float) summ;
 }
 
-// One Q6_K super-block (210 B, only 2-B aligned): aligned 32-bit loads + funnel shift by the misalignment.
-__device__ __forceinline__ float dot_q6K(const uint8_t * blk, const ActRegs & r) {
-    const uint32_t addr = smem_u32(blk);
-    const uint32_t sh = (addr & 3u) * 8u;
-    const uint32_t * base = reinterpret_cast<const uint32_t *>(blk - (addr & 3u));
+// One Q6_K super-block (210 B, only 2-B aligned; shared or global memory): aligned 32-bit loads + funnel shift by the misalignment
+// mis (blk's address mod 4, which the caller takes from the address in the block's own state space).  Reads whole words, so up to
+// 6 bytes past the block's end.
+__device__ __forceinline__ float dot_q6K(const uint8_t * blk, const ActRegs & r, uint32_t mis) {
+    const uint32_t sh = mis * 8u;
+    const uint32_t * base = reinterpret_cast<const uint32_t *>(blk - mis);
     // scales (bytes 192..207) and d (bytes 208..209)
     uint32_t tail[6];
 #pragma unroll

@@ -97,8 +97,8 @@ int gemv_set_trace(unsigned long long * dev_buf, int slots);   // profiling: per
 //      (one mode: written straight into `act`; several: PRO_RMSNORM materialises the vector in pro.f32 first, then quantize + matrices
 //      per mode);
 //   2. the GEMV: the bulk-copy ring kernel when the group fits it (gemv_plan), else per matrix: the ring for a 32-element block type
-//      matrix (Q8_0 / Q5_1 / Q4_0 / Q4_1 / Q5_0) that fits it on its own, k_gemv_blk32 (such rows that fit its activation stage) or
-//      k_gemv_generic.
+//      matrix (Q8_0 / Q5_1 / Q4_0 / Q4_1 / Q5_0) that fits it on its own, else k_gemv_generic (rows longer than 29 696, 32-element
+//      block type rows that are not 8-byte multiples, W not 16-byte aligned).
 // The first kernel gets `pdl`, every later one is chained to its predecessor by programmatic dependent launch.  Adds the number of
 // kernels enqueued to nlaunch.  start (optional, profiling): an event recorded just before the first GEMV kernel, i.e. after any
 // producer kernel.

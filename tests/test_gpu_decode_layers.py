@@ -22,8 +22,8 @@ fp32 summation order.  The oracle is the C port (k-quants, Q8_0, Q5_1) or legacy
 producers do (same f32 input, same block scale arithmetic), so a quantization code that differs shows up as a GEMV error.
 
 decode_launches() restates the branch choices of launch_gemv (gemv.cu) and launch_attn_step (ops.cu): the distributed prologue inside
-the ring kernel; a producer kernel and the ring per matrix group; the several-modes route of a Q8_0 matrix beside k-quants; the ring,
-k_gemv_blk32 or k_gemv_generic per matrix; k_attn2, or k_attn_rows plus a quantize kernel in front of wo.  The launch count of every
+the ring kernel; a producer kernel and the ring per matrix group; the several-modes route of a Q8_0 matrix beside k-quants; the ring
+or k_gemv_generic per matrix; k_attn2, or k_attn_rows plus a quantize kernel in front of wo.  The launch count of every
 step must equal it, and a CPU-only test checks that each case reaches the branches it is there for.  The same tokens then go through
 the unsplit model (logits bit-identical to the shard composition), and direct launches must equal the CUDA-graph replay bit for bit.
 
@@ -54,18 +54,11 @@ def act_mode(t):
 
 # ---- the branch choices of one decode step, restated ----
 def gemv_kernels(types, Ns, K):
-    """gemv.cu gemv_kernels: the ring for the whole group, else per matrix the ring (32-element types on their own), k_gemv_blk32
-    (8-byte rows, K <= 131 072) or k_gemv_generic.  Weights are 256-byte aligned in the engine."""
+    """gemv.cu gemv_kernels: the ring for the whole group, else per matrix the ring (32-element types on their own) or
+    k_gemv_generic.  Weights are 256-byte aligned in the engine."""
     if gemv_plan(types, Ns, K):
         return 1, "ring"
-    kinds = []
-    for t, N in zip(types, Ns):
-        if t in BLK32 and gemv_plan((t,), (N,), K):
-            kinds.append("ring")
-        elif t in BLK32 and K % 32 == 0 and L.row_size(t, K) % 8 == 0 and K <= 131072:
-            kinds.append("blk32")
-        else:
-            kinds.append("generic")
+    kinds = ["ring" if t in BLK32 and gemv_plan((t,), (N,), K) else "generic" for t, N in zip(types, Ns)]
     return len(kinds), ",".join(kinds)
 
 
@@ -160,8 +153,8 @@ CASES = {
                           {"qkv:dist", "attn:attn2", "down:producer+ring", "head:dist"}),
     "qwen2_q5_K_M_generic": (_tiny(arch="qwen2", ftype="q5_K_M", n_ff=1056), 40,       # Q8_0 rows of 1 122 bytes: k_gemv_generic
                              {"down:producer+ring", "down:producer+generic"}),
-    "qwen2_q5_K_M_blk32": (_tiny(arch="qwen2", ftype="q5_K_M", n_ff=29824), 8,         # K past the ring's 116 super-blocks
-                           {"down:producer+blk32"}),
+    "qwen2_q5_K_M_longK": (_tiny(arch="qwen2", ftype="q5_K_M", n_ff=29824), 8,         # Q5_1 / Q8_0 K past the ring's 116 super-blocks
+                           {"down:producer+generic"}),
     "qwen2_q4_K_M": (_qwen2_q4_K_M, 40, {"qkv:dist", "attn:attn2", "down:producer+ring"}),
     "llama_q4_0": (_llama_q4_0, 40, {"qkv:producer+ring,ring,ring", "attn:rows", "wo:producer+ring", "gu:producer+ring,ring",
                                      "down:producer+ring", "head:dist"}),

@@ -90,7 +90,7 @@ def test_gemv_fused_prologue_rungs(cuda, lib, port, prologue):
 @pytest.mark.parametrize("t", [O.Q8_0, O.Q5_1], ids=lambda t: O.TYPE_NAME[t])
 def test_gemv_fused_small_block_types_each_take_the_ring(cuda, lib, port, t):
     """The ring kernel takes Q8_0 / Q5_1 matrices one at a time: a group of two still runs both on it (two instrumented ring
-    launches leave their CTA stamps in the trace buffer), not on the per-warp or generic kernels."""
+    launches leave their CTA stamps in the trace buffer), not on the generic kernel."""
     K, Ns = 4096, [64, 48]
     Ws = [O.synth_blocks(t, n, K, seed=31 + i) for i, n in enumerate(Ns)]
     x = np.random.default_rng(5).standard_normal(K).astype(np.float32)

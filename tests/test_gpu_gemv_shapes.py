@@ -350,7 +350,7 @@ def test_plan_sweep_vs_oracle(cuda, lib, port, case):
     for i, m in enumerate(ms):
         m.check(port, x, f"{sweep_id(case)} matrix {i}")
     # the launch above ran the ring kernel on the grid the plan implies: its instrumented instantiation stamps one trace entry per CTA
-    # (k_gemv_blk32 / k_gemv_generic stamp nothing)
+    # (k_gemv_generic stamps nothing)
     trace = torch.zeros(4096, dtype=torch.int64, device="cuda")
     lib.c.pb200_debug_set_trace.argtypes = [C.c_void_p, C.c_int]
     lib.check(lib.c.pb200_debug_set_trace(trace.data_ptr(), 1), "trace")

@@ -40,7 +40,7 @@ def test_quantize_act_bit_exact(cuda, lib, port, t):
 
 @pytest.mark.parametrize("t", KQ, ids=lambda t: O.TYPE_NAME[t])
 @pytest.mark.parametrize("N,K", [(64, 256), (37, 512), (8, 2048), (129, 4096), (24, 8192), (19, 14336), (10, 28672),
-                                 (21, 29952), (9, 53248)])   # beyond the ring's 29 696: k_gemv_generic (aligned k-quant dots, scalar Q6_K)
+                                 (21, 29952), (9, 53248)])   # beyond the ring's 29 696: k_gemv_generic (the ring's dot routines)
 def test_gemv_kquant_vs_oracle(cuda, lib, port, t, N, K):
     W = O.synth_blocks(t, N, K, seed=N * 31 + K)
     rng = np.random.default_rng(K + N)
@@ -55,7 +55,7 @@ def test_gemv_kquant_vs_oracle(cuda, lib, port, t, N, K):
 
 
 @pytest.mark.parametrize("t", [O.Q8_0, O.Q5_1], ids=lambda t: O.TYPE_NAME[t])
-@pytest.mark.parametrize("N,K", [(16, 64), (33, 7392), (5, 29568), (301, 29568), (64, 1280), (40, 4096), (7, 8192), (130, 14336)])   # K % 128 == 0: the bulk-copy ring (columns of 8 blocks; 29 568 = 115.5 columns, split rows), else the per-warp kernels
+@pytest.mark.parametrize("N,K", [(16, 64), (33, 7392), (5, 29568), (301, 29568), (64, 1280), (40, 4096), (7, 8192), (130, 14336)])   # K % 128 == 0: the bulk-copy ring (columns of 8 blocks; 29 568 = 115.5 columns, split rows), else k_gemv_generic
 def test_gemv_small_block_types_vs_oracle(cuda, lib, port, t, N, K):
     W = O.synth_blocks(t, N, K, seed=N + K)
     x = np.random.default_rng(K).standard_normal(K).astype(np.float32)
@@ -71,7 +71,7 @@ def test_gemv_small_block_types_vs_oracle(cuda, lib, port, t, N, K):
 @pytest.mark.parametrize("t", O.QUANT_TYPES, ids=lambda t: O.TYPE_NAME[t])
 def test_gemv_weight_bit_patterns_vs_oracle(cuda, lib, port, t):
     """The weight blocks of oracle_lib.edge_blocks (quant bytes all 0x00 / 0xFF, Q8_0 q = -128, Q6_K scale -128 with q = -32, scales and
-    mins of 63, d = 0) through the GEMV families above: k-quant ring; Q8_0 / Q5_1 on the ring (K % 128 == 0) and the per-warp kernels."""
+    mins of 63, d = 0) through the GEMV families above: k-quant ring; Q8_0 / Q5_1 on the ring (K % 128 == 0) and on k_gemv_generic."""
     for K in ([2048] if t in KQ else [2048, 1984]):
         N = 96
         W = O.edge_blocks(t, N, K, seed=K + t)

@@ -1,5 +1,5 @@
 """-m gpu: the legacy 32-element weight types Q4_0, Q4_1 and Q5_0 on every path, against the CPU oracles: the activation quantizer,
-the decode GEMV on each of its kernels (bulk-copy ring, split rows, k_gemv_blk32, k_gemv_generic), the tensor-core prefill product,
+the decode GEMV on each of its kernels (bulk-copy ring, split rows, k_gemv_generic), the tensor-core prefill product,
 get_rows, the engine (decode, prefill, GGUF load, synthetic Qwen2.5-72B Q4_K_M types) and whole decode graphs through the ggml-backend
 plugin."""
 import ctypes as C
@@ -67,8 +67,8 @@ def gemv(lib, t, W, N, K, x, shift=0, bias=None, resid=None, trace_slots=0):
 
 
 # (N, K, W shift, ring expected): the ring (whole rows, K = 8 192 and Llama-3-8B's 4 096 / 14 336), split rows at Qwen2.5-72B's ffn_down
-# (8 192 x 29 568: rows 8- but not 16-byte aligned) and a ragged N; a W 8 bytes off a 16-byte boundary (k_gemv_blk32); W 2 bytes off
-# and K = 1 056, whose rows are not 8-byte multiples (k_gemv_generic)
+# (8 192 x 29 568: rows 8- but not 16-byte aligned) and a ragged N; on k_gemv_generic, a W 8 or 2 bytes off a 16-byte boundary and
+# K = 1 056, whose rows are not 8-byte multiples
 GEMV_CASES = [(1000, 8192, 0, True), (333, 4096, 0, True), (200, 14336, 0, True), (8192, 29568, 0, True), (77, 29568, 0, True),
               (300, 8192, 8, False), (129, 29568, 8, False), (300, 4096, 2, False), (100, 1056, 0, False)]
 
