@@ -23,8 +23,11 @@
 
 #define QK_K 256
 
-/* ---- block layouts: ggml/src/ggml-common.h:173-204, 286-335 (byte-for-byte wire format) ---- */
+/* ---- block layouts: ggml/src/ggml-common.h:143-170, 173-204, 286-335 (byte-for-byte wire format) ---- */
 #pragma pack(push, 1)
+typedef struct { uint16_t d; uint8_t qs[16]; } blk_q4_0;                                          /* 18 B */
+typedef struct { uint16_t d, m; uint8_t qs[16]; } blk_q4_1;                                       /* 20 B */
+typedef struct { uint16_t d; uint8_t qh[4]; uint8_t qs[16]; } blk_q5_0;                           /* 22 B */
 typedef struct { uint16_t d, dmin; uint8_t scales[12]; uint8_t qs[128]; } blk_q4_K;              /* 144 B */
 typedef struct { uint16_t d, dmin; uint8_t scales[12]; uint8_t qh[32]; uint8_t qs[128]; } blk_q5_K; /* 176 B */
 typedef struct { uint8_t ql[128]; uint8_t qh[64]; int8_t scales[16]; uint16_t d; } blk_q6_K;     /* 210 B */
@@ -34,7 +37,7 @@ typedef struct { uint16_t d, s; int8_t qs[32]; } blk_q8_1;                      
 typedef struct { float d; int8_t qs[256]; int16_t bsums[16]; } blk_q8_K;                         /* 292 B */
 #pragma pack(pop)
 
-enum { T_F32 = 0, T_F16 = 1, T_Q5_1 = 7, T_Q8_0 = 8, T_Q4_K = 12, T_Q5_K = 13, T_Q6_K = 14 }; /* ggml.h:356-395 */
+enum { T_F32 = 0, T_F16 = 1, T_Q4_0 = 2, T_Q4_1 = 3, T_Q5_0 = 6, T_Q5_1 = 7, T_Q8_0 = 8, T_Q4_K = 12, T_Q5_K = 13, T_Q6_K = 14 }; /* ggml.h:356-395 */
 
 /* ---- fp16 <-> fp32, IEEE round-to-nearest-even (ggml-impl.h GGML_FP16_TO_FP32 / FP32_TO_FP16) ---- */
 float port_fp16_to_fp32(uint16_t h) {
@@ -93,7 +96,9 @@ static inline void get_scale_min_k4(int j, const uint8_t *q, uint8_t *d, uint8_t
     }
 }
 
-/* ---------------- dequantization (ggml-quants.c:2555-2577, 2763-2788, 2977-3006, 1616-1634, 1589-1613) ---------------- */
+/* ---------------- dequantization (ggml-quants.c:2555-2577, 2763-2788, 2977-3006, 1616-1634, 1589-1613, 1522-1580) ----------------
+ * In the 32-element blocks element j < 16 is the low nibble of qs[j], element j + 16 its high nibble; the fifth bit of element j is
+ * bit j of qh. */
 void port_dequantize_row_q4_K(const void *vx, float *y, int64_t k) {
     const blk_q4_K *x = (const blk_q4_K *)vx;
     for (int64_t i = 0; i < k / QK_K; i++) {
@@ -172,6 +177,51 @@ void port_dequantize_row_q5_1(const void *vx, float *y, int64_t k) {
     }
 }
 
+/* ggml-quants.c:1522-1540 */
+void port_dequantize_row_q4_0(const void *vx, float *y, int64_t k) {
+    const blk_q4_0 *x = (const blk_q4_0 *)vx;
+    for (int64_t i = 0; i < k / 32; i++) {
+        const float d = port_fp16_to_fp32(x[i].d);
+        for (int j = 0; j < 16; ++j) {
+            const int x0 = (x[i].qs[j] & 0x0F) - 8;
+            const int x1 = (x[i].qs[j] >> 4) - 8;
+            y[i * 32 + j] = x0 * d;
+            y[i * 32 + j + 16] = x1 * d;
+        }
+    }
+}
+
+/* ggml-quants.c:1542-1561 */
+void port_dequantize_row_q4_1(const void *vx, float *y, int64_t k) {
+    const blk_q4_1 *x = (const blk_q4_1 *)vx;
+    for (int64_t i = 0; i < k / 32; i++) {
+        const float d = port_fp16_to_fp32(x[i].d), m = port_fp16_to_fp32(x[i].m);
+        for (int j = 0; j < 16; ++j) {
+            const int x0 = x[i].qs[j] & 0x0F;
+            const int x1 = x[i].qs[j] >> 4;
+            y[i * 32 + j] = x0 * d + m;
+            y[i * 32 + j + 16] = x1 * d + m;
+        }
+    }
+}
+
+/* ggml-quants.c:1563-1586 */
+void port_dequantize_row_q5_0(const void *vx, float *y, int64_t k) {
+    const blk_q5_0 *x = (const blk_q5_0 *)vx;
+    for (int64_t i = 0; i < k / 32; i++) {
+        const float d = port_fp16_to_fp32(x[i].d);
+        uint32_t qh; memcpy(&qh, x[i].qh, 4);
+        for (int j = 0; j < 16; ++j) {
+            const uint8_t xh_0 = ((qh >> (j + 0)) << 4) & 0x10;
+            const uint8_t xh_1 = ((qh >> (j + 12))) & 0x10;
+            const int32_t x0 = ((x[i].qs[j] & 0x0F) | xh_0) - 16;
+            const int32_t x1 = ((x[i].qs[j] >> 4) | xh_1) - 16;
+            y[i * 32 + j] = x0 * d;
+            y[i * 32 + j + 16] = x1 * d;
+        }
+    }
+}
+
 int64_t port_row_size(int type, int64_t k) {   /* ggml_row_size, ggml.c type-traits table :732-1100 */
     switch (type) {
         case T_F32: return k * 4;
@@ -181,6 +231,9 @@ int64_t port_row_size(int type, int64_t k) {   /* ggml_row_size, ggml.c type-tra
         case T_Q6_K: return k / 256 * 210;
         case T_Q8_0: return k / 32 * 34;
         case T_Q5_1: return k / 32 * 24;
+        case T_Q4_0: return k / 32 * 18;
+        case T_Q4_1: return k / 32 * 20;
+        case T_Q5_0: return k / 32 * 22;
     }
     return -1;
 }
@@ -192,6 +245,9 @@ void port_dequantize_row(int type, const void *vx, float *y, int64_t k) {
         case T_Q6_K: port_dequantize_row_q6_K(vx, y, k); break;
         case T_Q8_0: port_dequantize_row_q8_0(vx, y, k); break;
         case T_Q5_1: port_dequantize_row_q5_1(vx, y, k); break;
+        case T_Q4_0: port_dequantize_row_q4_0(vx, y, k); break;
+        case T_Q4_1: port_dequantize_row_q4_1(vx, y, k); break;
+        case T_Q5_0: port_dequantize_row_q5_0(vx, y, k); break;
         case T_F32:  memcpy(y, vx, (size_t)k * 4); break;
         case T_F16:  for (int64_t i = 0; i < k; i++) y[i] = port_fp16_to_fp32(((const uint16_t *)vx)[i]); break;
     }
@@ -377,13 +433,71 @@ float port_vec_dot_q5_1_q8_1(int n, const void *vx, const void *vy) {
     return sumf;
 }
 
+/* ggml-quants.c:3921-4500, scalar tail :4481-4496 */
+float port_vec_dot_q4_0_q8_0(int n, const void *vx, const void *vy) {
+    const blk_q4_0 *x = (const blk_q4_0 *)vx; const blk_q8_0 *y = (const blk_q8_0 *)vy;
+    float sumf = 0;
+    for (int ib = 0; ib < n / 32; ++ib) {
+        int sumi0 = 0, sumi1 = 0;
+        for (int j = 0; j < 16; ++j) {
+            const int v0 = (x[ib].qs[j] & 0x0F) - 8;
+            const int v1 = (x[ib].qs[j] >> 4) - 8;
+            sumi0 += v0 * y[ib].qs[j];
+            sumi1 += v1 * y[ib].qs[j + 16];
+        }
+        int sumi = sumi0 + sumi1;
+        sumf += sumi * port_fp16_to_fp32(x[ib].d) * port_fp16_to_fp32(y[ib].d);
+    }
+    return sumf;
+}
+
+/* ggml-quants.c:4502-4787, scalar tail :4770-4783 */
+float port_vec_dot_q4_1_q8_1(int n, const void *vx, const void *vy) {
+    const blk_q4_1 *x = (const blk_q4_1 *)vx; const blk_q8_1 *y = (const blk_q8_1 *)vy;
+    float sumf = 0;
+    for (int ib = 0; ib < n / 32; ++ib) {
+        int sumi0 = 0, sumi1 = 0;
+        for (int j = 0; j < 16; ++j) {
+            const int v0 = x[ib].qs[j] & 0x0F;
+            const int v1 = x[ib].qs[j] >> 4;
+            sumi0 += v0 * y[ib].qs[j];
+            sumi1 += v1 * y[ib].qs[j + 16];
+        }
+        int sumi = sumi0 + sumi1;
+        sumf += (port_fp16_to_fp32(x[ib].d) * port_fp16_to_fp32(y[ib].d)) * sumi
+              + port_fp16_to_fp32(x[ib].m) * port_fp16_to_fp32(y[ib].s);
+    }
+    return sumf;
+}
+
+/* ggml-quants.c:4789-5142, scalar tail :5120-5138 */
+float port_vec_dot_q5_0_q8_0(int n, const void *vx, const void *vy) {
+    const blk_q5_0 *x = (const blk_q5_0 *)vx; const blk_q8_0 *y = (const blk_q8_0 *)vy;
+    float sumf = 0;
+    for (int ib = 0; ib < n / 32; ++ib) {
+        uint32_t qh; memcpy(&qh, x[ib].qh, 4);
+        int sumi0 = 0, sumi1 = 0;
+        for (int j = 0; j < 16; ++j) {
+            const uint8_t xh_0 = ((qh >> (j + 0)) << 4) & 0x10;
+            const uint8_t xh_1 = ((qh >> (j + 12))) & 0x10;
+            const int32_t x0 = ((x[ib].qs[j] & 0xF) | xh_0) - 16;
+            const int32_t x1 = ((x[ib].qs[j] >> 4) | xh_1) - 16;
+            sumi0 += x0 * y[ib].qs[j];
+            sumi1 += x1 * y[ib].qs[j + 16];
+        }
+        int sumi = sumi0 + sumi1;
+        sumf += (port_fp16_to_fp32(x[ib].d) * port_fp16_to_fp32(y[ib].d)) * sumi;
+    }
+    return sumf;
+}
+
 /* size in bytes of the activation row after conversion to the weight type's vec_dot_type
- * (type-traits table ggml.c:732-1100: Q4_K/Q5_K/Q6_K -> Q8_K, Q8_0 -> Q8_0, Q5_1 -> Q8_1, F16 -> F16) */
+ * (type-traits table ggml.c:732-1100: Q4_K/Q5_K/Q6_K -> Q8_K, Q8_0/Q4_0/Q5_0 -> Q8_0, Q5_1/Q4_1 -> Q8_1, F16 -> F16) */
 static int64_t act_row_size(int wtype, int64_t k) {
     switch (wtype) {
         case T_Q4_K: case T_Q5_K: case T_Q6_K: return k / 256 * (int64_t)sizeof(blk_q8_K);
-        case T_Q8_0: return k / 32 * 34;
-        case T_Q5_1: return k / 32 * 36;
+        case T_Q8_0: case T_Q4_0: case T_Q5_0: return k / 32 * 34;
+        case T_Q5_1: case T_Q4_1: return k / 32 * 36;
         case T_F16: return k * 2;
         default: return k * 4;
     }
@@ -392,8 +506,8 @@ static int64_t act_row_size(int wtype, int64_t k) {
 static void act_quantize(int wtype, const float *x, void *q, int64_t k) {
     switch (wtype) {
         case T_Q4_K: case T_Q5_K: case T_Q6_K: port_quantize_row_q8_K(x, q, k); break;
-        case T_Q8_0: port_quantize_row_q8_0(x, q, k); break;
-        case T_Q5_1: port_quantize_row_q8_1(x, q, k); break;
+        case T_Q8_0: case T_Q4_0: case T_Q5_0: port_quantize_row_q8_0(x, q, k); break;
+        case T_Q5_1: case T_Q4_1: port_quantize_row_q8_1(x, q, k); break;
         case T_F16: for (int64_t i = 0; i < k; i++) ((uint16_t *)q)[i] = port_fp32_to_fp16(x[i]); break;
         default: memcpy(q, x, (size_t)k * 4);
     }
@@ -406,6 +520,9 @@ static float vec_dot(int wtype, int64_t k, const void *w, const void *q) {
         case T_Q6_K: return port_vec_dot_q6_K_q8_K((int)k, w, q);
         case T_Q8_0: return port_vec_dot_q8_0_q8_0((int)k, w, q);
         case T_Q5_1: return port_vec_dot_q5_1_q8_1((int)k, w, q);
+        case T_Q4_0: return port_vec_dot_q4_0_q8_0((int)k, w, q);
+        case T_Q4_1: return port_vec_dot_q4_1_q8_1((int)k, w, q);
+        case T_Q5_0: return port_vec_dot_q5_0_q8_0((int)k, w, q);
         case T_F16: {  /* ggml_vec_dot_f16 ggml.c:1893-1930: f32 accumulation of f16*f16 */
             float s = 0; const uint16_t *a = (const uint16_t *)w, *b = (const uint16_t *)q;
             for (int64_t i = 0; i < k; i++) s += port_fp16_to_fp32(a[i]) * port_fp16_to_fp32(b[i]);

@@ -3,6 +3,7 @@ ggml_backend_graph_compute on the registered "B200_0" backend vs the reference C
 in and out (ggml_backend_tensor_set / _get) — what llama_decode does.  Prints one JSON line.
 
     python tests/ggml_graph_parity.py <llama|qwen2> <n_tokens> [n_layer n_embd n_head n_head_kv n_ff n_vocab n_ctx]
+    python tests/ggml_graph_parity.py <qwen2_q4_K_M|llama_q4_0> <n_tokens>     (a model of tiny_model.legacy_golden_models())
 
 Script mode drives both backends through a list of steps the way llama_decode would: a prompt of n tokens at position pos is one
 graph of n tokens (a decode step is n = 1), "clear" empties both KV caches.  Every step computes all its rows' logits.
@@ -23,7 +24,7 @@ import numpy as np
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT)); sys.path.insert(0, str(ROOT / "tests")); sys.path.insert(0, str(ROOT / "host"))
-from tiny_model import TinyModel   # noqa: E402  (weights as raw GGUF blocks; loads no ggml)
+from tiny_model import TinyModel, legacy_golden_models   # noqa: E402  (weights as raw GGUF blocks; loads no ggml)
 import host_graph as HG            # noqa: E402
 
 arch = sys.argv[1]
@@ -36,13 +37,18 @@ if script_mode:
 else:
     n_tok = int(sys.argv[2])
     dims = [int(x) for x in sys.argv[3:10]] if len(sys.argv) >= 10 else None
-dims = dims or [3, 1024, 8, 2, 2816 if arch == "llama" else 3072, 384, 96]
 reserve = int(opts.get("--reserve", n_tok)) if script_mode else 1   # the token-by-token run keeps the one-token reservation
-n_layer, n_embd, n_head, n_head_kv, n_ff, n_vocab, n_ctx = dims
-tm = TinyModel(n_layer=n_layer, n_embd=n_embd, n_head=n_head, n_head_kv=n_head_kv, n_ff=n_ff, n_vocab=n_vocab, n_ctx=n_ctx, arch=arch,
-               ftype="q4_K_M" if arch == "llama" else "q5_K_M", freq_factors=(arch == "llama"), seed=31, branch_scale=0.1)
+if arch in ("llama", "qwen2"):
+    dims = dims or [3, 1024, 8, 2, 2816 if arch == "llama" else 3072, 384, 96]
+    n_layer, n_embd, n_head, n_head_kv, n_ff, n_vocab, n_ctx = dims
+    tm = TinyModel(n_layer=n_layer, n_embd=n_embd, n_head=n_head, n_head_kv=n_head_kv, n_ff=n_ff, n_vocab=n_vocab, n_ctx=n_ctx, arch=arch,
+                   ftype="q4_K_M" if arch == "llama" else "q5_K_M", freq_factors=(arch == "llama"), seed=31, branch_scale=0.1)
+else:
+    tm = legacy_golden_models()[arch][0]
+    n_layer, n_embd, n_head, n_head_kv, n_ff, n_vocab, n_ctx = (tm.hp[k] for k in ("n_layer", "n_embd", "n_head", "n_head_kv", "n_ff",
+                                                                                   "n_vocab", "n_ctx"))
 types = {name: t for name, (t, a) in tm.tensors.items() if name.endswith(".weight") and a.dtype == np.uint8}
-has_bias = arch == "qwen2"
+has_bias = tm.arch == "qwen2"
 has_ff = "rope_freqs.weight" in tm.tensors
 g, plug = HG.load(with_plugin=True)
 libpb = C.CDLL(str(ROOT / "prima.cpp_b200" / "libprima_b200.so"))
@@ -123,6 +129,7 @@ res = {"arch": arch, "n_tokens": n_tok, "max_abs_per_token": [float(x) for x in 
        "hidden_max_abs": float(np.max(np.abs(hid["CPU"] - hid["B200_0"]))), "kv_max_abs": kv_err,
        "argmax_agree": float(np.mean(out["CPU"].argmax(1) == out["B200_0"].argmax(1))),
        "launches_per_token": launches, "n_layer": n_layer, "graph_nodes": models["B200_0"].graph_nodes,
+       "unsupported_nodes": int(models["B200_0"].unsupported_nodes),
        "fused_steps": int(plug.ggml_backend_b200_fused_steps() - fused0), "graph_builds": int(models["B200_0"].graph_builds),
-       "graph_replays": int(plug.ggml_backend_b200_graph_replays())}
+       "graph_replays": int(plug.ggml_backend_b200_graph_replays()), "types": sorted({int(t) for t in types.values()})}
 print(json.dumps(res))

@@ -20,7 +20,7 @@ def main():
     w = (0.1 + 2.0 * np.cos(i + 0.0)).reshape(N, K).astype(np.float32) * 0.05
     x = (0.1 + 2.0 * np.cos(np.arange(K, dtype=np.float32) + 1.0)).astype(np.float32)
     out = {"w": w, "x": x}
-    for t in O.QUANT_TYPES:
+    for t in O.GOLDEN_TYPES:
         n = O.TYPE_NAME[t]
         blocks = r.quantize(t, w)
         out[f"{n}_blocks"] = blocks

@@ -4,7 +4,7 @@ CUDA kernels are checked against real reference arithmetic on machines without t
 
 Per type: ggml_quantize_chunk blocks of seeded f32 weights, their dequantize_row_* rows, the q8_0 (Q4_0, Q5_0) or q8_1 (Q4_1) activation
 the CPU quantizes for that type, and gref_mul_mat at T = 1 and T > 1 (K = 512 and K = 7 392 = 231 x 32, a row that is not a multiple of
-256).  Per model: 40 tokens of gref_decode logits of the two tiny models of tests/legacy_types.py (weights regenerated from seeds):
+256).  Per model: 40 tokens of gref_decode logits of tiny_model.legacy_golden_models() (weights regenerated from seeds):
 a Qwen2 Q4_K_M with n_ff % 256 != 0 (ffn_down Q5_0 in layer 0, Q8_0 in layer 1) and a llama Q4_0 (Q6_K head, Q4_0 everywhere else)."""
 import sys
 from pathlib import Path
@@ -13,8 +13,8 @@ import numpy as np
 
 HERE = Path(__file__).resolve().parent
 sys.path.insert(0, str(HERE.parent))
-import legacy_types as L  # noqa: E402
 import oracle_lib as O  # noqa: E402
+from tiny_model import legacy_golden_models  # noqa: E402
 
 MULMAT_CASES = [(16, 512, 1), (12, 7392, 3)]   # N, K, T
 
@@ -30,16 +30,16 @@ def main():
     assert O.build_ref(), "the reference tree is needed to record the golden file"
     r = O.Ref()
     out = {}
-    for t in L.LEGACY_TYPES:
-        n = L.NAME[t]
+    for t in (O.Q4_0, O.Q4_1, O.Q5_0):
+        n = O.TYPE_NAME[t]
         for i, (N, K, T) in enumerate(MULMAT_CASES):
             w, x = mulmat_inputs(t, i, N, K, T)
-            blocks = L.ref_quantize(r, t, w)
+            blocks = r.quantize(t, w)
             out[f"{n}_{i}_blocks"] = blocks
-            out[f"{n}_{i}_dequant"] = L.ref_dequantize(r, t, blocks, K)
-            out[f"{n}_{i}_act"] = np.stack([L.ref_quantize_act(r, t, x[j]) for j in range(T)])
+            out[f"{n}_{i}_dequant"] = r.dequantize(t, blocks, K)
+            out[f"{n}_{i}_act"] = np.stack([r.quantize_act(t, x[j]) for j in range(T)])
             out[f"{n}_{i}_mulmat"] = r.mul_mat(t, blocks, N, K, x)
-    for name, (tm, toks) in L.models().items():
+    for name, (tm, toks) in legacy_golden_models().items():
         logits, hidden = tm.ref_decode(r, toks)
         out[f"{name}_tokens"] = np.asarray(toks, np.int32)
         out[f"{name}_logits"] = logits

@@ -18,10 +18,19 @@ ROOT = Path(__file__).resolve().parent.parent
 ORACLE = ROOT / "oracle"
 
 # enum ggml_type (ggml/include/ggml.h:356-395)
-F32, F16, Q5_1, Q8_0, Q4_K, Q5_K, Q6_K = 0, 1, 7, 8, 12, 13, 14
-TYPE_NAME = {F32: "f32", F16: "f16", Q5_1: "q5_1", Q8_0: "q8_0", Q4_K: "q4_K", Q5_K: "q5_K", Q6_K: "q6_K"}
-BLOCK = {Q4_K: (256, 144), Q5_K: (256, 176), Q6_K: (256, 210), Q8_0: (32, 34), Q5_1: (32, 24), F32: (1, 4), F16: (1, 2)}
-QUANT_TYPES = [Q4_K, Q5_K, Q6_K, Q8_0, Q5_1]
+F32, F16, Q4_0, Q4_1, Q5_0, Q5_1, Q8_0, Q4_K, Q5_K, Q6_K = 0, 1, 2, 3, 6, 7, 8, 12, 13, 14
+TYPE_NAME = {F32: "f32", F16: "f16", Q4_0: "q4_0", Q4_1: "q4_1", Q5_0: "q5_0", Q5_1: "q5_1", Q8_0: "q8_0", Q4_K: "q4_K", Q5_K: "q5_K",
+             Q6_K: "q6_K"}
+# (elements, bytes) per block: ggml/src/ggml-common.h:143-335
+BLOCK = {Q4_K: (256, 144), Q5_K: (256, 176), Q6_K: (256, 210), Q8_0: (32, 34), Q5_1: (32, 24), Q4_0: (32, 18), Q4_1: (32, 20),
+         Q5_0: (32, 22), F32: (1, 4), F16: (1, 2)}
+KQ = [Q4_K, Q5_K, Q6_K]
+BLK32 = [Q8_0, Q5_1, Q4_0, Q4_1, Q5_0]                  # the 32-element block types
+QUANT_TYPES = KQ + BLK32
+GOLDEN_TYPES = KQ + [Q8_0, Q5_1]                        # the types kquants_golden.npz and reference_golden.npz hold
+# the format the CPU quantizes the activation to for each weight type (its vec_dot_type, ggml.c type-traits table :732-1100)
+ACT_TYPE = {Q4_K: "q8_K", Q5_K: "q8_K", Q6_K: "q8_K", Q8_0: "q8_0", Q4_0: "q8_0", Q5_0: "q8_0", Q5_1: "q8_1", Q4_1: "q8_1"}
+ACT_BLOCK = {"q8_K": (256, 292), "q8_0": (32, 34), "q8_1": (32, 36)}
 
 
 def row_size(t: int, k: int) -> int:
@@ -207,11 +216,10 @@ class Ref:
         g.ggml_free(g.ggml_init(_IP(1 << 16, None, False)))
         g.ggml_quantize_chunk.restype = C.c_size_t
         g.ggml_quantize_chunk.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]
-        g.quantize_row_q8_K.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-        g.quantize_row_q8_0.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-        g.quantize_row_q8_1.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-        for n in ("q4_K", "q5_K", "q6_K", "q8_0", "q5_1"):
-            getattr(g, f"dequantize_row_{n}").argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        for n in ACT_BLOCK:
+            getattr(g, f"quantize_row_{n}").argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+        for t in QUANT_TYPES:
+            getattr(g, f"dequantize_row_{TYPE_NAME[t]}").argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
         self.graph.gref_mul_mat.argtypes = [C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int]
         self.graph.gref_create.restype = C.c_void_p
         self.graph.gref_create.argtypes = [C.POINTER(Model), C.c_int]
@@ -238,15 +246,10 @@ class Ref:
 
     def quantize_act(self, wtype: int, x: np.ndarray) -> np.ndarray:
         x = np.ascontiguousarray(x, dtype=np.float32)
-        if wtype in (Q4_K, Q5_K, Q6_K):
-            q = np.zeros(x.size // 256 * 292, dtype=np.uint8)
-            self.ggml.quantize_row_q8_K(_ptr(x), _ptr(q), x.size)
-        elif wtype == Q8_0:
-            q = np.zeros(x.size // 32 * 34, dtype=np.uint8)
-            self.ggml.quantize_row_q8_0(_ptr(x), _ptr(q), x.size)
-        else:
-            q = np.zeros(x.size // 32 * 36, dtype=np.uint8)
-            self.ggml.quantize_row_q8_1(_ptr(x), _ptr(q), x.size)
+        a = ACT_TYPE[wtype]
+        be, bb = ACT_BLOCK[a]
+        q = np.zeros(x.size // be * bb, dtype=np.uint8)
+        getattr(self.ggml, f"quantize_row_{a}")(_ptr(x), _ptr(q), x.size)
         return q
 
     def mul_mat(self, t: int, W: np.ndarray, N: int, K: int, x: np.ndarray, n_threads: int | None = None) -> np.ndarray:
@@ -293,20 +296,31 @@ def synth_blocks(t: int, N: int, K: int, seed: int, scale: float = 1.0) -> np.nd
         out[:, 0:2] = _f16_bits(d).view(np.uint8).reshape(nb, 2)
         out[:, 2:4] = _f16_bits(m).view(np.uint8).reshape(nb, 2)
         out[:, 4:] = rng.integers(0, 256, (nb, 20), dtype=np.uint8)
+    elif t in (Q4_0, Q4_1, Q5_0):       # q uniform: (q - 8) d, q d + m, (q - 16) d
+        d = (rng.uniform(0.5, 1.5, nb) * s / (9.0 if t == Q5_0 else 4.5)).astype(np.float32)
+        out[:, 0:2] = d.astype(np.float16).view(np.uint8).reshape(nb, 2)
+        if t == Q4_1:
+            m = -d * 7.5 * rng.uniform(0.9, 1.1, nb).astype(np.float32)
+            out[:, 2:4] = m.astype(np.float16).view(np.uint8).reshape(nb, 2)
+            out[:, 4:] = rng.integers(0, 256, (nb, 16), dtype=np.uint8)
+        else:
+            out[:, 2:] = rng.integers(0, 256, (nb, bb - 2), dtype=np.uint8)
     else:
         raise ValueError(t)
     return out.reshape(-1)
 
 
 # byte ranges of the quants and of the block scale d inside one block
-_QBYTES = {Q4_K: slice(16, 144), Q5_K: slice(16, 176), Q6_K: slice(0, 192), Q8_0: slice(2, 34), Q5_1: slice(4, 24)}
-_DBYTES = {Q4_K: slice(0, 2), Q5_K: slice(0, 2), Q6_K: slice(208, 210), Q8_0: slice(0, 2), Q5_1: slice(0, 2)}
+_QBYTES = {Q4_K: slice(16, 144), Q5_K: slice(16, 176), Q6_K: slice(0, 192), Q8_0: slice(2, 34), Q5_1: slice(4, 24), Q4_0: slice(2, 18),
+           Q4_1: slice(4, 20), Q5_0: slice(2, 22)}
+_DBYTES = {t: slice(208, 210) if t == Q6_K else slice(0, 2) for t in QUANT_TYPES}
 
 
 def edge_blocks(t: int, N: int, K: int, seed: int) -> np.ndarray:
     """synth_blocks with the bit patterns random blocks (almost) never hold, by row r % 6: 0 random; 1 every quant byte 0x00; 2 every
     quant byte 0xFF; 3 the type's extreme: Q8_0 q = -128, Q6_K sub-block scales -128 with q = -32, Q4_K / Q5_K 6-bit scales and mins all
-    63, Q5_1 offset m = 0 with q = 31; 4 d = 0 in every block; 5 d = 0 in every other block."""
+    63, Q5_1 / Q4_1 offset m = 0 with q = 31 / 15, Q4_0 / Q5_0 q - 8 = -8 / q - 16 = -16 (the largest magnitude); 4 d = 0 in every block;
+    5 d = 0 in every other block."""
     be, bb = BLOCK[t]
     b = synth_blocks(t, N, K, seed).reshape(N, K // be, bb)
     q, dd = _QBYTES[t], _DBYTES[t]
@@ -319,9 +333,11 @@ def edge_blocks(t: int, N: int, K: int, seed: int) -> np.ndarray:
         b[3::6, :, 192:208] = 0x80
     elif t in (Q4_K, Q5_K):
         b[3::6, :, 4:16] = 0xFF
-    else:
+    elif t in (Q5_1, Q4_1):
         b[3::6, :, 2:4] = 0x00
         b[3::6, :, q] = 0xFF
+    else:
+        b[3::6, :, q] = 0x00
     b[4::6, :, dd] = 0x00
     b[5::6, ::2, dd] = 0x00
     return b.reshape(-1)

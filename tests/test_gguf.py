@@ -6,12 +6,42 @@ import ctypes as C
 import numpy as np
 import pytest
 
+import oracle_lib as O
 from tiny_model import TinyModel
 
 
 def _tiny(arch="llama", **kw):
     return TinyModel(n_layer=2, n_embd=512, n_head=4, n_head_kv=2, n_ff=1024, n_vocab=320, n_ctx=64, arch=arch,
                      ftype="q4_K_M" if arch == "llama" else "q5_K_M", seed=4, branch_scale=0.1, freq_factors=(arch == "llama"), **kw)
+
+
+def _q4_0_mix():
+    """A Q4_0 model whose ffn_down are Q4_1 (the reference's imatrix rule for the first layers) and attn_output Q5_0."""
+    tm = TinyModel.q4_0(4, n_layer=2, n_embd=512, n_head=4, n_head_kv=2, n_ff=1024, n_vocab=320, n_ctx=64)
+    for il in range(2):
+        tm.retype(f"blk.{il}.ffn_down.weight", O.Q4_1, 70 + il)
+        tm.retype(f"blk.{il}.attn_output.weight", O.Q5_0, 80 + il)
+    return tm
+
+
+@pytest.mark.parametrize("t,bpb", [(O.Q4_0, 18), (O.Q4_1, 20), (O.Q5_0, 22)])
+def test_row_bytes(lib, t, bpb):
+    for k in (32, 4096, 7392, 29568):
+        assert lib.c.pb200_row_bytes(t, k) == k // 32 * bpb == O.row_size(t, k)
+
+
+def test_probe_accepts_the_legacy_types(pkg, tmp_path):
+    """A Q4_0 file with a Q4_1 ffn_down and a Q5_0 attn_output: the parser sizes every tensor of the three types."""
+    tm = _q4_0_mix()
+    assert {t for t, _ in tm.tensors.values()} == {O.F32, O.Q4_0, O.Q4_1, O.Q5_0, O.Q6_K}
+    path = tmp_path / "q4_0.gguf"
+    tm.write_gguf(path)
+    lib = pkg.Lib.get()
+    hp = pkg.HParams()
+    n, nbytes, a = C.c_int32(), C.c_int64(), C.create_string_buffer(16)
+    assert lib.c.pb200_gguf_probe(str(path).encode(), C.byref(hp), C.byref(n), C.byref(nbytes), a) == 0
+    assert a.value.decode() == "llama" and n.value == len(tm.tensors) and hp.n_ff == 1024
+    assert nbytes.value >= sum(np.asarray(a_).nbytes for _, a_ in tm.tensors.values())
 
 
 @pytest.mark.parametrize("arch", ["llama", "qwen2"])
@@ -74,7 +104,6 @@ def test_probe_accepts_version_2_and_custom_alignment(pkg, tmp_path):
         if t == 0:
             w.add_tensor(name, np.ascontiguousarray(a, dtype=np.float32))
         else:
-            import oracle_lib as O
             w.add_tensor(name, np.ascontiguousarray(a).view(np.uint8).reshape(-1, O.row_size(t, tm._row_len(name))), raw_dtype=gguf.GGMLQuantizationType(t))
     w.write_header_to_file(); w.write_kv_data_to_file(); w.write_tensors_to_file(); w.close()
     nb = C.c_int64()
@@ -83,10 +112,7 @@ def test_probe_accepts_version_2_and_custom_alignment(pkg, tmp_path):
     assert (al.stat().st_size - nb.value) % 64 == 0                          # the data section starts on the custom alignment
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("arch", ["llama", "qwen2"])
-def test_gguf_loaded_model_decodes_like_set_tensor_model(cuda, pkg, tmp_path, arch):
-    tm = _tiny(arch)
+def check_gguf_load(pkg, tmp_path, tm):
     path = tmp_path / "m.gguf"
     tm.write_gguf(path)
     toks = [(i * 7919 + 13) % 320 for i in range(8)]
@@ -113,3 +139,15 @@ def test_gguf_loaded_model_decodes_like_set_tensor_model(cuda, pkg, tmp_path, ar
         s1.decode(int(t), i, got2[i])
     s0.close(); s1.close()
     assert np.array_equal(got2, want)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("arch", ["llama", "qwen2"])
+def test_gguf_loaded_model_decodes_like_set_tensor_model(cuda, pkg, tmp_path, arch):
+    check_gguf_load(pkg, tmp_path, _tiny(arch))
+
+
+@pytest.mark.gpu
+def test_gguf_loaded_legacy_types_model_decodes_like_set_tensor_model(cuda, pkg, tmp_path):
+    """A Q4_0 file with a Q4_1 ffn_down and a Q5_0 attn_output."""
+    check_gguf_load(pkg, tmp_path, _q4_0_mix())

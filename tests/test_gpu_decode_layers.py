@@ -18,7 +18,7 @@ checked on the values the device itself handed it, so errors never compound and 
 The attention bar is test_attn_decode's (max 3e-4, mean 2e-5) plus f16_flip_slack: for the few cells whose probability lies within
 the derived f32 error of an f16 rounding boundary, one f16 step times |V|.  Both sides round p to f16, and where the device's expf
 ulps tip one to the other side of a boundary near p = 1 that is worth up to |V| 2^-11.  The GEMV bar is that of test_gpu_gemv_shapes.Scattered.check: 4e-6 max(1, max |ref|), the
-fp32 summation order.  The oracle is the C port (k-quants, Q8_0, Q5_1) or legacy_types' restatement (Q4_0, Q4_1, Q5_0); it quantizes the activation exactly as the device's
+fp32 summation order.  The oracle is the C port; it quantizes the activation exactly as the device's
 producers do (same f32 input, same block scale arithmetic), so a quantization code that differs shows up as a GEMV error.
 
 decode_launches() restates the branch choices of launch_gemv (gemv.cu) and launch_attn_step (ops.cu): the distributed prologue inside
@@ -34,10 +34,9 @@ import numpy as np
 import pytest
 import torch
 
-import legacy_types as L
 import oracle_lib as O
 from gpu_util import dev_f32, ptr, sync
-from test_gpu_gemv_shapes import BLK32, KQ, gemv_plan, oracle_mul_mat
+from test_gpu_gemv_shapes import gemv_plan
 from test_gpu_kv_shift import _dev, kv_tensors, load
 from tiny_model import TinyModel, use_more_bits
 
@@ -49,7 +48,7 @@ ACT_MAX_NBLK = 116
 
 def act_mode(t):
     """common.cuh act_mode_for: the CPU's vec_dot_type of the weight type."""
-    return ACT_Q8_K if t in KQ else (ACT_Q8_1 if t in (O.Q5_1, L.Q4_1) else ACT_Q8_0)
+    return {"q8_K": ACT_Q8_K, "q8_0": ACT_Q8_0, "q8_1": ACT_Q8_1}[O.ACT_TYPE[t]]
 
 
 # ---- the branch choices of one decode step, restated ----
@@ -58,7 +57,7 @@ def gemv_kernels(types, Ns, K):
     k_gemv_generic.  Weights are 256-byte aligned in the engine."""
     if gemv_plan(types, Ns, K):
         return 1, "ring"
-    kinds = ["ring" if t in BLK32 and gemv_plan((t,), (N,), K) else "generic" for t, N in zip(types, Ns)]
+    kinds = ["ring" if t in O.BLK32 and gemv_plan((t,), (N,), K) else "generic" for t, N in zip(types, Ns)]
     return len(kinds), ",".join(kinds)
 
 
@@ -67,7 +66,7 @@ def gemv_launches(types, Ns, K, pro):
     1. rms_norm / silu_mul on a k-quant group that fits the ring: one launch, the prologue distributed over its CTAs ("dist");
     2. one activation mode: a producer kernel unless the activation is ready, then the kernels ("producer" / "ready");
     3. several modes: rms_norm * w to an f32 scratch, then per mode a quantize kernel and that mode's kernels ("modes")."""
-    if pro in ("rms_norm", "silu_mul") and all(t in KQ for t in types) and gemv_plan(types, Ns, K):
+    if pro in ("rms_norm", "silu_mul") and all(t in O.KQ for t in types) and gemv_plan(types, Ns, K):
         return 1, "dist"
     modes = list(dict.fromkeys(act_mode(t) for t in types))
     if len(modes) == 1:
@@ -128,16 +127,16 @@ def _qwen2_q4_K_M(seed, n_ctx):
     tm = TinyModel(n_layer=3, n_embd=1024, n_head=8, n_head_kv=2, n_ff=1152, n_vocab=512, n_ctx=n_ctx, arch="qwen2", ftype="q4_K_M",
                    seed=seed, branch_scale=0.1, types={"ffn_down": O.Q5_K})
     for il in range(3):
-        L.retype(tm, f"blk.{il}.ffn_down.weight", O.Q8_0 if use_more_bits(il, 3) else L.Q5_0, 500 + il)
+        tm.retype(f"blk.{il}.ffn_down.weight", O.Q8_0 if use_more_bits(il, 3) else O.Q5_0, 500 + il)
     return tm
 
 
 def _llama_q4_0(seed, n_ctx):
     """The Q4_0 mixture (a Q6_K head) with the imatrix rule's Q4_1 ffn_down in layers 0 and 1 and a Q5_0 attn_output in layer 0."""
-    tm = L.q4_0_model(seed, n_layer=3, n_embd=1024, n_head=8, n_head_kv=2, n_ff=2048, n_vocab=512, n_ctx=n_ctx)
+    tm = TinyModel.q4_0(seed, n_layer=3, n_embd=1024, n_head=8, n_head_kv=2, n_ff=2048, n_vocab=512, n_ctx=n_ctx)
     for il in range(2):
-        L.retype(tm, f"blk.{il}.ffn_down.weight", L.Q4_1, 600 + il)
-    L.retype(tm, "blk.0.attn_output.weight", L.Q5_0, 610)
+        tm.retype(f"blk.{il}.ffn_down.weight", O.Q4_1, 600 + il)
+    tm.retype("blk.0.attn_output.weight", O.Q5_0, 610)
     return tm
 
 
@@ -277,9 +276,9 @@ def check_bits(where, got, want):
 
 
 def dequant_row(port, t, W, K, row):
-    rb = L.row_size(t, K)
+    rb = O.row_size(t, K)
     blk = np.ascontiguousarray(W.reshape(-1)[row * rb:(row + 1) * rb])
-    return L.dequantize(t, blk, K)[0] if t in L.LEGACY_TYPES else port.dequantize(t, blk, K)[0]
+    return port.dequantize(t, blk, K)[0]
 
 
 class Shard:
@@ -327,7 +326,7 @@ def check_step(lib, port, s, tag, pos, slot=0, check_att=True, f32_scratch_att=F
 
     def mm(name, xin, N, K):
         t, W = w[name]
-        return oracle_mul_mat(port, t, W, N, K, xin)[0]
+        return port.mul_mat(t, W, N, K, xin)[0]
 
     def bias(name, n):
         return w[name][1] if name in w else np.zeros(n, np.float32)
@@ -514,6 +513,27 @@ def synth_weights(eng, hp, il):
 
 
 @pytest.mark.gpu
+def test_synth_qwen72b_types(cuda, pkg):
+    """pb200_model_synth(ftype 0) on two Qwen2.5-72B layers: the reference's Q4_K_M types tensor by tensor (80 layers = MODEL_70B: attn_v
+    Q5_K; n_ff 29 568: ffn_down Q4_K -> Q5_0, or Q6_K -> Q8_0 in the use_more_bits layers), and ftype 2 gives Q4_0 everywhere."""
+    hp = pkg.HParams(**QWEN72B)
+    want = {0: {11: {"attn_v": O.Q5_K, "ffn_down": O.Q5_0}, 12: {"attn_v": O.Q6_K, "ffn_down": O.Q8_0}},
+            2: {11: {"attn_v": O.Q4_0, "ffn_down": O.Q4_0}, 12: {"attn_v": O.Q4_0, "ffn_down": O.Q4_0}}}
+    for ftype, layers in want.items():
+        m = pkg.Model(hp, 0, (11, 13), False, False)
+        m.synth(ftype, 5)
+        default = O.Q4_K if ftype == 0 else O.Q4_0
+        for il, special in layers.items():
+            for w, K in (("attn_q", 8192), ("attn_k", 8192), ("attn_v", 8192), ("attn_output", 8192), ("ffn_gate", 8192), ("ffn_up", 8192),
+                         ("ffn_down", 29568)):
+                _, nbytes, t = m.tensor_device(f"blk.{il}.{w}.weight")
+                assert t == special.get(w, default), (ftype, il, w, t)
+                N = {"attn_k": 1024, "attn_v": 1024, "ffn_gate": 29568, "ffn_up": 29568}.get(w, 8192)
+                assert nbytes == O.row_size(t, K) * N
+        m.close()
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("model,ftype,il", FULL, ids=[f"{m}-ftype{f}-layer{il}" for m, f, il in FULL])
 def test_full_size_layer_vs_oracle(cuda, lib, pkg, port, model, ftype, il):
     hp = dict(QWEN72B if model == "qwen2.5-72b" else LLAMA8B)
@@ -524,7 +544,7 @@ def test_full_size_layer_vs_oracle(cuda, lib, pkg, port, model, ftype, il):
     try:
         types = layer_types(s.w, il)
         if model == "qwen2.5-72b" and ftype == 0:
-            assert (types["down"], types["v"]) == ((L.Q5_0, O.Q5_K) if il == 11 else (O.Q8_0, O.Q6_K)), types
+            assert (types["down"], types["v"]) == ((O.Q5_0, O.Q5_K) if il == 11 else (O.Q8_0, O.Q6_K)), types
         rng = np.random.default_rng(il)
         s.fill(0, 37, rng)
         for p in (37, 38):

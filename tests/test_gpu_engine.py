@@ -7,7 +7,7 @@ import pytest
 
 import oracle_lib as O
 from golden import make_reference_golden as RG
-from tiny_model import TinyModel, from_golden
+from tiny_model import TinyModel, from_golden, legacy_golden_models
 
 pytestmark = pytest.mark.gpu
 G = Path(__file__).resolve().parent / "golden"
@@ -40,6 +40,41 @@ def test_engine_matches_golden_reference_logits(cuda, pkg, arch):
     assert np.max(np.abs(out - logits)) < TOL, np.max(np.abs(out - logits))
     assert np.array_equal(out.argmax(1), logits.argmax(1))
     eng.close()
+
+
+@pytest.mark.parametrize("name", ["qwen2_q4_K_M", "llama_q4_0"])
+def test_engine_decode_vs_reference(cuda, pkg, name):
+    """A golden legacy-type model: 40 tokens against the compiled reference's graph on the same weights (recorded), under the multi-token
+    parity bar."""
+    tm, toks = legacy_golden_models()[name]
+    eng = tm.load_engine(pkg)
+    got = np.zeros((len(toks), tm.hp["n_vocab"]), np.float32)
+    for i, tk in enumerate(toks):
+        eng.decode(int(tk), i, got[i])
+    eng.close()
+    check_decode_parity(got, np.load(G / "legacy_types_golden.npz")[f"{name}_logits"])
+
+
+@pytest.mark.parametrize("name", ["qwen2_q4_K_M", "llama_q4_0"])
+def test_engine_prefill_then_decode(cuda, pkg, name):
+    """A golden legacy-type model's 24-token prompt through pb200_prefill (tensor-core mat-muls, the Q5_0 / Q4_0 weights expanded to
+    fp16), then 8 decode steps: the prompt's last logits and every step after it agree with token-by-token decode (NMSE 1e-3, the
+    prefill bar of the smoke run)."""
+    tm, toks = legacy_golden_models()[name]
+    nv = tm.hp["n_vocab"]
+    eng = tm.load_engine(pkg)
+    seq = np.zeros((32, nv), np.float32)
+    for i in range(32):
+        eng.decode(int(toks[i]), i, seq[i])
+    eng.close()
+    eng = tm.load_engine(pkg)
+    got = [eng.prefill(toks[:24], 0)]
+    for i in range(24, 32):
+        got.append(eng.decode(int(toks[i]), i, np.zeros(nv, np.float32)))
+    eng.close()
+    for j, g in enumerate(got):
+        w = seq[23 + j]
+        assert np.sum((g - w) ** 2) / np.sum(w ** 2) < 1e-3, j
 
 
 # Why branch_scale: activation quantization q = round(x * 127/amax) turns a 1-ulp fp32 difference in x (summation order of

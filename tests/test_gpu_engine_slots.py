@@ -12,7 +12,6 @@ import numpy as np
 import pytest
 import torch
 
-import legacy_types as L
 from tiny_model import TinyModel
 
 pytestmark = pytest.mark.gpu
@@ -27,7 +26,7 @@ def q4_k_m():
 
 
 def q4_0():
-    return L.q4_0_model(22, **SHAPE)
+    return TinyModel.q4_0(22, **SHAPE)
 
 
 def load(tm, pkg, n_seq=N_SEQ, layers=None, with_embd=True, with_head=True):

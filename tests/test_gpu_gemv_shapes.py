@@ -19,14 +19,11 @@ import numpy as np
 import pytest
 import torch
 
-import legacy_types as L
 import oracle_lib as O
 from gpu_util import act_ws, act_ws_fields, dev_f32, ptr, sync
 from test_gpu_fallbacks import GemvMat
 
-KQ = [O.Q4_K, O.Q5_K, O.Q6_K]
-BLK32 = [O.Q8_0, O.Q5_1, L.Q4_0, L.Q4_1, L.Q5_0]   # the 32-element block types (common.cuh is_blk32_type)
-TN = O.TYPE_NAME | L.NAME
+KQ, BLK32, TN = O.KQ, O.BLK32, O.TYPE_NAME   # BLK32: common.cuh is_blk32_type
 ENOTSUP = -3
 U_ROWS = 2048              # unique rows per matrix
 SWEEP_BYTES = 192 << 20    # weight bytes per sweep case: >= 3 turns of every CTA's ring whatever depth the plan picks
@@ -53,7 +50,7 @@ def gemv_plan(types, Ns, K):
     rpw = 1 if wpr > 1 else 32 // nbp
     rows, biggest = [], 0
     for t, N in zip(types, Ns):
-        rb = L.row_size(t, K)
+        rb = O.row_size(t, K)
         if not (t in KQ or b32) or (b32 and rb % 8):           # the column dots read 64-bit words
             return None
         R = max(rpw, max(1, STAGE_TARGET // rb) // rpw * rpw)
@@ -94,7 +91,7 @@ def ring_turns(p, sms):
 
 # ---- sweep cases: (weight types of the group, K, rows of each matrix) ----
 def _n_for(t, K, n_min=1):
-    return max(n_min, -(-SWEEP_BYTES // L.row_size(t, K)))
+    return max(n_min, -(-SWEEP_BYTES // O.row_size(t, K)))
 
 
 SWEEP_K = [768, 1280, 1536, 3072, 3584, 4096, 5120, 8192, 8448, 8960, 13824, 14336, 16384, 16640, 18944, 27648, 28672, 29696]
@@ -104,8 +101,8 @@ SWEEP += [((O.Q5_1,), 7392, (_n_for(O.Q5_1, 7392, 8192),))]
 # q|k|v-like groups at K 8192: mixed types (the TYPE = 0 instantiation, unequal R), one type with R 5 and a 1-row last tile (owner_only off)
 SWEEP += [((O.Q4_K, O.Q4_K, O.Q6_K), 8192, (24576, 8192, 8192)), ((O.Q5_K, O.Q5_K, O.Q5_K), 8192, (24576, 4096, 4101))]
 # Q4_0 / Q4_1 / Q5_0 at Llama-3-8B's K, a Q4_1 K whose last 8-block column holds 2 blocks, and Qwen2.5-72B Q4_K_M's Q5_0 ffn_down
-SWEEP += [((t,), K, (_n_for(t, K),)) for t in L.LEGACY_TYPES for K in (4096, 8192, 14336)]
-SWEEP += [((L.Q4_1,), 4160, (_n_for(L.Q4_1, 4160),)), ((L.Q5_0,), 29568, (_n_for(L.Q5_0, 29568, 8192),))]
+SWEEP += [((t,), K, (_n_for(t, K),)) for t in (O.Q4_0, O.Q4_1, O.Q5_0) for K in (4096, 8192, 14336)]
+SWEEP += [((O.Q4_1,), 4160, (_n_for(O.Q4_1, 4160),)), ((O.Q5_0,), 29568, (_n_for(O.Q5_0, 29568, 8192),))]
 
 
 def sweep_id(case):
@@ -126,9 +123,9 @@ FAMILIES = {
     ((O.Q4_K,), 18944): dict(wpr=4, rows=[2]),
     ((O.Q4_K, O.Q4_K, O.Q6_K), 8192): dict(owner_only=False),
     ((O.Q5_K, O.Q5_K, O.Q5_K), 8192): dict(owner_only=False),
-    ((L.Q4_0,), 4096): dict(wpr=1, rpw=2, rows=[12], nstage=4, owner_only=True),              # Llama-3-8B Q4_0 q, k, v, wo, gate, up
-    ((L.Q4_0,), 14336): dict(wpr=2, rows=[2], nstage=6, nstage_init=4, owner_only=True),       # Llama-3-8B Q4_0 ffn_down
-    ((L.Q5_0,), 29568): dict(wpr=4, rows=[1], nstage=4, nstage_init=2, owner_only=True),       # Qwen2.5-72B Q4_K_M ffn_down
+    ((O.Q4_0,), 4096): dict(wpr=1, rpw=2, rows=[12], nstage=4, owner_only=True),              # Llama-3-8B Q4_0 q, k, v, wo, gate, up
+    ((O.Q4_0,), 14336): dict(wpr=2, rows=[2], nstage=6, nstage_init=4, owner_only=True),       # Llama-3-8B Q4_0 ffn_down
+    ((O.Q5_0,), 29568): dict(wpr=4, rows=[1], nstage=4, nstage_init=2, owner_only=True),       # Qwen2.5-72B Q4_K_M ffn_down
 }
 
 
@@ -145,21 +142,13 @@ def test_sweep_cases_wrap_their_rings():
         assert {k: p[k] for k in want} == want, (sweep_id(case), p)
     # rows that are not 8-byte multiples leave the ring: Q8_0 at K 7392, Q4_0 / Q5_0 at K 4160 (130 blocks of 18 / 22 bytes)
     assert gemv_plan((O.Q8_0,), (4096,), 7392) is None and gemv_plan((O.Q5_1,), (4096,), 7392) is not None
-    assert gemv_plan((L.Q4_0,), (4096,), 4160) is None and gemv_plan((L.Q5_0,), (4096,), 4160) is None
-    assert gemv_plan((L.Q4_1,), (4096,), 4160) is not None
+    assert gemv_plan((O.Q4_0,), (4096,), 4160) is None and gemv_plan((O.Q5_0,), (4096,), 4160) is None
+    assert gemv_plan((O.Q4_1,), (4096,), 4160) is not None
     # 32-element block types take the ring one matrix at a time
-    assert gemv_plan((L.Q4_0, L.Q4_0), (4096, 1024), 4096) is None and gemv_plan((O.Q4_K, O.Q4_K), (4096, 1024), 4096) is not None
+    assert gemv_plan((O.Q4_0, O.Q4_0), (4096, 1024), 4096) is None and gemv_plan((O.Q4_K, O.Q4_K), (4096, 1024), 4096) is not None
 
 
 # ---- device helpers ----
-def oracle_mul_mat(port, t, W, N, K, x):
-    """The CPU's mat-vec for any weight type: the C port, or legacy_types' restatement for Q4_0 / Q4_1 / Q5_0."""
-    return L.mul_mat(port, t, W, N, K, x) if t in L.LEGACY_TYPES else port.mul_mat(t, W, N, K, x)
-
-
-def oracle_quantize_act(port, t, x):
-    return L.quantize_act(port, t, x) if t in L.LEGACY_TYPES else port.quantize_act(t, x)
-
 
 def _fused(lib):
     fn = lib.c.pb200_gemv_fused
@@ -176,8 +165,8 @@ class Scattered:
     def __init__(self, t, N, K, seed, with_add=False, U=U_ROWS):
         self.t, self.N, self.K = t, N, K
         self.U = U = min(U, N)
-        rb = L.row_size(t, K)
-        self.Wu = L.synth_blocks(t, U, K, seed=seed)
+        rb = O.row_size(t, K)
+        self.Wu = O.synth_blocks(t, U, K, seed=seed)
         self.src = (torch.randperm(N, generator=torch.Generator().manual_seed(seed)) % U).numpy()
         Wud = torch.from_numpy(self.Wu.reshape(U, rb)).cuda()
         self.W = torch.zeros(N * rb + 64, dtype=torch.uint8, device="cuda")
@@ -194,7 +183,7 @@ class Scattered:
 
     def check(self, port, x, what, add_rows=None):
         """y against the oracle's mat-vec of the source rows on activation x (+ the per-source add, or add_rows per row)."""
-        want_u = oracle_mul_mat(port, self.t, self.Wu, self.U, self.K, x)[0]
+        want_u = port.mul_mat(self.t, self.Wu, self.U, self.K, x)[0]
         if self.add_u is not None:
             want_u = want_u + self.add_u
         want = want_u[self.src]
@@ -273,8 +262,7 @@ def run_blk32(lib, port, ms, K, prologue, eps=1e-5, seed=0, what=""):
         lib.check(lib.c.pb200_mul_mat_vec_q(m.t, ptr(m.W), m.N, K, ptr(ws), ptr(m.y), None, ptr(m.add) if m.add is not None else None, None),
                   "mul_mat_vec_q")
         _no_abort(lib, what)
-        mode = "q8_1" if m.t in (O.Q5_1, L.Q4_1) else "q8_0"
-        assert np.array_equal(act_ws_fields(ws, K, mode), oracle_quantize_act(port, m.t, x)), f"{what} matrix {i}: act_ws differs"
+        assert np.array_equal(act_ws_fields(ws, K, O.ACT_TYPE[m.t]), port.quantize_act(m.t, x)), f"{what} matrix {i}: act_ws differs"
         m.check(port, x, f"{what} matrix {i}")
 
 
@@ -283,7 +271,7 @@ MODELS = {   # bench.py's hyper-parameters; default weight type of the mixture (
     "llama3-8b": dict(E=4096, QD=4096, EK=1024, F=14336, V=128256, t=O.Q4_K, eps=1e-5, qwen=False),
     "llama3-70b": dict(E=8192, QD=8192, EK=1024, F=28672, V=128256, t=O.Q4_K, eps=1e-5, qwen=False),
     "qwen2.5-72b": dict(E=8192, QD=8192, EK=1024, F=29568, V=152064, t=O.Q5_K, eps=1e-6, qwen=True),
-    "llama3-8b-q4_0": dict(E=4096, QD=4096, EK=1024, F=14336, V=128256, t=L.Q4_0, eps=1e-5, qwen=False),
+    "llama3-8b-q4_0": dict(E=4096, QD=4096, EK=1024, F=14336, V=128256, t=O.Q4_0, eps=1e-5, qwen=False),
     "qwen2.5-72b-q4_K_M": dict(E=8192, QD=8192, EK=1024, F=29568, V=152064, t=O.Q4_K, eps=1e-6, qwen=True),
 }
 LAUNCHES = ["qkv-v_q5_K", "qkv-v_q6_K", "wo", "gate_up", "down-default", "down-q6_K", "head"]
@@ -301,9 +289,9 @@ def test_model_launch_vs_oracle(cuda, lib, port, model, launch):
     h = MODELS[model]
     E, t, eps, seed = h["E"], h["t"], h["eps"], 1000 * list(MODELS).index(model) + 10 * ALL_LAUNCHES.index(launch)
     what = f"{model} {launch}"
-    if t == L.Q4_0 and launch != "head":
+    if t == O.Q4_0 and launch != "head":
         K, ms, pro = {"qkv": (E, [(t, h["QD"]), (t, h["EK"]), (t, h["EK"])], 1), "wo": (h["QD"], [(t, E)], 0), "gate_up": (E, [(t, h["F"])] * 2, 1),
-                      "down-default": (h["F"], [(t, E)], 2), "down-q4_1": (h["F"], [(L.Q4_1, E)], 2)}[launch]
+                      "down-default": (h["F"], [(t, E)], 2), "down-q4_1": (h["F"], [(O.Q4_1, E)], 2)}[launch]
         run_blk32(lib, port, [Scattered(tt, n, K, seed + i, with_add=pro != 1) for i, (tt, n) in enumerate(ms)], K, pro, eps, seed, what)
     elif launch.startswith("qkv"):
         tv = O.Q5_K if launch.endswith("q5_K") else O.Q6_K
@@ -316,7 +304,7 @@ def test_model_launch_vs_oracle(cuda, lib, port, model, launch):
     elif launch.startswith("down"):
         td = O.Q6_K if launch.endswith("q6_K") else t
         if h["F"] % 256:
-            td = {O.Q4_K: L.Q5_0, O.Q5_K: O.Q5_1, O.Q6_K: O.Q8_0}[td]   # the mixture's fallback types for n_ff % 256 != 0
+            td = {O.Q4_K: O.Q5_0, O.Q5_K: O.Q5_1, O.Q6_K: O.Q8_0}[td]   # the mixture's fallback types for n_ff % 256 != 0
             run_blk32(lib, port, [Scattered(td, E, h["F"], seed, with_add=True)], h["F"], 2, seed=seed, what=f"{what} ({TN[td]})")
         else:
             run_fused(lib, port, [Scattered(td, E, h["F"], seed, with_add=True)], h["F"], 2, eps, seed, what)

@@ -9,6 +9,8 @@ from pathlib import Path
 
 import pytest
 
+import oracle_lib as O
+
 pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parent.parent
 
@@ -38,6 +40,18 @@ def test_whole_graph_matches_cpu_backend_and_is_fused(cuda, arch, dims):
     assert r["fused_steps"] >= 40 * (5 * r["n_layer"]), r["fused_steps"]
     assert r["graph_builds"] <= 3          # one topology per 32-cell bucket of n_kv: the plan is reused token after token
     assert r["graph_replays"] >= 40 - 2 * 3, r["graph_replays"]   # per bucket: one direct call, one capture, then CUDA-graph replays
+
+
+@pytest.mark.parametrize("name,t", [("qwen2_q4_K_M", O.Q5_0), ("llama_q4_0", O.Q4_0)])
+def test_golden_legacy_model_whole_graph(cuda, name, t):
+    """40 decode steps of a golden legacy-type model (tiny_model.legacy_golden_models) through the plugin against the CPU backend.
+    The host stand-in places every node on B200_0 and the plugin refuses a node it does not claim, so the run also shows that no node
+    fell back to the CPU."""
+    r = run(name, 40)
+    assert r["unsupported_nodes"] == 0, r
+    assert r["first_token_err"] < 1e-4, r
+    assert r["nmse"] < 2e-3 and r["max_abs"] < 0.25 and r["argmax_agree"] >= 0.9, r
+    assert t in r["types"], r
 
 
 def test_graph_replay_equals_direct_launches(cuda):

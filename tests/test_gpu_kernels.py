@@ -11,8 +11,7 @@ import oracle_lib as O
 from gpu_util import act_ws, act_ws_fields, dev_f32, dev_u8, ptr, sync
 
 pytestmark = pytest.mark.gpu
-KQ = [O.Q4_K, O.Q5_K, O.Q6_K]
-MODE = {O.Q4_K: "q8_K", O.Q5_K: "q8_K", O.Q6_K: "q8_K", O.Q8_0: "q8_0", O.Q5_1: "q8_1"}
+KQ = O.KQ
 
 
 def rel_tol(ref):
@@ -27,15 +26,18 @@ def test_quantize_act_bit_exact(cuda, lib, port, t):
     cases += [np.zeros(K, np.float32), np.tile(np.array([1.0, -1.0, 0.5, -0.5], np.float32), K // 4),
               np.tile(np.array([-3.0, 3.0, 1.5, 0.0], np.float32), K // 4)]
     z = np.zeros(K, np.float32); z[300] = -2.5; cases.append(z)
-    for offset in (0, 1):   # 1: x one float past a 16-byte boundary, so the kernel must not use its 128-bit loads
-        for x in cases:
-            ws = act_ws(lib, K)
-            xd = dev_f32(np.concatenate([np.zeros(offset, np.float32), x]))
-            lib.check(lib.c.pb200_quantize_act(t, C.c_void_p(xd.data_ptr() + 4 * offset), K, ptr(ws), None), "quantize_act")
-            sync()
-            got = act_ws_fields(ws, K, MODE[t])
-            want = port.quantize_act(t, x)
-            assert np.array_equal(got, want), f"activation quantization differs for {O.TYPE_NAME[t]} (x offset {offset})"
+    cases = [(x, offset) for offset in (0, 1) for x in cases]   # 1: x one float past a 16-byte boundary, so no 128-bit loads
+    if t in O.BLK32:   # Qwen2.5-72B's ffn_down K (29 568) and a K that is not a multiple of 256 (7 392)
+        cases += [(np.random.default_rng(K + t).standard_normal(K).astype(np.float32), 0) for K in (512, 7392, 29568)]
+    for x, offset in cases:
+        K = x.size
+        ws = act_ws(lib, K)
+        xd = dev_f32(np.concatenate([np.zeros(offset, np.float32), x]))
+        lib.check(lib.c.pb200_quantize_act(t, C.c_void_p(xd.data_ptr() + 4 * offset), K, ptr(ws), None), "quantize_act")
+        sync()
+        got = act_ws_fields(ws, K, O.ACT_TYPE[t])
+        want = port.quantize_act(t, x)
+        assert np.array_equal(got, want), f"activation quantization differs for {O.TYPE_NAME[t]} (K {K}, x offset {offset})"
 
 
 @pytest.mark.parametrize("t", KQ, ids=lambda t: O.TYPE_NAME[t])
@@ -54,7 +56,7 @@ def test_gemv_kquant_vs_oracle(cuda, lib, port, t, N, K):
     assert np.max(np.abs(got - want)) <= rel_tol(want), (np.max(np.abs(got - want)), rel_tol(want))
 
 
-@pytest.mark.parametrize("t", [O.Q8_0, O.Q5_1], ids=lambda t: O.TYPE_NAME[t])
+@pytest.mark.parametrize("t", O.BLK32, ids=lambda t: O.TYPE_NAME[t])
 @pytest.mark.parametrize("N,K", [(16, 64), (33, 7392), (5, 29568), (301, 29568), (64, 1280), (40, 4096), (7, 8192), (130, 14336)])   # K % 128 == 0: the bulk-copy ring (columns of 8 blocks; 29 568 = 115.5 columns, split rows), else k_gemv_generic
 def test_gemv_small_block_types_vs_oracle(cuda, lib, port, t, N, K):
     W = O.synth_blocks(t, N, K, seed=N + K)
@@ -68,11 +70,63 @@ def test_gemv_small_block_types_vs_oracle(cuda, lib, port, t, N, K):
     assert np.max(np.abs(got - want)) <= rel_tol(want)
 
 
+def gemv_traced(lib, t, W, N, K, x, shift=0, bias=None, resid=None):
+    """pb200_quantize_act + pb200_mul_mat_vec_q with W placed `shift` bytes past a 256-byte boundary; returns (y, launches, ring
+    launches)."""
+    buf = torch.zeros(W.size + 320, dtype=torch.uint8, device="cuda")
+    buf[shift: shift + W.size] = torch.from_numpy(np.ascontiguousarray(W).view(np.uint8).reshape(-1))
+    ws = act_ws(lib, K)
+    lib.check(lib.c.pb200_quantize_act(t, ptr(dev_f32(x)), K, ptr(ws), None), "q")
+    y = torch.full((N,), float("nan"), device="cuda")
+    bd = dev_f32(bias) if bias is not None else None
+    rd = dev_f32(resid) if resid is not None else None
+    trace = torch.zeros(4 * 4096, dtype=torch.int64, device="cuda")
+    lib.c.pb200_debug_set_trace.argtypes = [C.c_void_p, C.c_int]
+    lib.check(lib.c.pb200_debug_set_trace(trace.data_ptr(), 4), "trace")
+    try:
+        sync()
+        n0 = lib.c.pb200_kernel_launches()
+        lib.check(lib.c.pb200_mul_mat_vec_q(t, C.c_void_p(buf.data_ptr() + shift), N, K, ptr(ws), ptr(y), ptr(bd) if bd is not None else None,
+                                            ptr(rd) if rd is not None else None, None), "mul_mat_vec_q")
+        sync()
+        n = lib.c.pb200_kernel_launches() - n0
+    finally:
+        lib.c.pb200_debug_set_trace(None, 0)
+    ring = int((trace.view(4, 4096) != 0).any(dim=1).sum().item())
+    assert lib.c.pb200_aborted() == 0
+    return y.cpu().numpy(), n, ring
+
+
+# (N, K, W shift): the ring (whole rows, K = 8 192 and Llama-3-8B's 4 096 / 14 336), split rows at Qwen2.5-72B's ffn_down (8 192 x
+# 29 568: Q4_0 / Q8_0 rows 8- but not 16-byte aligned) and a ragged N; on k_gemv_generic, a W 8 or 2 bytes off a 16-byte boundary
+# (the ring's bulk copies need 16-byte aligned sources) and K = 1 056, whose rows are not 8-byte multiples but for Q5_1
+GEMV_ROUTES = [(1000, 8192, 0), (333, 4096, 0), (200, 14336, 0), (8192, 29568, 0), (77, 29568, 0), (300, 8192, 8), (129, 29568, 8),
+               (300, 4096, 2), (100, 1056, 0)]
+
+
+@pytest.mark.parametrize("t", O.BLK32, ids=lambda t: O.TYPE_NAME[t])
+@pytest.mark.parametrize("N,K,shift", GEMV_ROUTES)
+def test_gemv_small_block_routes(cuda, lib, port, t, N, K, shift):
+    """One launch, on the ring exactly where gemv_plan (test_gpu_gemv_shapes) gives a plan and W is 16-byte aligned; bias and residual
+    in the epilogue."""
+    from test_gpu_gemv_shapes import gemv_plan
+    rng = np.random.default_rng(N + K + t)
+    W = O.synth_blocks(t, N, K, seed=7 * t + N)
+    x = rng.standard_normal(K).astype(np.float32)
+    bias, resid = rng.standard_normal(N).astype(np.float32), rng.standard_normal(N).astype(np.float32)
+    y, n, rl = gemv_traced(lib, t, W, N, K, x, shift, bias, resid)
+    assert n == 1
+    assert rl == (shift % 16 == 0 and gemv_plan((t,), (N,), K) is not None), rl
+    want = (port.mul_mat(t, W, N, K, x)[0] + bias) + resid
+    assert np.max(np.abs(y - want)) <= rel_tol(want), np.max(np.abs(y - want))
+
+
 @pytest.mark.parametrize("t", O.QUANT_TYPES, ids=lambda t: O.TYPE_NAME[t])
 def test_gemv_weight_bit_patterns_vs_oracle(cuda, lib, port, t):
     """The weight blocks of oracle_lib.edge_blocks (quant bytes all 0x00 / 0xFF, Q8_0 q = -128, Q6_K scale -128 with q = -32, scales and
-    mins of 63, d = 0) through the GEMV families above: k-quant ring; Q8_0 / Q5_1 on the ring (K % 128 == 0) and on k_gemv_generic."""
-    for K in ([2048] if t in KQ else [2048, 1984]):
+    mins of 63, d = 0) through the GEMV families above: k-quant ring; the 32-element types on the ring where their rows allow it, and
+    with W 2 bytes off a 16-byte boundary on k_gemv_generic."""
+    for K in ([2048] if t in KQ else [2048, 1984, 4096]):
         N = 96
         W = O.edge_blocks(t, N, K, seed=K + t)
         x = np.random.default_rng(K + t).standard_normal(K).astype(np.float32)
@@ -83,6 +137,9 @@ def test_gemv_weight_bit_patterns_vs_oracle(cuda, lib, port, t):
         sync()
         got = y.cpu().numpy()
         assert np.max(np.abs(got - want)) <= rel_tol(want), (K, np.max(np.abs(got - want)), rel_tol(want))
+        if t in O.BLK32:
+            got, _, ring = gemv_traced(lib, t, W, N, K, x, shift=2)
+            assert ring == 0 and np.max(np.abs(got - want)) <= rel_tol(want), (K, ring, np.max(np.abs(got - want)))
 
 
 def test_gemv_golden_reference_quantized_weights(cuda, lib):
@@ -90,7 +147,7 @@ def test_gemv_golden_reference_quantized_weights(cuda, lib):
     from pathlib import Path
     z = np.load(Path(__file__).resolve().parent / "golden" / "kquants_golden.npz")
     x = z["x"]; K = x.size; N = z["w"].shape[0]
-    for t in O.QUANT_TYPES:
+    for t in O.GOLDEN_TYPES:
         n = O.TYPE_NAME[t]
         for tag in ("", "synth_"):
             Wd, xd, ws = dev_u8(z[f"{n}_{tag}blocks"]), dev_f32(x), act_ws(lib, K)
@@ -134,20 +191,20 @@ def test_gemv_fused_bias_resid_and_host_path(cuda, lib, port):
 
 @pytest.mark.parametrize("t", O.QUANT_TYPES + [O.F16, O.F32], ids=lambda t: O.TYPE_NAME[t])
 def test_get_rows_dequant_bit_exact(cuda, lib, port, t):
-    K, N = 1024, 9
-    if t == O.F32:
-        tab = np.random.default_rng(0).standard_normal((N, K)).astype(np.float32); want_all = tab
-    elif t == O.F16:
-        tab = np.random.default_rng(0).standard_normal((N, K)).astype(np.float16); want_all = tab.astype(np.float32)
-    else:
-        tab = O.synth_blocks(t, N, K, seed=3); want_all = port.dequantize(t, tab, K)
-    ids = np.array([8, 0, 3, 3], dtype=np.int32)
-    y = torch.zeros(len(ids) * K, device="cuda")
-    idd = torch.from_numpy(ids).cuda()
-    tabd = dev_u8(tab)
-    lib.check(lib.c.pb200_get_rows(t, ptr(tabd), K, ptr(idd), len(ids), ptr(y), None), "get_rows")
-    sync()
-    assert np.array_equal(y.cpu().numpy().reshape(len(ids), K), want_all[ids])
+    for K, N, ids, seed in ((1024, 9, [8, 0, 3, 3], 3), (4096, 64, [0, 63, 5, 5, 17, 32], 11 + t)):
+        if t == O.F32:
+            tab = np.random.default_rng(0).standard_normal((N, K)).astype(np.float32); want_all = tab
+        elif t == O.F16:
+            tab = np.random.default_rng(0).standard_normal((N, K)).astype(np.float16); want_all = tab.astype(np.float32)
+        else:
+            tab = O.synth_blocks(t, N, K, seed=seed); want_all = port.dequantize(t, tab, K)
+        ids = np.array(ids, dtype=np.int32)
+        y = torch.zeros(len(ids) * K, device="cuda")
+        idd = torch.from_numpy(ids).cuda()
+        tabd = dev_u8(tab)
+        lib.check(lib.c.pb200_get_rows(t, ptr(tabd), K, ptr(idd), len(ids), ptr(y), None), "get_rows")
+        sync()
+        assert np.array_equal(y.cpu().numpy().reshape(len(ids), K), want_all[ids]), K
 
 
 def test_rms_norm(cuda, lib, port):

@@ -24,8 +24,7 @@ from gpu_util import dev_f32, dev_u8, ptr, sync
 from tiny_model import TinyModel
 
 pytestmark = pytest.mark.gpu
-KQ = [O.Q4_K, O.Q5_K, O.Q6_K]
-BLK32 = [O.Q8_0, O.Q5_1]
+KQ, BLK32 = O.KQ, O.BLK32
 FP16_MAX = 65504.0
 
 MmqPlan = namedtuple("MmqPlan", "bn tpad ttiles rtiles ngrp total upc split ctas_per_tile short_group_split")
@@ -101,7 +100,7 @@ N_RUNGS = [1, 16, 64, 65, 127, 129]
 K_MODEL = [3584, 4096, 5120, 8192, 13824, 14336, 18944, 27648, 28672]
 KQ_CASES = ([(128, 256, 16), (256, 512, 33), (384, 1024, 128), (200, 768, 7), (128, 2048, 300)]
             + [(136, 512, T) for T in T_RUNGS] + [(N, 512, 24) for N in N_RUNGS] + [(136, K, 24) for K in K_MODEL])
-BLK32_CASES = ([(256, 448, 33), (128, 1984, 64), (200, 512, 9), (128, 29568, 24)]
+BLK32_CASES = ([(256, 448, 33), (128, 1984, 64), (200, 512, 9), (128, 29568, 24), (136, 448, 24), (136, 448, 100), (200, 4096, 33)]
                + [(136, 448, T) for T in T_RUNGS] + [(N, 448, 24) for N in N_RUNGS] + [(136, K, 24) for K in K_MODEL + [29568]])
 
 
@@ -137,8 +136,8 @@ def test_mmq_vs_oracle(cuda, lib, port, t, N, K, T):
 @pytest.mark.parametrize("t", BLK32, ids=lambda t: O.TYPE_NAME[t])
 @pytest.mark.parametrize("N,K,T", BLK32_CASES)
 def test_mmq_small_block_types_vs_oracle(cuda, lib, port, t, N, K, T):
-    """Q8_0 / Q5_1 (32-element blocks; the CPU dot quantizes the activation per 32 values): K % 64 == 0 is enough, so rows that are
-    not 16-byte aligned and a short last 256-K group are the norm here; K = 29 568 is Qwen2.5-72B's ffn_down K."""
+    """The 32-element block types (the CPU dot quantizes the activation per 32 values): K % 64 == 0 is enough, so rows that are not
+    16-byte aligned and a short last 256-K group are the norm here; K = 29 568 is Qwen2.5-72B's ffn_down K (Q5_0 in its Q4_K_M)."""
     X = rung_inputs(lib, N, K, T, 100 * t + N + K + T)
     W = O.synth_blocks(t, N, K, seed=5 * t + N)
     got = run_mmq(lib, t, W, N, K, X)
@@ -191,7 +190,7 @@ def test_mmq_bias_residual_ragged_rows_and_strided_input(cuda, lib, port):
 @pytest.mark.parametrize("t", KQ + BLK32, ids=lambda t: O.TYPE_NAME[t])
 def test_mmq_split_tiles_add_bias_and_residual_once(cuda, lib, port, t):
     """Stream-K tiles shared by several CTAs: the K group 0 segment adds bias and residual, every other segment adds only its partial
-    sum into the pre-zeroed output.  Two token tiles, a ragged row tile, >= 3 CTAs per tile; for Q8_0 / Q5_1 K = 4160 = 65 steps of
+    sum into the pre-zeroed output.  Two token tiles, a ragged row tile, >= 3 CTAs per tile; for the 32-element types K = 4160 = 65 steps of
     64, so the short last 256-K group is a partial segment.  Bias and residual together, and each alone."""
     N, T = 200, 150
     K = 8192 if t in KQ else 4160
@@ -218,7 +217,7 @@ def test_mmq_split_tiles_add_bias_and_residual_once(cuda, lib, port, t):
 
 def range_rows(t, K, rng):
     """Rows 2^s * N(0, 1) over the exponent range the CPU backend's activation quantizer represents, and the edge rows."""
-    smax = 60 if t in KQ else 20               # Q8_0 / Q5_1: the CPU's own f16 d overflows above amax = 127 * 65504 ~ 8.3e6
+    smax = 60 if t in KQ else 20               # q8_0 / q8_1: the CPU's own f16 d overflows above amax = 127 * 65504 ~ 8.3e6
     base = rng.standard_normal((1, K)).astype(np.float32)
     rows = [rng.standard_normal(K).astype(np.float32) * np.float32(2.0 ** s) for s in range(-60, smax + 1, 2)]
     unit = base[0] / np.abs(base[0]).max()
@@ -231,7 +230,7 @@ def range_rows(t, K, rng):
     if t in BLK32:
         rows.append(unit * np.float32(8.0e6))
     X = np.stack(rows)
-    if t == O.Q5_1:
+    if O.ACT_TYPE[t] == "q8_1":
         # the CPU's q8_1 also stores the block sum s = d * sum(q) as f16, which overflows once |sum of 32 values| > 65 504: rows of
         # (v, -v) pairs keep s = 0 at every magnitude, so the oracle stays finite
         X[:, 1::2] = -X[:, 0::2]
@@ -240,7 +239,7 @@ def range_rows(t, K, rng):
 
 @pytest.mark.parametrize("t", KQ + BLK32, ids=lambda t: O.TYPE_NAME[t])
 def test_mmq_activation_range(cuda, lib, port, t):
-    """Activation rows from 2^-60 to 2^60 (k-quants) / 8e6 (Q8_0, Q5_1) against the oracle under the module's row-relative bound, and
+    """Activation rows from 2^-60 to 2^60 (k-quants) / 8e6 (32-element types) against the oracle under the module's row-relative bound, and
     per row NMSE <= 4e-6: no overflow to inf at |x| >= 65 520, no precision lost to fp16 subnormals on small rows.  The rows repeat
     in changing order over more than one 128-column token tile, so each token column must find its own row scale."""
     N, K = 136, 1024

@@ -31,7 +31,7 @@ import torch
 import oracle_lib as O
 from gpu_util import act_ws, dev_f32, dev_u8, ptr, sync
 from test_gpu_kv_shift import _dev, kv_tensors
-from test_gpu_mmq import BLK32, KQ, T_RUNGS, mmq_plan, range_rows
+from test_gpu_mmq import KQ, T_RUNGS, mmq_plan, range_rows
 from tiny_model import TinyModel
 
 D = 128
@@ -47,7 +47,7 @@ def mmq_supported(t, K):
     """mmq.cu mmq_supported."""
     if is_kquant(t):
         return K % 256 == 0 and K >= 256
-    return t in BLK32 and K % 64 == 0 and K >= 256
+    return t in O.BLK32 and K % 64 == 0 and K >= 256
 
 
 def pf_tc(t, K, T):
@@ -90,8 +90,9 @@ def expected_image(port, t, X, tpad):
     return img.view(np.uint16), rs.view(np.uint32)
 
 
-K_IMAGE = {t: (256, 1024, 8192) for t in KQ} | {t: (448, 4160, 29568) for t in BLK32}
-IMAGE_CASES = [(t, K, T) for t in KQ + BLK32 for K in K_IMAGE[t] for T in T_RUNGS]
+IMAGE_BLK32 = [O.Q8_0, O.Q5_1]   # the image depends on the activation format alone: q8_0 and q8_1
+K_IMAGE = {t: (256, 1024, 8192) for t in KQ} | {t: (448, 4160, 29568) for t in IMAGE_BLK32}
+IMAGE_CASES = [(t, K, T) for t in KQ + IMAGE_BLK32 for K in K_IMAGE[t] for T in T_RUNGS]
 
 
 def image_inputs(t, K, T, seed):

@@ -16,7 +16,6 @@ import numpy as np
 import pytest
 import torch
 
-import legacy_types as L
 from tiny_model import TinyModel
 
 pytestmark = pytest.mark.gpu
@@ -30,7 +29,7 @@ MODELS = ["q4_K_M", "q4_0"]
 def tiny(name, **kw):
     """The tiny models of test_gpu_engine_slots.py, with their shape changed by kw."""
     shape = {**SHAPE, **kw}
-    return TinyModel(**shape, seed=21, branch_scale=0.3) if name == "q4_K_M" else L.q4_0_model(22, **shape)
+    return TinyModel(**shape, seed=21, branch_scale=0.3) if name == "q4_K_M" else TinyModel.q4_0(22, **shape)
 
 
 def load(tm, pkg, layers=None, with_embd=True, with_head=True):

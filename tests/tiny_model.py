@@ -29,10 +29,10 @@ class TinyModel:
         default = O.Q4_K if ftype == "q4_K_M" else O.Q5_K
         self._seed = seed * 1000
 
-        def fallback(t, K):
+        def fallback(t, K):   # rows that are not whole 256-element super-blocks (src/llama.cpp:19516-19551)
             if K % 256 == 0:
                 return t
-            return {O.Q5_K: O.Q5_1, O.Q6_K: O.Q8_0}[t]
+            return {O.Q4_K: O.Q5_0, O.Q5_K: O.Q5_1, O.Q6_K: O.Q8_0}[t]
 
         def qmat(name, t, N, K, scale=1.0):
             if types and name.split(".")[-2] in types:
@@ -69,6 +69,25 @@ class TinyModel:
                 fvec(p + "attn_q.bias", QD, 0.0, 0.05)
                 fvec(p + "attn_k.bias", EK, 0.0, 0.05)
                 fvec(p + "attn_v.bias", EK, 0.0, 0.05)
+
+    @classmethod
+    def q4_0(cls, seed, **kw):
+        """The reference's Q4_0 mixture without an imatrix (src/llama.cpp:19271-19556): every matrix and the embedding Q4_0, the head
+        Q6_K."""
+        tm = cls(arch="llama", ftype="q4_K_M", seed=seed, branch_scale=0.1, **kw)
+        for i, (name, (t, a)) in enumerate(list(tm.tensors.items())):
+            if a.dtype == np.uint8 and name != "output.weight":
+                tm.retype(name, O.Q4_0, 1000 * seed + i)
+        return tm
+
+    def retype(self, name, t, seed):
+        """Replaces a weight matrix by synthetic blocks of type t (same shape)."""
+        t0, a = self.tensors[name]
+        K = self._row_len(name)
+        N = a.size // O.row_size(t0, K)
+        # the scales __init__ gives its matrices: sqrt(n_embd) for the embedding, branch_scale 0.1 for the residual branches' outputs
+        scale = np.sqrt(K) if name == "token_embd.weight" else 0.1 if name.endswith(("attn_output.weight", "ffn_down.weight")) else 1.0
+        self.tensors[name] = (t, O.synth_blocks(t, N, K, seed, scale))
 
     # ---- oracle-side model struct (shared by port_llama_decode and gref_decode) ----
     def oracle_struct(self):
@@ -198,3 +217,16 @@ def from_golden(path):
             _, name, t = k.split("|")
             tm.tensors[name] = (int(t), np.ascontiguousarray(z[k]))
     return tm, z["tokens"], z["logits"], z["hidden"]
+
+
+def legacy_golden_models():
+    """name -> (TinyModel, tokens) of tests/golden/legacy_types_golden.npz: a Qwen2 Q4_K_M with n_ff 1 152 (not a multiple of 256: ffn_down
+    Q4_K -> Q5_0 in layer 0, Q6_K -> Q8_0 in the use_more_bits layer 1) and a llama Q4_0.  The Qwen2's two ffn_down are the retyped
+    blocks the reference's logits were recorded on."""
+    qwen = TinyModel(n_layer=2, n_embd=512, n_head=4, n_head_kv=2, n_ff=1152, n_vocab=320, n_ctx=64, arch="qwen2", ftype="q4_K_M", seed=41,
+                     branch_scale=0.1, types={"ffn_down": O.Q5_K})
+    qwen.retype("blk.0.ffn_down.weight", O.Q5_0, 4101)
+    qwen.retype("blk.1.ffn_down.weight", O.Q8_0, 4102)
+    llama = TinyModel.q4_0(43, n_layer=2, n_embd=512, n_head=4, n_head_kv=2, n_ff=1024, n_vocab=320, n_ctx=64)
+    toks = [(i * 7919 + 13) % 320 for i in range(40)]
+    return {"qwen2_q4_K_M": (qwen, toks), "llama_q4_0": (llama, toks)}
