@@ -97,6 +97,9 @@ PB200_API int pb200_rope_f16(const void * x, void * y, int64_t n_rows, int n_hea
                              float freq_base, float freq_scale, float ext_factor, float attn_factor, float beta_fast, float beta_slow,
                              int n_ctx_orig, const float * freq_factors, void * stream);
 PB200_API int pb200_soft_max(const float * x, const float * mask, float * y, int64_t ncols, int64_t nrows, int64_t mask_rows, float scale, void * stream);
+/* the shared memory pb200_soft_max launches rows of ncols with on the current device: *dyn_bytes = the row staged in dynamic shared
+ * memory, 0 when it does not fit beside the kernel's *static_bytes and the softmax runs in place in y (global memory) */
+PB200_API int pb200_soft_max_smem(int64_t ncols, int64_t * dyn_bytes, int64_t * static_bytes);
 PB200_API int pb200_silu_mul(const float * gate, const float * up, float * y, int64_t n, void * stream);
 /* element-wise glue of the graph (binbcast.cu / unary.cu / cpy.cu): y = a (+|*) b[i % nb]  (op 0 add, 1 mul); y = silu(x);
  * 4-D strided copy f32 -> f32|f16 (byte strides; dst logical order) — CPY / CONT / DUP incl. the transposed V-cache store */

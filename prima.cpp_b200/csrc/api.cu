@@ -150,6 +150,16 @@ int pb200_soft_max(const float * x, const float * mask, float * y, int64_t ncols
     return launch_soft_max(x, mask, y, (int) ncols, nrows, mask_rows > 0 ? mask_rows : 1, scale, (cudaStream_t) stream);
 }
 
+int pb200_soft_max_smem(int64_t ncols, int64_t * dyn_bytes, int64_t * static_bytes) {
+    if (ncols <= 0 || ncols > INT32_MAX || !dyn_bytes || !static_bytes) return PB200_EINVAL;
+    size_t st = 0;
+    const size_t dyn = soft_max_smem((int) ncols, &st);
+    if (st == 0) return PB200_ENOTSUP;   // the device or the kernel's attributes could not be queried
+    *dyn_bytes = (int64_t) dyn;
+    *static_bytes = (int64_t) st;
+    return 0;
+}
+
 int pb200_silu_mul(const float * gate, const float * up, float * y, int64_t n, void * stream) {
     if (!gate || !up || !y || n <= 0) return PB200_EINVAL;
     g_launches++;
@@ -195,7 +205,7 @@ int pb200_mul_mat_q(int type, const void * W, int64_t n, int64_t k, const float 
 int pb200_aborted(void) { return check_clear_abort(); }
 
 int pb200_get_rows(int type, const void * table, int64_t k, const int32_t * ids, int64_t n_ids, float * y, void * stream) {
-    if (!table || !ids || !y || k <= 0 || n_ids <= 0) return PB200_EINVAL;
+    if (!table || !ids || !y || k <= 0 || n_ids <= 0 || k > INT32_MAX || n_ids > INT32_MAX) return PB200_EINVAL;
     if (!(is_quant_type(type) || type == T_F32 || type == T_F16)) return PB200_ENOTSUP;
     g_launches++;
     return launch_get_rows(table, type, (int) k, ids, (int) n_ids, y, (cudaStream_t) stream, false);

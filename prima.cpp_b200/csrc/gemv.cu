@@ -562,6 +562,7 @@ size_t dyn_smem_limit(FuncAttrCache & c, const void * fn) {
             return 0;
         }
         c.limit[dev] = (size_t) optin > fa.sharedSizeBytes ? (size_t) optin - fa.sharedSizeBytes : 0;
+        c.stat[dev] = fa.sharedSizeBytes;
     }
     return c.limit[dev];
 }
@@ -570,7 +571,7 @@ cudaError_t ensure_dyn_smem(FuncAttrCache & c, const void * fn, size_t bytes, bo
     if (bytes <= c.bytes[dev]) return cudaSuccess;
     const size_t limit = dyn_smem_limit(c, fn);
     if (limit && bytes > limit) return cudaErrorNotSupported;   // refused here: a failed cudaFuncSetAttribute would linger as the last error
-    if (bytes > 48 * 1024 || max_carveout) {
+    if (bytes + c.stat[dev] > 48 * 1024 || max_carveout) {   // the 48 KB default covers static and dynamic shared memory together
         cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(bytes, 48 * 1024));
         if (e != cudaSuccess) return e;
         if (max_carveout) {

@@ -74,13 +74,14 @@ struct LaunchCfg {
 
 // ---- per-device host state (gemv.cu): cudaFuncSetAttribute / SM count are per device, one process may drive several ----
 constexpr int PB_MAX_DEV = 64;
-struct FuncAttrCache { size_t bytes[PB_MAX_DEV] = {0}; size_t limit[PB_MAX_DEV] = {0}; };
+struct FuncAttrCache { size_t bytes[PB_MAX_DEV] = {0}; size_t limit[PB_MAX_DEV] = {0}; size_t stat[PB_MAX_DEV] = {0}; };   // stat: fn's static shared memory
 int cur_device();
 int sm_count();                       // of the current device
 // the most dynamic shared memory a launch of fn may request on the current device: the opt-in limit per block minus fn's static
 // shared memory (0 if the device cannot be queried)
 size_t dyn_smem_limit(FuncAttrCache & c, const void * fn);
-// raise a kernel's dynamic shared-memory limit on the current device if needed (max_carveout: also prefer the full 228 KB carve-out);
+// raise a kernel's dynamic shared-memory limit on the current device if needed, i.e. when its static plus `bytes` of dynamic shared memory
+// exceed the default 48 KB per block (max_carveout: also prefer the full 228 KB carve-out);
 // cudaErrorNotSupported, with nothing changed, when bytes exceed dyn_smem_limit
 cudaError_t ensure_dyn_smem(FuncAttrCache & c, const void * fn, size_t bytes, bool max_carveout);
 // wait watchdogs (common.cuh): host-mapped flag every kernel with a bounded wait gets a pointer to; check_clear_abort() returns 1
@@ -168,6 +169,9 @@ int launch_flash_attn_ext(const float * q, const void * k, const void * v, const
                           float softcap, cudaStream_t stream);
 
 // soft_max_ext for the plugin: y[r][:] = softmax(x[r][:]*scale + mask[r % mask_rows][:])  (softmax.cu:14-116)
+// soft_max_smem: the dynamic shared memory launch_soft_max gives rows of ncols on the current device (the staged row, or 0 when it does
+// not fit and the softmax runs in place in y); static_bytes (optional): k_soft_max's static shared memory
+size_t soft_max_smem(int ncols, size_t * static_bytes);
 int launch_soft_max(const float * x, const float * mask, float * y, int ncols, int64_t nrows, int64_t rows_per_mask_cycle, float scale,
                     cudaStream_t stream);
 

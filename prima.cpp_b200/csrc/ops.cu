@@ -955,14 +955,14 @@ __device__ float dequant_elem(int type, const uint8_t * row, int e) {
     return 0.f;
 }
 
+// Ids on grid.y, which is capped at 65 535: a CTA row takes ids blockIdx.y, blockIdx.y + gridDim.y, ...
 __global__ void __launch_bounds__(256) k_get_rows(const uint8_t * __restrict__ table, int type, int K, int64_t row_bytes_,
-                                                  const int32_t * __restrict__ ids, float * __restrict__ y) {
+                                                  const int32_t * __restrict__ ids, int n_ids, float * __restrict__ y) {
     pdl_trigger();   // dependents may launch now; they still wait for this grid's completion in their own pdl_wait()
     pdl_wait();
-    const int64_t id = ids[blockIdx.y];
-    const uint8_t * row = table + id * row_bytes_;
     const int e = blockIdx.x * 256 + threadIdx.x;
-    if (e < K) y[(int64_t) blockIdx.y * K + e] = dequant_elem(type, row, e);
+    if (e >= K) return;
+    for (int64_t i = blockIdx.y; i < n_ids; i += gridDim.y) y[i * K + e] = dequant_elem(type, table + (int64_t) ids[i] * row_bytes_, e);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1302,22 +1302,27 @@ int launch_flash_attn_ext(const float * q, const void * k, const void * v, const
     return (int) cudaGetLastError();
 }
 
+static FuncAttrCache sm_attr;   // k_soft_max
+size_t soft_max_smem(int ncols, size_t * static_bytes) {
+    const size_t bytes = (size_t) ncols * sizeof(float);
+    const size_t limit = dyn_smem_limit(sm_attr, (const void *) k_soft_max);
+    if (static_bytes) *static_bytes = sm_attr.stat[cur_device()];
+    return limit && bytes > limit ? 0 : bytes;   // 0: the row does not fit, softmax in place in y
+}
 int launch_soft_max(const float * x, const float * mask, float * y, int ncols, int64_t nrows, int64_t rows_per_mask_cycle, float scale,
                     cudaStream_t stream) {
-    size_t smem = (size_t) ncols * sizeof(float);
-    static FuncAttrCache sm_attr;
-    {
+    const size_t smem = soft_max_smem(ncols, nullptr);
+    if (smem) {
         cudaError_t e = ensure_dyn_smem(sm_attr, (const void *) k_soft_max, smem, false);
-        if (e == cudaErrorNotSupported) smem = 0;   // the row does not fit: softmax in place in y
-        else if (e != cudaSuccess) return (int) e;
+        if (e != cudaSuccess) return (int) e;
     }
     k_soft_max<<<(unsigned) nrows, 256, smem, stream>>>(x, mask, y, ncols, rows_per_mask_cycle, scale, smem != 0);
     return (int) cudaGetLastError();
 }
 
 int launch_get_rows(const void * table, int type, int K, const int32_t * ids, int n_ids, float * y, cudaStream_t stream, bool pdl) {
-    LaunchCfg lc(dim3((K + 255) / 256, n_ids), dim3(256), 0, stream, pdl);
-    return (int) cudaLaunchKernelEx(&lc.cfg, k_get_rows, (const uint8_t *) table, type, K, row_bytes(type, K), ids, y);
+    LaunchCfg lc(dim3((K + 255) / 256, std::min(n_ids, 65535)), dim3(256), 0, stream, pdl);
+    return (int) cudaLaunchKernelEx(&lc.cfg, k_get_rows, (const uint8_t *) table, type, K, row_bytes(type, K), ids, n_ids, y);
 }
 
 int launch_binary(int op, const float * a, const float * b, float * y, int64_t n, int64_t nb, cudaStream_t stream) {

@@ -302,7 +302,8 @@ static bool b200_supports_op(ggml_backend_dev_t, const ggml_tensor * op) {
         }
         case GGML_OP_GET_ROWS:
             return (a->type == GGML_TYPE_F32 || a->type == GGML_TYPE_F16 || type_is_quant(a->type)) && b->type == GGML_TYPE_I32 && op->type == GGML_TYPE_F32 &&
-                   ggml_is_contiguous(a) && ggml_is_contiguous(b) && ggml_is_contiguous(op) && a->ne[2] == 1 && a->ne[3] == 1 && b->ne[2] == 1 && b->ne[3] == 1;
+                   ggml_is_contiguous(a) && ggml_is_contiguous(b) && ggml_is_contiguous(op) && a->ne[2] == 1 && a->ne[3] == 1 && b->ne[2] == 1 && b->ne[3] == 1 &&
+                   a->ne[0] <= INT32_MAX && ggml_nelements(b) <= INT32_MAX;   // pb200_get_rows takes int32 row lengths and id counts
         default:
             return false;
     }

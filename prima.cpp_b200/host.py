@@ -115,6 +115,7 @@ class Lib:
         c.pb200_rms_norm.argtypes = [vp, vp, i64, i64, f32, vp]
         c.pb200_rope.argtypes = [vp, vp, i64, C.c_int, C.c_int, C.c_int, C.c_int, vp, f32, f32, f32, f32, f32, f32, C.c_int, vp, vp]
         c.pb200_soft_max.argtypes = [vp, vp, vp, i64, i64, i64, f32, vp]
+        c.pb200_soft_max_smem.argtypes = [i64, C.POINTER(i64), C.POINTER(i64)]
         c.pb200_silu_mul.argtypes = [vp, vp, vp, i64, vp]
         c.pb200_get_rows.argtypes = [C.c_int, vp, i64, vp, i64, vp, vp]
         c.pb200_mul_mat_q_workspace_bytes.restype = C.c_size_t
