@@ -9,12 +9,18 @@ Script mode drives both backends through a list of steps the way llama_decode wo
 graph of n tokens (a decode step is n = 1), "clear" empties both KV caches.  Every step computes all its rows' logits.
 
     python tests/ggml_graph_parity.py <llama|qwen2> --script STEPS_JSON [--dims n_layer,n_embd,n_head,n_head_kv,n_ff,n_vocab,n_ctx]
-                                      [--reserve N_TOKENS_MAX] [--dump FILE.npz]
+                                      [--reserve N_TOKENS_MAX] [--dump FILE.npz] [--seed S] [--ftype q4_K_M|q5_K_M]
+                                      [--no-freq-factors] [--engine]
 
 STEPS_JSON is a JSON list of {"n": T, "pos": p} and "clear".  The compute buffers are reserved for the largest T of the script
-unless --reserve says otherwise.  One JSON line per run with one entry per step; --dump also writes every step's logits of both
-backends and the layer-0 K / V cache contents after it.
+unless --reserve says otherwise.  One JSON line per run with one entry per step; --dump also writes every step's logits and last
+hidden states of both backends and the layer-0 K / V cache contents after it (the cells up to the script's last position).  The model is TinyModel(dims, seed 31 unless --seed,
+q4_K_M for llama / q5_K_M for qwen2 unless --ftype, rope freq factors for llama unless --no-freq-factors, branch_scale 0.1): with the
+dims, seed and ftype of tests/golden/make_reference_golden.py's engine_70b_model / engine_q72b_model it is that model.  --engine also
+loads it into the engine (pb200_decode) and decodes every step there (decode steps only); the dump then holds the engine's logits,
+hidden state and layer-0 K / V cells as well ("eng").
 """
+import argparse
 import ctypes as C
 import json
 import sys
@@ -29,20 +35,32 @@ import host_graph as HG            # noqa: E402
 
 arch = sys.argv[1]
 script_mode = sys.argv[2] == "--script"
-opts = dict(zip(sys.argv[2::2], sys.argv[3::2])) if script_mode else {}
+opts = {}
 if script_mode:
-    steps = json.loads(opts["--script"])
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--script", required=True)
+    ap.add_argument("--dims")
+    ap.add_argument("--reserve", type=int)
+    ap.add_argument("--dump")
+    ap.add_argument("--seed", type=int, default=31)
+    ap.add_argument("--ftype", choices=("q4_K_M", "q5_K_M"))
+    ap.add_argument("--no-freq-factors", action="store_true")
+    ap.add_argument("--engine", action="store_true")
+    opts = ap.parse_args(sys.argv[2:])
+    steps = json.loads(opts.script)
     n_tok = max([st["n"] for st in steps if st != "clear"])
-    dims = [int(x) for x in opts["--dims"].split(",")] if "--dims" in opts else None
+    dims = [int(x) for x in opts.dims.split(",")] if opts.dims else None
 else:
     n_tok = int(sys.argv[2])
     dims = [int(x) for x in sys.argv[3:10]] if len(sys.argv) >= 10 else None
-reserve = int(opts.get("--reserve", n_tok)) if script_mode else 1   # the token-by-token run keeps the one-token reservation
+reserve = (opts.reserve or n_tok) if script_mode else 1   # the token-by-token run keeps the one-token reservation
 if arch in ("llama", "qwen2"):
     dims = dims or [3, 1024, 8, 2, 2816 if arch == "llama" else 3072, 384, 96]
     n_layer, n_embd, n_head, n_head_kv, n_ff, n_vocab, n_ctx = dims
+    ftype = (opts.ftype if script_mode else None) or ("q4_K_M" if arch == "llama" else "q5_K_M")
+    freq_factors = arch == "llama" and not (script_mode and opts.no_freq_factors)
     tm = TinyModel(n_layer=n_layer, n_embd=n_embd, n_head=n_head, n_head_kv=n_head_kv, n_ff=n_ff, n_vocab=n_vocab, n_ctx=n_ctx, arch=arch,
-                   ftype="q4_K_M" if arch == "llama" else "q5_K_M", freq_factors=(arch == "llama"), seed=31, branch_scale=0.1)
+                   ftype=ftype, freq_factors=freq_factors, seed=opts.seed if script_mode else 31, branch_scale=0.1)
 else:
     tm = legacy_golden_models()[arch][0]
     n_layer, n_embd, n_head, n_head_kv, n_ff, n_vocab, n_ctx = (tm.hp[k] for k in ("n_layer", "n_embd", "n_head", "n_head_kv", "n_ff",
@@ -66,13 +84,31 @@ def cache(be, il, nm):
     return models[be].get_tensor(f"blk.{il}.{nm}", EK * n_ctx * 2).view(np.float16).astype(np.float32)
 
 
+def engine_cells(eng, v):
+    """Layer-0 cells of sequence 0 in the engine's f16 cache ([n_seq][layer][n_ctx][n_head_kv * 128], pb200_kv_device), row = cell."""
+    import torch
+
+    class Dev:
+        __cuda_array_interface__ = {"shape": (n_ctx, EK), "typestr": "<f2", "data": (eng.kv_ptr(v), False), "version": 2}
+    torch.cuda.synchronize()
+    return torch.as_tensor(Dev(), device="cuda").cpu().numpy().astype(np.float32)
+
+
 if script_mode:
     toks = [(i * 7919 + 13) % n_vocab for i in range(n_ctx)]   # the token at a position does not depend on how the prompt is cut
     out_steps, dump = [], {}
+    n_rows = max(st["pos"] + st["n"] for st in steps if st != "clear")   # the cells the script writes: what --dump keeps of the caches
+    eng = None
+    if opts.engine:
+        import pkgload
+        assert all(st == "clear" or st["n"] == 1 for st in steps), "--engine runs decode steps only"
+        eng = tm.load_engine(pkgload.load())
     for si, st in enumerate(steps):
         if st == "clear":
             for m in models.values():
                 m.kv_clear()
+            if eng is not None:
+                eng.kv_clear()
             out_steps.append({"clear": True})
             continue
         T, pos = st["n"], st["pos"]
@@ -96,14 +132,26 @@ if script_mode:
                           "unsupported_nodes": int(models["B200_0"].unsupported_nodes),
                           "buffer_base": int(models["B200_0"].compute_buffer_base),
                           "kv_max_abs": max(kv_err), "kv0_max_abs": kv_err[0]})
-        if "--dump" in opts:
+        if eng is not None:
+            e_lg = np.zeros(n_vocab, np.float32)
+            eng.decode(int(toks[pos]), pos, e_lg)
+            out_steps[-1]["eng_max_abs"] = float(np.max(np.abs(e_lg - b[0])))
+        if opts.dump:
             for be in models:
                 tag = "cpu" if be == "CPU" else "b200"
                 dump[f"logits_{tag}_{si}"] = lg[be]
-                dump[f"k0_{tag}_{si}"] = kv[(be, 0, "cache_k")].reshape(n_ctx, EK)    # row = cell
-                dump[f"v0_{tag}_{si}"] = kv[(be, 0, "cache_v")].reshape(EK, n_ctx).T  # transposed cache: row = cell
-    if "--dump" in opts:
-        np.savez(opts["--dump"], **dump)
+                dump[f"hidden_{tag}_{si}"] = hd[be]
+                dump[f"k0_{tag}_{si}"] = kv[(be, 0, "cache_k")].reshape(n_ctx, EK)[:n_rows]    # row = cell
+                dump[f"v0_{tag}_{si}"] = kv[(be, 0, "cache_v")].reshape(EK, n_ctx).T[:n_rows]  # transposed cache: row = cell
+            if eng is not None:
+                dump[f"logits_eng_{si}"] = e_lg[None]
+                dump[f"hidden_eng_{si}"] = eng.hidden().reshape(1, n_embd)
+                dump[f"k0_eng_{si}"] = engine_cells(eng, False)[:n_rows]
+                dump[f"v0_eng_{si}"] = engine_cells(eng, True)[:n_rows]
+    if eng is not None:
+        eng.close()
+    if opts.dump:
+        np.savez(opts.dump, **dump)
     print(json.dumps({"arch": arch, "n_layer": n_layer, "n_tokens_max": reserve, "steps": out_steps}))
     sys.exit(0)
 

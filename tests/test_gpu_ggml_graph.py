@@ -10,6 +10,7 @@ from pathlib import Path
 import pytest
 
 import oracle_lib as O
+from ggml_parity_util import Layer0, check_logits, decodes, prompt, prompt_steps, run_script, sessions
 
 pytestmark = pytest.mark.gpu
 ROOT = Path(__file__).resolve().parent.parent
@@ -81,115 +82,6 @@ def test_fused_equals_unfused_node_by_node(cuda):
 # permuted KQV.  The fused decode plan then continues on the K / V rows that path wrote.  The host stand-in reserves its compute
 # buffer once, as llama.cpp does, so a topology seen before comes back at the same addresses and the plugin replays its CUDA graph.
 
-def run_script(arch, steps, dims=None, reserve=None, env=None, dump=None):
-    import os
-    if not (ROOT / "host" / "_ggml" / "libllama_graph_host.so").exists() or not (ROOT / "prima.cpp_b200" / "libggml-b200.so").exists():
-        pytest.skip("host/_ggml or the plugin is not built (build() builds them only where the reference source tree is readable)")
-    cmd = [sys.executable, str(ROOT / "tests" / "ggml_graph_parity.py"), arch, "--script", json.dumps(steps)]
-    cmd += ["--dims", ",".join(str(d) for d in dims)] if dims else []
-    cmd += ["--reserve", str(reserve)] if reserve else []
-    cmd += ["--dump", str(dump)] if dump else []
-    p = subprocess.run(cmd, capture_output=True, text=True, timeout=1800, env=dict(os.environ, **(env or {})))
-    assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-4000:]
-    return json.loads(p.stdout.strip().splitlines()[-1])
-
-
-def prompt(T, pos):
-    return {"n": T, "pos": pos}
-
-
-def decodes(pos, k):
-    return [{"n": 1, "pos": pos + i} for i in range(k)]
-
-
-def check_logits(rows):
-    """The multi-token bar of check_decode_parity / test_whole_graph_matches_cpu_backend_and_is_fused over a session's prompt rows
-    and decode steps: once an activation code flips upstream (q = round(x*127/amax) of a 1-ulp fp32 difference), the deviation is
-    the noise the reference's own SIMD builds show against each other, so NMSE < 2e-3, max-abs < 0.25, >= 90 % same argmax."""
-    sq_err = sum(r["sq_err"] for r in rows)
-    sq_ref = sum(r["sq_ref"] for r in rows)
-    agree = [a for r in rows for a in r["argmax_agree_per_row"]]
-    worst = max(max(r["max_abs_per_row"]) for r in rows)
-    assert sq_err / sq_ref < 2e-3 and worst < 0.25 and sum(agree) >= 0.9 * len(agree), (sq_err / sq_ref, worst, sum(agree), len(agree))
-    for r in rows:
-        assert r["kv_max_abs"] < 0.25, r   # f16 cache rows of magnitude ~20: a flipped activation code upstream moves them by a few 1e-2
-        if r["n"] > 1 and r["n"] < 8 and r["pos"] == 0:
-            # T < 8 runs one integer-dot GEMV per column, like the CPU's vec_dot: the first row depends on token 0 alone and agrees
-            # to fp32 summation order
-            assert r["max_abs_per_row"][0] < 1e-4, r["max_abs_per_row"]
-
-
-class Layer0:
-    """Bars for the layer-0 K / V cache rows a prompt writes.  Their input is rms_norm(token_embd[tok]) * attn_norm on both backends,
-    so no activation code can have flipped upstream; what is left is the mat-mul's own arithmetic, RoPE and the f16 store."""
-
-    def __init__(self, arch, dims=None):
-        import numpy as np
-        import oracle_lib as O
-        from tiny_model import TinyModel
-        n_layer, n_embd, n_head, n_head_kv, n_ff, n_vocab, n_ctx = dims or [3, 1024, 8, 2, 2816 if arch == "llama" else 3072, 384, 96]
-        tm = TinyModel(n_layer=n_layer, n_embd=n_embd, n_head=n_head, n_head_kv=n_head_kv, n_ff=n_ff, n_vocab=n_vocab, n_ctx=n_ctx, arch=arch,
-                       ftype="q4_K_M" if arch == "llama" else "q5_K_M", freq_factors=(arch == "llama"), seed=31, branch_scale=0.1)
-        port = O.Port()
-        deq = lambda name, k: port.dequantize(tm.tensors[name][0], tm.tensors[name][1], k).astype(np.float64)
-        emb = deq("token_embd.weight", n_embd)
-        toks = [(i * 7919 + 13) % n_vocab for i in range(n_ctx)]   # the driver's token at each position
-        x = emb[toks]
-        x = x / np.sqrt(np.mean(x * x, axis=1, keepdims=True) + tm.hp["rms_eps"]) * tm.tensors["blk.0.attn_norm.weight"][1].astype(np.float64)
-        self.x = np.abs(x)
-        self.d_x = self.x.max(axis=1, keepdims=True) / 127          # largest q8 step of each row's activation quantization
-        self.neox = tm.hp["rope_mode"] == 2
-        self.w = {}
-        for nm, wn in (("k", "blk.0.attn_k.weight"), ("v", "blk.0.attn_v.weight")):
-            W = np.abs(deq(wn, n_embd))
-            sub = np.repeat(W.reshape(W.shape[0], -1, 32).max(axis=2), 32, axis=1)
-            self.w[nm] = (W, W + sub)
-
-    def pair(self, b):
-        """Error bound after RoPE: a rotation mixes each pair (a, b) of a head, |R e| <= |e_a| + |e_b| per component."""
-        import numpy as np
-        h = b.reshape(b.shape[0], -1, 128)
-        if self.neox:
-            s = h[..., :64] + h[..., 64:]
-            out = np.concatenate([s, s], axis=-1)
-        else:
-            s = h[..., 0::2] + h[..., 1::2]
-            out = np.repeat(s, 2, axis=-1)
-        return out.reshape(b.shape)
-
-    def check(self, dump, si, pos, T):
-        """T < 8 (integer-dot GEMVs like the CPU's): every element within one f16 ulp of the CPU's plus the fp32 summation-order
-        floor 2^-22 * sum|x_j w_j|, except in at most one row, where a rare q8 code flip of the activation (~3e-4 relative, see the
-        comment above test_engine_vs_port_longer_decode) is allowed up to two flips' worth, 2 * d_x * max_j |w_j|.
-        T >= 8 (tensor cores): the element-wise fp16-roundings bound of tests/test_gpu_mmq.py, 2^-9 * |x| @ (|W| + sub)^T, plus the
-        same floor and the f16 store's ulp."""
-        import numpy as np
-        rows = slice(pos, pos + T)
-        x, d_x = self.x[rows], self.d_x[rows]
-        for nm in ("k", "v"):
-            a, b = dump[f"{nm}0_cpu_{si}"][rows].astype(np.float64), dump[f"{nm}0_b200_{si}"][rows].astype(np.float64)
-            W, Wsub = self.w[nm]
-            floor = 2.0 ** -22 * (x @ W.T) + 1e-7
-            bound = 2.0 ** -9 * (x @ Wsub.T) + 1e-6 if T >= 8 else floor
-            kick = 2 * d_x * W.max(axis=1)[None, :]
-            if nm == "k":   # the f32 RoPE of the two backends differs by a few fp32 ulps of the rotated pair as well
-                bound, kick = self.pair(bound) + 2.0 ** -17 * self.pair(np.abs(a)), self.pair(kick)
-            ulp = np.spacing(np.maximum(np.abs(a), np.abs(b)).astype(np.float16)).astype(np.float64)
-            err = np.abs(a - b)
-            over = err > ulp + bound
-            worst = float((err / (ulp + bound)).max())
-            if T >= 8:
-                assert not over.any(), f"{nm} rows {pos}..{pos + T - 1}: {int(over.sum())} elements exceed the fp16-roundings bound (worst ratio {worst:.2f})"
-            else:
-                rows_over = int(over.any(axis=1).sum())
-                assert rows_over <= 1, f"{nm} rows {pos}..{pos + T - 1}: {rows_over} rows beyond 1 f16 ulp + fp32 order (worst ratio {worst:.2f})"
-                assert (err <= ulp + bound + kick).all(), f"{nm}: deviation larger than two q8 code flips (worst {float((err / (ulp + bound + kick)).max()):.2f})"
-
-
-def prompt_steps(r):
-    return [(si, st) for si, st in enumerate(r["steps"]) if "clear" not in st and st["n"] > 1]
-
-
 @pytest.mark.parametrize("arch", ["llama", "qwen2"])
 def test_prompt_batches_match_cpu_backend(cuda, arch, tmp_path):
     """Prompts of T in {2, 7, 8, 9, 33, 64} tokens at position 0, each followed by 8 decode steps, through graph_compute vs the CPU
@@ -200,20 +92,16 @@ def test_prompt_batches_match_cpu_backend(cuda, arch, tmp_path):
         steps += ["clear", prompt(T, 0)] + decodes(T, 8)
     r = run_script(arch, steps, reserve=64, dump=tmp_path / "d.npz")
     dump, l0, L = np.load(tmp_path / "d.npz"), Layer0(arch), r["n_layer"]
-    sessions = [[]]
-    for st in r["steps"]:
-        if "clear" in st:
-            sessions.append([])
-            continue
-        sessions[-1].append(st)
-        assert st["unsupported_nodes"] == 0, st
-        if st["n"] > 1:
-            assert st["fused_steps"] == 0, st                    # the planner declines multi-token motifs
-        else:
-            assert st["fused_steps"] >= 5 * L, st                # and the decode after it is fused again
+    for s in sessions(r):
+        for st in s:
+            assert st["unsupported_nodes"] == 0, st
+            if st["n"] > 1:
+                assert st["fused_steps"] == 0, st                    # the planner declines multi-token motifs
+            else:
+                assert st["fused_steps"] >= 5 * L, st                # and the decode after it is fused again
     for si, st in prompt_steps(r):
         l0.check(dump, si, st["pos"], st["n"])
-    for s in sessions[1:]:
+    for s in sessions(r):
         check_logits(s)
 
 
@@ -287,16 +175,7 @@ def test_replay_across_workspace_growth(cuda, tmp_path):
     assert [s["graph_replays"] for s in steps if s["n"] == 40] == [0], rep
     dec = [s["graph_replays"] for s in steps if s["n"] == 1]
     assert dec == ([0, 0] + [1] * 10) * 2, rep                       # per bucket: direct, capture, then replays
-    sessions, cur = [], []
-    for s in r["steps"]:
-        if "clear" in s:
-            if cur:
-                sessions.append(cur)
-            cur = []
-        else:
-            cur.append(s)
-    sessions.append(cur)
-    for s in sessions:
+    for s in sessions(r):
         check_logits(s)
     g = np.load(tmp_path / "g.npz")
     l0 = Layer0("llama")
@@ -321,15 +200,6 @@ def test_plan_cache_eviction(cuda):
         steps += ["clear", prompt(T, 0)]
     steps += ["clear", prompt(2, 0)] + decodes(2, 4)
     r = run_script("qwen2", steps, reserve=18)
-    sessions, cur = [], []
-    for s in r["steps"]:
-        if "clear" in s:
-            if cur:
-                sessions.append(cur)
-            cur = []
-        else:
-            cur.append(s)
-    sessions.append(cur)
-    assert len(sessions) == 18
-    for s in sessions:
+    assert len(sessions(r)) == 18
+    for s in sessions(r):
         check_logits(s)
